@@ -23,9 +23,16 @@ e2e         : ONE full window through the public call SimplePrior.sample(...) wi
 roofline    : the persistent decode kernel: algorithmic bytes per launch (fp16 Conv1D weights + fp32 x_out +
               LN / bias + KV rows read + KV rows written, SURVEY.md section 8d) / launch duration measured with
               CUDA events around single launches at 8 octile positions x 48 launches, vs MEASURED_PEAKS.json
+              (else the H100 SXM data sheet: 3.35 TB/s HBM3, 989 TFLOP/s dense BF16)
 cpu_baseline: oracle (numpy fp32 restatement of the reference) on the host cores, bounded sample; its fp16
               twin gives `parity_rel_err` against the GPU logits of the same positions
 secondary   : VQ-VAE decode clips/s (BASELINE configs[4]) measured in the same run
+
+--dump-outputs DIR writes what the last timed step returned, as DIR/<name>.npy (float32 / float64): for a prior
+workload the codes that step sampled (tokens.npy, [n_samples, positions]) and the logits of its last position
+(logits.npy, [n_samples, bins]); for vqvae_decode a fixed seeded sample of 2^20 values of the decoded audio of each
+start level (audio_level<l>.npy).  Weights, labels and sampling seeds are fixed, so two builds run with the same
+arguments can be compared output for output.
 """
 import argparse
 import contextlib
@@ -40,6 +47,8 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 N_SLICES = 8
+HBM_GBS_H100, BF16_TFLOPS_H100 = 3350.0, 989.0      # H100 SXM data sheet (700 W card), when no measured peaks exist
+DUMP_SAMPLE = 1 << 20                                # values kept per dumped audio level
 
 WORKLOADS = {
     # BASELINE configs[1]
@@ -69,6 +78,8 @@ def parse():
     ap.add_argument("--small", action="store_true", help="tiny debug configuration (not a valid bench number)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-secondary", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy")
     a = ap.parse_args()
     if a.workload == "prior":
         a.workload = "1b_lyrics"
@@ -243,19 +254,13 @@ class ClockSampler:
         return dict(sm_mhz=sm[len(sm) // 2], sm_max_mhz=mx, reasons=sorted(reasons), samples=len(sm))
 
 
-def ncu_dram_bytes(path):
-    """dram__bytes_read.sum + dram__bytes_write.sum of a committed ncu capture of the decode kernel (bytes per
-    launch), or None"""
-    try:
-        tot = 0.0
-        scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-        for line in open(path):
-            f = line.split()
-            if len(f) >= 4 and f[0] in ("dram__bytes_read.sum", "dram__bytes_write.sum") and f[1] == "=":
-                tot += float(f[2]) * scale.get(f[3], 1.0)
-        return tot or None
-    except Exception:
-        return None
+def dump_outputs(d, arrays):
+    """arrays: name -> numpy array (float32 / float64), written as d/<name>.npy"""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        np.save(os.path.join(d, name + ".npy"), a)
 
 
 def load_peaks():
@@ -443,10 +448,19 @@ def measure_vqvae(args, rank, world, local, steps, warmup, small=False):
     c0 = _lib.CALLS
     e0.record()
     for _ in range(steps):
-        step(zs_dev)
+        outs = step(zs_dev)
     e1.record()
     torch.cuda.synchronize()
     launches = _lib.CALLS - c0
+    dumped = None
+    if args.dump_outputs and args.workload == "vqvae_decode" and rank == 0 and steps > 0:
+        gs = torch.Generator().manual_seed(0)
+        dumped = {}
+        for l, o in enumerate(outs):
+            flat = o.reshape(-1)
+            idx = torch.randperm(flat.numel(), generator=gs)[:DUMP_SAMPLE].sort().values
+            dumped[f"audio_level{l}"] = flat[idx.to(flat.device)].float().cpu().numpy()
+    outs = None
     ms = torch.tensor([e0.elapsed_time(e1)], device="cuda")
     if world > 1:
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
@@ -465,10 +479,11 @@ def measure_vqvae(args, rank, world, local, steps, warmup, small=False):
     flops_clip = 373e9 * (T / 1048576)
     bytes_plan = 7.3e9 * (T / 1048576)
     peaks = load_peaks()
-    hbm = float(peaks.get("hbm_gbs", 6650.0))
-    tf = float(peaks.get("bf16_tflops", 1690.0))
+    hbm = float(peaks.get("hbm_gbs", HBM_GBS_H100))
+    tf = float(peaks.get("bf16_tflops", BF16_TFLOPS_H100))
     t_clip = float(ms) * 1e-3 / (n * steps)
-    traffic = ncu_dram_bytes(os.path.join(ROOT, "profiles", "ncu_vqvae_resblock_r02.txt"))
+    if dumped is not None:
+        dump_outputs(args.dump_outputs, dumped)
     return dict(metric="vqvae_decode_clips_per_sec", value=value, unit="clips/s (3 levels each)", n_gpus=world,
                 steps=steps, warmup=warmup, ms_per_step=float(ms) / steps, higher_is_better=True, scaling="weak",
                 dtype="f32", data="synthetic",
@@ -480,9 +495,7 @@ def measure_vqvae(args, rank, world, local, steps, warmup, small=False):
                          api="VQVAE.decode(zs[l:], start_level=l, bs_chunks=N) for l in 0..2"),
                 gpu_launches=int(launches),
                 roofline=dict(bound="hbm", achieved=bytes_plan / t_clip / 1e9, peak=hbm, unit="GB/s",
-                              frac=bytes_plan / t_clip / 1e9 / hbm, traffic=traffic,
-                              traffic_source="profiles/ncu_vqvae_resblock_r02.txt: dram bytes of ONE launch of the dominant "
-                                             "kernel, resblock_t5_kernel<64> on [4, 262144, 64] (algorithmic: 537 MB in + out)",
+                              frac=bytes_plan / t_clip / 1e9 / hbm,
                               note="per-block-fused activation plan 7.3 GB fp32 per clip (SURVEY 8d); compute side: "
                                    "%.1f TFLOP/s achieved of %.0f (bf16 dense peak)" % (flops_clip / t_clip / 1e12, tf)))
 
@@ -564,7 +577,7 @@ def main():
                 enc_kv = prior.get_encoder_kv(prime, fp16=True, sample=True)
             return SamplingWindow(ca, n, z_in, x_cond, y_cond, enc_kv, True, 0.99, 0, 0.0, False, None)
 
-    state = dict(win=None, k=0)
+    state = dict(win=None, k=0, last=None)
     per_slice = n_ctx // N_SLICES
 
     def slice_step():
@@ -572,7 +585,9 @@ def main():
         if k == 0:
             state["win"] = begin_window()
         win = state["win"]
+        lo = win.pos
         win.advance(win.P + per_slice * (k + 1) if k < N_SLICES - 1 else win.sample_tokens)
+        state["last"] = (win, lo, win.pos)         # the positions this step sampled (they are written once)
         if k == N_SLICES - 1:
             if prior.single_enc_dec:
                 prior.prior_postprocess(win.finish())
@@ -598,6 +613,10 @@ def main():
     e1.record()
     barrier()
     torch.cuda.profiler.stop()
+    dumped = None
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        lwin, lo, hi = state["last"]
+        dumped = dict(tokens=lwin.tokens[:, lo:hi].double().cpu().numpy(), logits=lwin.lbuf.float().cpu().numpy())
     launches_timed = _lib.CALLS - calls0       # C-ABI calls that launched our kernels in the timed region
     ms = torch.tensor([e0.elapsed_time(e1)], device="cuda")
     if world > 1:
@@ -663,17 +682,13 @@ def main():
     ca.transformer.del_cache()
     total_bytes, w_bytes = algorithmic_bytes(prior, n, positions)
     peaks = load_peaks()
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", HBM_GBS_H100))
     achieved = total_bytes / (kern_ms * 1e-3) / 1e9
-    cap = os.path.join(ROOT, "profiles", "ncu_decode_step_final_p4000_r02.txt")      # the shipped kernel, position 4000
-    traffic = None if args.small or args.workload != "1b_lyrics" else ncu_dram_bytes(cap)
-    roof = dict(bound="hbm", achieved=achieved, peak=peak, unit="GB/s", frac=achieved / peak, traffic=traffic,
-                traffic_source="profiles/ncu_decode_step_final_p4000_r02.txt (ncu --set full, one launch at position 4000; "
-                               "positions 500 / 8000: ncu_decode_step_final_p500_r02.txt / _p8000_r02.txt)",
+    roof = dict(bound="hbm", achieved=achieved, peak=peak, unit="GB/s", frac=achieved / peak,
                 kernel="jk_decode_step_kernel", launches=len(positions), avg_launch_us=1e3 * kern_ms / len(positions),
                 positions=f"{reps} consecutive launches from each of {octile}",
                 algorithmic_bytes_per_launch=total_bytes / len(positions), weight_bytes_per_launch=w_bytes,
-                peak_source="MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "fallback 6650 GB/s")
+                peak_source="MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "H100 SXM data sheet")
     # ---- secondary metric: VQ-VAE decode (BASELINE configs[4]) -----------------------------------------
     secondary = None
     if not args.no_secondary and args.workload == "1b_lyrics":
@@ -738,6 +753,8 @@ def main():
                                   positions=f"0..{np_pos - 1}", samples=n, full_size=not args.small)
         except Exception as e:
             line["cpu_baseline_error"] = repr(e)
+    if dumped is not None:
+        dump_outputs(args.dump_outputs, dumped)
     print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()

@@ -1,5 +1,5 @@
 /*
- * jkb200.h - C ABI of libjkb200.so: B200 (sm_100a) kernels for Jukebox's sampling hot path.
+ * jkb200.h - C ABI of libjkb200.so: H100 (sm_90a) kernels for Jukebox's sampling hot path.
  *
  * Boundary contract (SURVEY.md section 8b):
  *   - plain C: pointers, sizes, cudaStream_t (passed as void*); no torch types
@@ -147,7 +147,7 @@ typedef struct jk_step_args {
 /* Chunked prefill of the given (prime) tokens: positions 0 .. n_positions-1 of every sample through all
  * layers in one call - the chunked half of ConditionalAutoregressive2D.primed_sample
  * (prior/autoregressive.py:251-359), whose own check_chunks asserts it equals stepping token by token.
- * The four Conv1Ds of each layer run as [n_samples * n_positions, K] x [K, N] GEMMs on tcgen05.  On return
+ * The four Conv1Ds of each layer run as [n_samples * n_positions, K] x [K, N] GEMMs on wgmma.  On return
  * the engine stands at position n_positions (K/V caches filled), exactly as after that many jk_prior_step
  * calls.  tokens[b * tok_stride + t] is the token AT position t (the input of position t+1), as in
  * jk_step_args; h_out (optional, fp32 [n_samples, n_positions, width]) receives the transformer output -
@@ -175,7 +175,7 @@ int jk_prior_position(const jk_prior* p, int* t);
  * which: 0 = h, 1 = qkv, 2 = attention out, 3 = x1 (x + a), 4 = gelu out.  Returns device ptr. */
 int jk_prior_debug_buffer(const jk_prior* p, int which, const void** ptr, size_t* n_halfs);
 
-/* Conv1D at prefill / training shape on the tensor cores (tcgen05 + TMA): y[M, N] = x[M, K] . w + b, fp16 in,
+/* Conv1D at prefill / training shape on the tensor cores (wgmma + TMA): y[M, N] = x[M, K] . w + b, fp16 in,
  * fp32 accumulate, fp16 out (transformer/ops.py:83-101).  w_t is the weight TRANSPOSED: [N, K] row-major fp16;
  * bias fp32 [N] or NULL; K must be a multiple of 64.  Used for c_enc_kv(encoder_kv)
  * (factored_attention.py:273-287) inside jk_prior_set_encoder_kv. */

@@ -1,4 +1,4 @@
-"""Build libjkb200.so in-tree with nvcc for sm_100a (no JIT cache, the .so travels with the repo).
+"""Build libjkb200.so in-tree with nvcc for sm_90a (H100; no JIT cache, the .so travels with the repo).
 
     python -m jukebox_b200.build [--force]
 """
@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libjkb200.so")
 STAMP = os.path.join(HERE, ".libjkb200.stamp")
 SOURCES = ["api.cu", "decode_engine.cu", "f32_path.cu", "prefill.cu", "prefill_gemm.cu", "sampling.cu", "vqvae_kernels.cu", "vqvae_t5.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "--shared", "-Xcompiler", "-fPIC", 
               "-Xcompiler", "-Wno-unused-function", "--expt-relaxed-constexpr", "-rdc=false"]
 

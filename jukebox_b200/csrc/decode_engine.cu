@@ -1,4 +1,4 @@
-// Persistent decode-step engine for Jukebox's autoregressive priors on B200 (sm_100a).
+// Persistent decode-step engine for Jukebox's autoregressive priors on H100 (sm_90a).
 //
 // One launch = one token position for up to 16 samples through the WHOLE transformer stack
 // (reference: ConditionalAutoregressive2D.sample loop body, prior/autoregressive.py:222-237,
@@ -121,16 +121,21 @@ __device__ __forceinline__ uint8_t* sm_uni() { return jk_smem + kHeaderBytes; }
 __device__ __forceinline__ const EngineDev* sm_E() { return reinterpret_cast<const EngineDev*>(jk_smem + 512); }
 __device__ __forceinline__ const LayerDev* sm_layer(int i) { return reinterpret_cast<const LayerDev*>(jk_smem + 1024 + 256 * (i & 1)); }
 
+// Position in the weight ring.  Only the slot and its parity travel (in registers) through the phase calls; the slot
+// count and slot 0's offset are per-launch constants read from the descriptor in shared memory where they are needed, so
+// that ptxas' inter-procedural allocation has two registers more for the phase functions.
 struct Ring {
-    int base_off;          // byte offset of slot 0 inside jk_smem
-    int nslot;
     int slot;
     uint32_t phase;
+    __device__ __forceinline__ static int nslot() { return sm_E()->nslot; }
     __device__ __forceinline__ uint64_t* full() const { return sm_full() + slot; }
     __device__ __forceinline__ uint64_t* empty() const { return sm_empty() + slot; }
-    __device__ __forceinline__ uint8_t* data() const { return jk_smem + base_off + slot * kSlotBytes; }
+    __device__ __forceinline__ uint8_t* data() const {
+        const EngineDev* E = sm_E();
+        return jk_smem + kHeaderBytes + E->uni_bytes + E->kvpre_bytes + slot * kSlotBytes;
+    }
     __device__ __forceinline__ void advance() {
-        if (++slot == nslot) { slot = 0; phase ^= 1u; }
+        if (++slot == nslot()) { slot = 0; phase ^= 1u; }
     }
 };
 
@@ -154,7 +159,7 @@ __device__ __forceinline__ void ll_st(unsigned long long* p, uint32_t data, uint
     asm volatile(JK_ST_LL ".u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 // Polled loads are relaxed gpu-scope loads (SASS LDG.E.STRONG.GPU).  A weak ld.global.cg compiles to the SAME SASS load
-// on sm_100a, but ptxas may hoist a weak load out of the polling loop (it did: the weak build deadlocked into the spin
+// on sm_90a, but ptxas may hoist a weak load out of the polling loop (it did: the weak build deadlocked into the spin
 // guard), so the strong form is the only usable one.
 __device__ __forceinline__ ulonglong2 ll_ld2(const unsigned long long* p) {
     ulonglong2 v;
@@ -259,8 +264,7 @@ __device__ __noinline__ void stage_acts(const unsigned long long* in, int K, int
     const int astride = (Ks + 8) * 2;
     // LayerNorm statistics of the 16 rows: lane r polls the two adjacent words (sum, sum of squares) of row r with one
     // 16-byte load until every CTA has contributed to both (16 pollers per CTA on 16 lines).  Called AFTER this thread's
-    // activation loads are issued: on the 16 polling threads the two latencies overlap instead of adding up
-    // (profiles/phase_profile_r02d.txt: statistics ready at 0.8 us, the pollers' own loads in at 1.8 us before this).
+    // activation loads are issued: on the 16 polling threads the two latencies overlap instead of adding up.
     auto row_statistics = [&]() {
         const int G = sm_E()->G;
         float mean = 0.f, rstd = 0.f;
@@ -425,7 +429,7 @@ __device__ __forceinline__ LogitsRec* sm_lrec() { return reinterpret_cast<Logits
 // One Conv1D of layer l (or the logits GEMM), identified by its epilogue.  The argument record is assembled HERE from the
 // descriptor / layer record / column table in shared memory: passed by value it had grown past what the call ABI keeps in
 // registers (896 bytes of stack), and with the shared-memory carve-out at its maximum every local-memory access is an L2
-// round trip - the step went from 1.95 to 2.5 ms (profiles/decode_variants_ab_r02b.txt).
+// round trip - the step went from 1.95 to 2.5 ms.
 __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int pslot_, uint32_t fl) {
     const EngineDev* E = sm_E();
     GemmArgs g;
@@ -500,7 +504,7 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
     // contiguous runs one warp would own several consecutive slots while the ring delivers them in order, i.e. one warp
     // would multiply at a time (5b_lyrics, one box: 6 192 us per step round robin, 6 691 us with contiguous runs).
     const int nslots_phase = (nkk + kpc - 1) >> (31 - __clz(kpc));
-    const bool in_order = !JK_SKIP_FOREIGN_WAIT || nslots_phase > ring.nslot;
+    const bool in_order = !JK_SKIP_FOREIGN_WAIT || nslots_phase > Ring::nslot();
     int slot_i = 0;
 #define JK_MMA_LOOP(NCG)                                                                      \
     {                                                                                         \
@@ -611,7 +615,7 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
         const float2 bias = (active && g.bias) ? *reinterpret_cast<const float2*>(g.bias + gc) : make_float2(0.f, 0.f);
         // warp-uniform trip count (the two half warps of the 16-pair layout hold rows 2w and 2w + 1; only the row index
         // differs), so that the shuffles below run under the constant full mask: a run-time member mask compiles to
-        // WARPSYNC.COLLECTIVE, which cost 3.5 us per residual epilogue (profiles/phase_profile_r02e.txt)
+        // WARPSYNC.COLLECTIVE, which cost 3.5 us per residual epilogue
         const int bw0 = two_rows ? 2 * warp : warp;
 #pragma unroll 1
         for (int bw = bw0; bw < B; bw += b_step) {
@@ -1425,6 +1429,24 @@ __device__ __noinline__ void cleaner_loop() {
 }
 
 // ---------------------------------------------------------------------------------------
+// Values of a launch that every phase call would otherwise have to keep in a register: ptxas allocates the __noinline__
+// phases inter-procedurally, so each value live across the calls is a register less inside them (on sm_90a, keeping
+// these in registers made gemm_phase spill).  The descriptor fields are re-read from its shared-memory copy; the position
+// and the step count live in header words [7724] and [7728], written by the kernel prologue.
+__device__ __forceinline__ int launch_pos() { return reinterpret_cast<const int*>(jk_smem + 7712)[3]; }
+__device__ __forceinline__ uint32_t launch_step() { return (uint32_t)reinterpret_cast<const int*>(jk_smem + 7712)[4]; }
+// LL flags of this launch: launch_fbase() + 1 .. launch_fbase() + depth + 1
+__device__ __forceinline__ uint32_t launch_fbase() { return launch_step() * (uint32_t)(sm_E()->depth + 2); }
+__device__ __forceinline__ int cta_unit() { return (int)blockIdx.x >> sm_E()->ks_shift; }
+__device__ __forceinline__ int cta_rank() { return (int)blockIdx.x & (sm_E()->KS - 1); }
+__device__ __forceinline__ bool wants_logits(const StepArgs& A) { return A.logits != nullptr && sm_E()->bins > 0; }
+// y = h + x_cond is not an fp16 value: those configurations (upsamplers) keep the fp32 FMA path (unless the caller supplies
+// x_cond . x_out^T, the logit bias of jkb200.h: the product is linear in the activation)
+__device__ __forceinline__ bool logits_on_mma(const StepArgs& A) {
+    const EngineDev* E = sm_E();
+    return JK_LOGITS_MMA && E->lg_on && (!(E->add_cond_after && A.x_cond) || A.logit_bias);
+}
+
 __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const EngineDev* __restrict__ Eg, StepArgs A) {
     const int tid = threadIdx.x, warp = tid >> 5;
     const int c = blockIdx.x;
@@ -1436,38 +1458,28 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
         reinterpret_cast<uint32_t*>(jk_smem + 1024)[tid] = reinterpret_cast<const uint32_t*>(&Eg->layer[0])[tid];
     __syncthreads();
     const EngineDev* E = sm_E();
-    const int KS = E->KS, unit = c >> E->ks_shift, rank = c & (KS - 1);
     if (tid >= 32 && tid < 36)
         reinterpret_cast<uint32_t*>(jk_smem + 1024 + 128)[tid - 32] =
-            reinterpret_cast<const uint32_t*>(E->cols + ((size_t)unit * E->depth + 0) * 4)[tid - 32];
+            reinterpret_cast<const uint32_t*>(E->cols + ((size_t)cta_unit() * E->depth + 0) * 4)[tid - 32];
     Ring ring;
-    ring.base_off = kHeaderBytes + E->uni_bytes + E->kvpre_bytes; ring.nslot = E->nslot; ring.slot = 0; ring.phase = 0;
+    ring.slot = 0; ring.phase = 0;
     if (tid == 0) {
         for (int i = 0; i < E->nslot; ++i) { mbar_init(sm_full() + i, 1); mbar_init(sm_empty() + i, 8); }
         mbar_fence_init();
     }
     __syncthreads();
-    const bool do_logits = (A.logits != nullptr) && E->bins > 0;
-    // y = h + x_cond is not an fp16 value: those configurations (upsamplers) keep the fp32 FMA path
-    // (unless the caller supplies x_cond . x_out^T, the logit bias of jkb200.h: the product is linear in the activation)
-    const bool lg_mma = JK_LOGITS_MMA && E->lg_on && (!(E->add_cond_after && A.x_cond) || A.logit_bias);
     // Register reallocation between warpgroups (setmaxnreg, sm_90a+): the block launches with 168 registers per
     // thread (65536 / 384); the producer warpgroup keeps 40 and hands the rest to the two consumer warpgroups.
     if (warp >= 8) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-        if (warp == 8) producer_loop(Eg, ring, do_logits ? (lg_mma ? 2 : 1) : 0, c);
+        if (warp == 8) producer_loop(Eg, ring, wants_logits(A) ? (logits_on_mma(A) ? 2 : 1) : 0, c);
 #if JK_CLEANER_WARP
         else if (warp == 9 && c == 0) cleaner_loop();
 #endif
         return;
     }
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-    const int t = *reinterpret_cast<volatile const int*>(E->t);
-    // steps executed so far: written only at the very end of a launch by CTA 0, after every CTA of that launch has
-    // passed an all-to-all point - so every CTA of this launch reads the same value
-    const unsigned step = *reinterpret_cast<volatile const unsigned*>(E->sync + 64);
-    const int B = A.n, W = E->W, S = E->S, M = E->M, G = E->G, depth = E->depth;
-    const uint32_t fbase = step * (uint32_t)(depth + 2);          // LL flags of this launch: fbase + 1 .. fbase + depth + 1
+    const int B = A.n;
     // statistics blocks: 2l = input of layer l's LN0, 2l + 1 = input of its LN1, 2 * depth = the final residual stream
     // (nobody normalises it; its count tells CTA 0 that every CTA is through the stack)
 #define LN_BLOCK(i_) (E->lnacc + (size_t)(i_) * 512)
@@ -1479,27 +1491,33 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
 #define CLEAR_AFTER(clear_, seen_)                                                             \
     do {                                                                                       \
         if (c == 0 && tid < 32) {                                                              \
-            if (tid == 0) wait_stat_word(LN_BLOCK(seen_), G);                                  \
+            if (tid == 0) wait_stat_word(LN_BLOCK(seen_), E->G);                               \
             __syncwarp();                                                                      \
             LN_BLOCK(clear_)[16 * (tid >> 1) + (tid & 1)] = 0;                                 \
         }                                                                                      \
     } while (0)
 #endif
     // thread layouts of the activation staging for the three K of a layer (integer divisions: once per launch, not per phase)
-    // per-launch constants that need an integer division live in shared memory (not in registers across the phase calls):
-    // [7712] p % block_ctx, [7716] p / block_ctx, [7720] CTAs available per (sample, head)
+    // per-launch values live in shared memory (not in registers across the phase calls):
+    // [7712] p % block_ctx, [7716] p / block_ctx, [7720] CTAs available per (sample, head), [7724] position t,
+    // [7728] steps executed so far
     if (tid == 0) {
         int* gq = reinterpret_cast<int*>(jk_smem + 7712);
+        const int t = *reinterpret_cast<volatile const int*>(E->t);
         gq[0] = E->blocks > 0 ? t % E->bc : 0;
         gq[1] = E->blocks > 0 ? t / E->bc : 0;
-        gq[2] = max(1, G / (B * E->H));
+        gq[2] = max(1, E->G / (B * E->H));
+        gq[3] = t;
+        // written only at the very end of a launch by CTA 0, after every CTA of that launch has passed an all-to-all
+        // point - so every CTA of this launch reads the same value
+        gq[4] = (int)*reinterpret_cast<volatile const unsigned*>(E->sync + 64);
     }
 #define PM (reinterpret_cast<const int*>(jk_smem + 7712)[0])
 #define PD (reinterpret_cast<const int*>(jk_smem + 7712)[1])
 #define GMAX (reinterpret_cast<const int*>(jk_smem + 7712)[2])
-    stage_map_init(0, W >> E->ks_shift);
-    stage_map_init(1, S >> E->ks_shift);
-    stage_map_init(2, M >> E->ks_shift);
+    stage_map_init(0, E->W >> E->ks_shift);
+    stage_map_init(1, E->S >> E->ks_shift);
+    stage_map_init(2, E->M >> E->ks_shift);
     consumer_sync();
     unsigned nph = 0;                                             // phase index (profiling slots)
 #define PHASE_DONE()                                                                           \
@@ -1535,18 +1553,18 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
         const int lane = tid & 31;
         for (int b = warp; b < B && lane < ppc; b += 8) {     // lane = column pair, warp = sample row (and row + 8)
             const int pl = lane;
-            const int col = wc.x * 8 + 2 * (rank * ppc + pl);
+            const int col = wc.x * 8 + 2 * (cta_rank() * ppc + pl);
             float2 x;
             if (A.x_in) {
-                x = *reinterpret_cast<const float2*>(A.x_in + (size_t)b * W + col);
+                x = *reinterpret_cast<const float2*>(A.x_in + (size_t)b * E->W + col);
             } else {
-                if (t == 0) x = A.y_cond ? *reinterpret_cast<const float2*>(A.y_cond + (size_t)b * W + col)
+                if (launch_pos() == 0) x = A.y_cond ? *reinterpret_cast<const float2*>(A.y_cond + (size_t)b * E->W + col)
                                          : *reinterpret_cast<const float2*>(E->start_token + col);
-                else x = *reinterpret_cast<const float2*>(E->x_emb + (size_t)A.tokens[(size_t)b * A.tok_stride + t - 1] * W + col);
-                const float2 pe = *reinterpret_cast<const float2*>(E->pos_emb + (size_t)t * W + col);
+                else x = *reinterpret_cast<const float2*>(E->x_emb + (size_t)A.tokens[(size_t)b * A.tok_stride + launch_pos() - 1] * E->W + col);
+                const float2 pe = *reinterpret_cast<const float2*>(E->pos_emb + (size_t)launch_pos() * E->W + col);
                 x.x += pe.x; x.y += pe.y;
                 if (A.x_cond) {
-                    const float2 xc = *reinterpret_cast<const float2*>(A.x_cond + ((size_t)b * A.x_cond_len + (A.x_cond_len > 1 ? t : 0)) * W + col);
+                    const float2 xc = *reinterpret_cast<const float2*>(A.x_cond + ((size_t)b * A.x_cond_len + (A.x_cond_len > 1 ? launch_pos() : 0)) * E->W + col);
                     x.x += xc.x; x.y += xc.y;
                 }
             }
@@ -1555,19 +1573,17 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
             res[b * 32 + pl] = hv;
             sfx[b * 32 + pl] = fx_sum(hv.x) + fx_sum(hv.y);
             sfx[1024 + b * 32 + pl] = fx_sq(hv.x) + fx_sq(hv.y);
-            ll_st(E->ll_h + (((size_t)b * W + col) >> 1), *reinterpret_cast<const uint32_t*>(&hh), fbase + 1);
+            ll_st(E->ll_h + (((size_t)b * E->W + col) >> 1), *reinterpret_cast<const uint32_t*>(&hh), launch_fbase() + 1);
         }
         publish_stats(LN_BLOCK(0), B, ppc);
     }
     PHASE_DONE();
 
 #pragma unroll 1
-    for (int l = 0; l < depth; ++l) {
+    for (int l = 0; l < E->depth; ++l) {
         const LayerDev& LD = *sm_layer(l);
-        const ushort2* cl = reinterpret_cast<const ushort2*>(jk_smem + 1024 + 256 * (l & 1) + 128);
-        const int Nqkv = (LD.attn_func == 6) ? S : 3 * S;
-        const uint32_t fl = fbase + (uint32_t)l + 1;              // flag of this layer's buffers
-        const int pre = attn_prefetch(LD, B, c, t, PM, PD, GMAX);
+        const uint32_t fl = launch_fbase() + (uint32_t)l + 1;              // flag of this layer's buffers
+        const int pre = attn_prefetch(LD, B, c, launch_pos(), PM, PD, GMAX);
         // a fresh argument record per phase: nothing of it stays live across the calls in between
         if (l == 1) PROF3(0, 0);
         ring = gemm_phase(ring, B, EPI_QKV, l, (int)nph, fl);
@@ -1577,7 +1593,7 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
         // next layer's record + column assignment -> the other shared-memory slot.  The descriptor is in
         // HBM (the weight stream evicts it from L2 every step): issue the loads here so their latency hides
         // behind the attention phase instead of sitting on the dependency chain.
-        if (l + 1 < depth) {
+        if (l + 1 < E->depth) {
 #if JK_ASYNC_RECORD
             // cp.async: no register sits between the HBM load and the shared-memory store, so no warp stalls on it here;
             // it is waited for in front of this layer's last Conv1D (whose barriers publish it to the other threads)
@@ -1586,7 +1602,7 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
                              "l"(reinterpret_cast<const uint32_t*>(&Eg->layer[l + 1]) + tid) : "memory");
             if (tid >= 32 && tid < 36)
                 asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(jk_smem + 1024 + 256 * ((l + 1) & 1) + 128 + 4 * (tid - 32))),
-                             "l"(reinterpret_cast<const uint32_t*>(E->cols + ((size_t)unit * depth + l + 1) * 4) + (tid - 32)) : "memory");
+                             "l"(reinterpret_cast<const uint32_t*>(E->cols + ((size_t)cta_unit() * E->depth + l + 1) * 4) + (tid - 32)) : "memory");
             asm volatile("cp.async.commit_group;" ::: "memory");
 #else
             if (tid < (int)(sizeof(LayerDev) / 4))
@@ -1594,15 +1610,15 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
                     reinterpret_cast<const uint32_t*>(&Eg->layer[l + 1])[tid];
             if (tid >= 32 && tid < 36)
                 reinterpret_cast<uint32_t*>(jk_smem + 1024 + 256 * ((l + 1) & 1) + 128)[tid - 32] =
-                    reinterpret_cast<const uint32_t*>(E->cols + ((size_t)unit * depth + l + 1) * 4)[tid - 32];
+                    reinterpret_cast<const uint32_t*>(E->cols + ((size_t)cta_unit() * E->depth + l + 1) * 4)[tid - 32];
 #endif
         }
         PHASE_DONE();
         if (l == 1) PROF3(1, 0);
         {
-            const AttnGeom geo = attn_geom(E, LD, t, PM, PD);
+            const AttnGeom geo = attn_geom(E, LD, launch_pos(), PM, PD);
             const int ns = attn_nsplit(E, GMAX, geo.R - ((geo.R > 0 && geo.cur) ? 1 : 0));
-            for (int it = c; it < B * E->H * ns; it += G) {
+            for (int it = c; it < B * E->H * ns; it += E->G) {
                 const int bh = div_small(it, ns), s = it - bh * ns, ib = bh / E->H;
                 attn_item(LD, ib, bh - ib * E->H, s, ns, geo, (int)nph, fl, pre && it == c);
                 consumer_sync();           // tile / q regions are reused by the next item or the next phase
@@ -1629,45 +1645,45 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
         PHASE_DONE();
     }
     if (A.h_out) {      // Transformer.forward boundary: this CTA's slice of the residual stream
-        const ushort2 wc = reinterpret_cast<const ushort2*>(jk_smem + 1024 + 256 * ((depth - 1) & 1) + 128)[1];
+        const ushort2 wc = reinterpret_cast<const ushort2*>(jk_smem + 1024 + 256 * ((E->depth - 1) & 1) + 128)[1];
         const int ppc = (wc.y * 4) >> E->ks_shift;
         const float2* res = sm_res();
         const int lane = tid & 31;
         for (int b = warp; b < B && lane < ppc; b += 8) {
-            const int col = wc.x * 8 + 2 * (rank * ppc + lane);
-            *reinterpret_cast<float2*>(A.h_out + (size_t)b * W + col) = res[b * 32 + lane];
+            const int col = wc.x * 8 + 2 * (cta_rank() * ppc + lane);
+            *reinterpret_cast<float2*>(A.h_out + (size_t)b * E->W + col) = res[b * 32 + lane];
         }
     }
-    if (do_logits && lg_mma) {
+    if (wants_logits(A) && logits_on_mma(A)) {
         // logits GEMM: [y | y] (the final residual stream, fp16-exact) x [hi(x_out) ; lo(x_out)] on the tensor cores, through
         // the same phase code as every Conv1D; the K-split partial sums (hi and lo halves on different ranks) meet in fp32
-        stage_map_init(2, (2 * W) >> E->ks_shift);
+        stage_map_init(2, (2 * E->W) >> E->ks_shift);
         consumer_sync();
         if (tid == 0) {
             LogitsRec* lr = sm_lrec();
-            lr->lg_out = A.logits + (size_t)t * A.logits_tstride; lr->lg_bs = A.logits_bstride;
-            lr->lb = (E->add_cond_after && A.x_cond) ? A.logit_bias + (size_t)t * A.lb_tstride : nullptr; lr->lb_bs = A.lb_bstride;
-            lr->cols = E->lg_cols[unit];
+            lr->lg_out = A.logits + (size_t)launch_pos() * A.logits_tstride; lr->lg_bs = A.logits_bstride;
+            lr->lb = (E->add_cond_after && A.x_cond) ? A.logit_bias + (size_t)launch_pos() * A.lb_tstride : nullptr; lr->lb_bs = A.lb_bstride;
+            lr->cols = E->lg_cols[cta_unit()];
         }
         consumer_sync();
-        ring = gemm_phase(ring, B, EPI_LOGITS, depth - 1, (int)nph, fbase + (uint32_t)depth + 1);
-    } else if (do_logits) {
-        logits_phase(A, ring, c, t, fbase + (uint32_t)depth + 1);
+        ring = gemm_phase(ring, B, EPI_LOGITS, E->depth - 1, (int)nph, launch_fbase() + (uint32_t)E->depth + 1);
+    } else if (wants_logits(A)) {
+        logits_phase(A, ring, c, launch_pos(), launch_fbase() + (uint32_t)E->depth + 1);
     }
     // the last LN1 block and the final block: clear them once every CTA is through the stack
-    CLEAR_AFTER(2 * depth - 1, 2 * depth);
+    CLEAR_AFTER(2 * E->depth - 1, 2 * E->depth);
     if (c == 0) {
         consumer_sync();
 #if !JK_CLEANER_WARP
-        if (tid < 32) LN_BLOCK(2 * depth)[16 * (tid >> 1) + (tid & 1)] = 0;
+        if (tid < 32) LN_BLOCK(2 * E->depth)[16 * (tid >> 1) + (tid & 1)] = 0;
 #endif
         if (tid == 0) {
             unsigned long long now;
             asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
             if (E->prof_on && nph + 1 < (unsigned)kProfSlots) E->prof[nph + 1] = now;
 #if !JK_CLEANER_WARP
-            *E->t = t + 1;
-            *(E->sync + 64) = step + 1;
+            *E->t = launch_pos() + 1;
+            *(E->sync + 64) = launch_step() + 1;
 #endif
         }
     }
@@ -1760,7 +1776,7 @@ __global__ void to_half_kernel(const T* __restrict__ src, __half* dst, size_t n)
 }
 
 // encoder K/V for attn_func 6: kv = fp16(fp16(enc) . Wkv + b), once per window.  The product itself runs on
-// the tcgen05 prefill GEMM (prefill_gemm.cu); these kernels only convert / lay out its operands and result.
+// the wgmma prefill GEMM (prefill_gemm.cu); these kernels only convert / lay out its operands and result.
 template <typename T>
 __global__ void transpose_to_half_kernel(const T* __restrict__ src, __half* __restrict__ dst, int K, int N) {
     // src [K][N] row-major -> dst [N][K] row-major (the K-major layout the tensor core reads)
@@ -1880,9 +1896,18 @@ int compute_layout(const jk_prior_config& c, int G, Layout& L) {
                 // CTA that finishes a column keeps that column of the residual stream in its shared memory
                 for (int i = 0; i < extra; ++i) n[i] += 1;
             } else {
-                for (int i = 0; i < U; ++i) order[i] = i;
-                std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return cum[a] < cum[b]; });
-                for (int i = 0; i < extra; ++i) n[order[i]] += 1;
+                // water-filling: each extra group goes to the unit whose stream is shortest so far, a unit may take more
+                // than one.  With 33 units (132 SMs, KS = 4) the fixed width-W assignment above leaves 8 units 10 KB per
+                // layer behind, more than one extra group per Conv1D can make up: the longest stream of 1b_lyrics was 3.1 %
+                // above the shortest, now 0.1 % (tests/test_decode_plan_cpu.py).  Its effect on the step time has not been
+                // measured separately.
+                const unsigned long long chunk = (unsigned long long)(Ks[gi] / KS / 16) * 256ull;
+                for (int i = 0; i < extra; ++i) {
+                    int best = -1;
+                    for (int u = 0; u < U; ++u)
+                        if (n[u] < 8 && (best < 0 || cum[u] + n[u] * chunk < cum[best] + n[best] * chunk)) best = u;
+                    n[best] += 1;
+                }
             }
             int g0 = 0;
             for (int u = 0; u < U; ++u) {
@@ -1993,8 +2018,8 @@ int compute_layout(const jk_prior_config& c, int G, Layout& L) {
         L.off_ency = off; if (any6) off = align_up(off + (size_t)c.max_batch * c.encoder_dims * 2 * c.n_state * 2, 1024);
     }
     {   // chunked prefill: K-major fp16 weight copies + activation workspace (prefill.cu).  Every GEMM K must give
-        // 16-byte rows (K % 8) and fill at least one tcgen05 K block; K tails are zero-filled by TMA.  The workspace
-        // holds a whole window (n_ctx positions x max_batch: 2.8 GB for 1b_lyrics - 180 GB of HBM is there to be used),
+        // 16-byte rows (K % 8) and fill at least one GEMM K block; K tails are zero-filled by TMA.  The workspace
+        // holds a whole window (n_ctx positions x max_batch: 2.8 GB for 1b_lyrics of the H100's 80 GB),
         // so continuation windows re-prime their 4096 given tokens in one pass; JK_PREFILL_MAX lowers it.
         auto k_ok = [](int k) { return k >= 64 && k % 8 == 0; };
         const bool ok = k_ok(c.width) && k_ok(c.n_state) && k_ok(c.mlp_width) && !getenv("JK_NO_PREFILL");
@@ -2268,7 +2293,7 @@ extern "C" int jk_prior_set_encoder_kv(jk_prior* p, const float* encoder_kv, int
     const jk_prior_config& c = p->cfg;
     JK_REQUIRE(n >= 1 && n <= c.max_batch, "n_samples out of range");
     const int rows = n * c.encoder_dims;
-    JK_REQUIRE(c.width >= 64 && c.width % 8 == 0, "encoder-decoder layers need width >= 64 and width %% 8 == 0 (tcgen05 GEMM operand rows)");
+    JK_REQUIRE(c.width >= 64 && c.width % 8 == 0, "encoder-decoder layers need width >= 64 and width %% 8 == 0 (GEMM operand rows)");
     {   // encoder_kv.type_as(x): fp32 -> fp16 once, shared by every enc-dec layer
         const size_t cnt = (size_t)rows * c.width;
         to_half_kernel<float><<<(unsigned)((cnt + 255) / 256), 256, 0, stream>>>(encoder_kv, p->enc_x16, cnt);

@@ -49,7 +49,7 @@ struct EngineDev {
     LayerDev layer[JK_MAX_DEPTH];
 };
 
-// prefill_gemm.cu: Y = epi(X . W^T + bias [, res]) on tcgen05; w_t is [N, K] fp16.
+// prefill_gemm.cu: Y = epi(X . W^T + bias [, res]) on wgmma; w_t is [N, K] fp16.
 //   epi 0: fp16(acc + b)   1: fp16(quick_gelu(fp16(acc + b)))   2: fp16(res + fp16(acc + b))
 int gemm_f16_tc(const void* x, const void* w_t, const float* bias, const void* res, void* y, int M, int N, int K,
                 int epi, cudaStream_t stream);

@@ -4,7 +4,7 @@
 // tokens through the transformer in chunks before sampling, and its own check (:330-338, check_chunks)
 // asserts chunked == token-by-token.  The decode kernel (decode_engine.cu) is the token-by-token form; this
 // file is the chunked form: M = n_samples x P rows per GEMM, so the four Conv1Ds of a layer run on the
-// tcgen05 GEMM (prefill_gemm.cu) instead of streaming 1.8 GB of weights once per position.
+// wgmma GEMM (prefill_gemm.cu) instead of streaming 1.8 GB of weights once per position.
 //
 // Per layer (rows m = b*P + p, fp16 activations, the decode kernel's rounding points):
 //   xn  = LN0(x)                      ln_rows_kernel            (ops.py:14-24)

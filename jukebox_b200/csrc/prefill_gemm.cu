@@ -1,21 +1,20 @@
-// Prefill-shape Conv1D on the 5th-generation tensor cores: Y[M, N] = X[M, K] . W[K, N] + b  (fp16 in,
-// fp32 accumulate in TMEM, fp16 out), M = n_samples * rows >= 128.
+// Prefill-shape Conv1D on the Hopper tensor cores: Y[M, N] = X[M, K] . W[K, N] + b  (fp16 in, fp32 accumulate in
+// registers, fp16 out), M = n_samples * rows >= 128.
 //
 // Reference: Conv1D.forward (transformer/ops.py:83-101) at the shapes where it is compute bound - here
 // `c_enc_kv(encoder_kv)` of the encoder-decoder attention layers (factored_attention.py:273-287,
 // M = n * encoder_dims = 4096, K = 4800, N = 2400 for 5b_lyrics), computed once per window.
 //
 // Kernel anatomy (one 128 x 128 output tile per CTA, K walked in 64-element blocks):
-//   warp 0   TMA producer : cp.async.bulk.tensor.2d (SASS UTMALDG) of the X tile [128 x 64] and the W^T tile
-//                           [128 x 64], both K-major with the 128-byte swizzle, into a 4-stage ring
-//   warp 1   MMA issuer   : one elected thread issues tcgen05.mma.cta_group::1.kind::f16 (SASS UTCHMMA),
-//                           M = 128, N = 128, K = 16, accumulator = 128 TMEM columns; tcgen05.commit frees
-//                           the smem stage / signals the epilogue.  This warp also owns the TMEM allocation.
-//   warps 2-5 epilogue    : tcgen05.ld (SASS LDTM) 32 lanes x 32 columns at a time, + bias, round to fp16,
-//                           16-byte stores (rows and columns beyond M, N are predicated off; TMA zero-fills
-//                           out-of-bounds loads)
+//   warp 8      TMA producer : cp.async.bulk.tensor.2d of the X tile [128 x 64] and the W^T tile [128 x 64], both
+//                              K-major with the 128-byte swizzle, into a 3-stage ring
+//   warps 0-7   consumers    : two warpgroups, rows 0-63 and 64-127 of the tile; each issues
+//                              wgmma.mma_async m64n128k16 (64 fp32 accumulators per thread), keeps one K block in
+//                              flight and frees the previous stage when it retires; then + bias, round to fp16 and
+//                              store (rows and columns beyond M, N are predicated off; TMA zero-fills
+//                              out-of-bounds loads)
 // W is supplied transposed ([N, K], K contiguous) - the engine packs it once at weight load - so both
-// operands are K-major, the layout the tensor core reads without a transpose bit.
+// operands are K-major, the layout wgmma reads without a transpose bit.
 #include "engine.cuh"
 #include <cuda.h>
 
@@ -25,7 +24,7 @@ namespace {
 
 constexpr int BM = 128, BN = 128, BK = 64, STAGES = 3;   // 3 x 32 KB: two CTAs per SM, one's epilogue overlaps the other's main loop
 constexpr int kTileBytes = BM * BK * 2;                  // 16 KB per operand tile
-constexpr int kGemmThreads = 192;
+constexpr int kGemmThreads = 288;                        // two consumer warpgroups + one producer warp
 constexpr int kGemmSmem = STAGES * 2 * kTileBytes + 1024 + 256;
 
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
@@ -34,34 +33,6 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
             smem_u32(smem_dst)),
         "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
-}
-
-// shared-memory matrix descriptor, K-major operand, 128-byte swizzle, 8-row groups 1024 bytes apart
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);          // start address, bits [0,14)
-    d |= (uint64_t)1 << 16;                                 // leading byte offset (unused for swizzled K-major)
-    d |= (uint64_t)(1024 >> 4) << 32;                       // stride byte offset: 8 rows * 128 B
-    d |= (uint64_t)1 << 46;                                 // descriptor version (sm_100)
-    d |= (uint64_t)2 << 61;                                 // layout type: SWIZZLE_128B
-    return d;
-}
-
-// instruction descriptor: D = F32, A = B = F16, both K-major, N >> 3 at bit 17, M >> 4 at bit 24
-__device__ __forceinline__ uint32_t umma_idesc() {
-    return (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-}
-
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
 // The decode kernel's epilogues (decode_engine.cu gemm_phase), same fp16 rounding points:
@@ -87,29 +58,19 @@ prefill_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
     uint8_t* tiles = gsm;                                               // [STAGES][A | B]
     uint64_t* full = reinterpret_cast<uint64_t*>(gsm + STAGES * 2 * kTileBytes);
     uint64_t* empty = full + STAGES;
-    uint64_t* acc_full = empty + STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
     const int nkb = (K + BK - 1) / BK;       // a K tail reads zeros: TMA zero-fills both operands beyond K
 
     if (tid == 0) {
-        for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-        mbar_init(acc_full, 1);
+        for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); }   // empty: one arrival per warpgroup
         mbar_fence_init();
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_x)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_w)) : "memory");
     }
-    if (warp == 1) {                                                     // TMEM: 128 columns of fp32 accumulators
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(128));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             for (int kb = 0; kb < nkb; ++kb) {
                 const int s = kb % STAGES;
@@ -119,70 +80,46 @@ prefill_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
                 tma_load_2d(tiles + s * 2 * kTileBytes + kTileBytes, &map_w, kb * BK, n0, &full[s]);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc = umma_idesc();
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int s = kb % STAGES;
-                mbar_wait(&full[s], (kb / STAGES) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t a0 = smem_u32(tiles + s * 2 * kTileBytes), b0 = a0 + kTileBytes;
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k)                        // 16 fp16 = 32 bytes per MMA K step
-                    umma_f16(tmem_base, umma_desc(a0 + k * 32), umma_desc(b0 + k * 32), idesc, (kb | k) ? 1u : 0u);
-                umma_commit(&empty[s]);                                  // frees the stage when these MMAs retire
-            }
-            umma_commit(acc_full);                                       // accumulator complete
-        }
-    } else {
-        const int q = warp & 3;                                          // TMEM lane quarter this warp may read
-        mbar_wait(acc_full, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int row = m0 + q * 32 + lane;
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 32) {
-            uint32_t r[32];
-            const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0;
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                  "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                  "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                  "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                : "r"(taddr));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            if (row < M) {
-                __half* yr = y + (size_t)row * N + n0 + c0;
-                const __half* rr = res ? res + (size_t)row * N + n0 + c0 : nullptr;
-                if (n0 + c0 + 32 <= N && (N & 7) == 0) {
-#pragma unroll
-                    for (int v = 0; v < 4; ++v) {
-                        uint4 rv = make_uint4(0, 0, 0, 0);
-                        if (epi == 2) rv = *reinterpret_cast<const uint4*>(rr + v * 8);
-                        const __half* rh = reinterpret_cast<const __half*>(&rv);
-                        __half h[8];
-#pragma unroll
-                        for (int e = 0; e < 8; ++e) {
-                            const int c = v * 8 + e;
-                            h[e] = epilogue_value(__uint_as_float(r[c]), bias ? bias[n0 + c0 + c] : 0.f, __half2float(rh[e]), epi);
-                        }
-                        *reinterpret_cast<uint4*>(yr + v * 8) = *reinterpret_cast<uint4*>(h);
-                    }
-                } else {
-                    for (int c = 0; c < 32 && n0 + c0 + c < N; ++c)
-                        yr[c] = epilogue_value(__uint_as_float(r[c]), bias ? bias[n0 + c0 + c] : 0.f,
-                                               epi == 2 ? __half2float(rr[c]) : 0.f, epi);
-                }
-            }
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+        return;
     }
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(128));
+    const int wg = warp >> 2, wt = tid & 127;                            // warpgroup: rows 64 wg .. 64 wg + 63
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < nkb; ++kb) {
+        const int s = kb % STAGES;
+        mbar_wait(&full[s], (kb / STAGES) & 1);
+        const uint32_t a0 = smem_u32(tiles + s * 2 * kTileBytes) + wg * (64 * 128), b0 = smem_u32(tiles + s * 2 * kTileBytes + kTileBytes);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)                                // 16 fp16 = 32 bytes per MMA K step
+            wgmma_ss<BN>(acc, wgmma_desc_sw128(a0 + k * 32), wgmma_desc_sw128(b0 + k * 32));
+        wgmma_commit();
+        wgmma_wait<1>();                                                 // block kb - 1 has retired: free its stage
+        if (kb > 0 && wt == 0) mbar_arrive(&empty[(kb - 1) % STAGES]);
+    }
+    wgmma_wait<0>();
+
+    const int r0 = m0 + wg * 64 + (wt >> 5) * 16 + (lane >> 2);
+    const bool pairs = (N & 1) == 0;                                     // 4-byte aligned column pairs
+#pragma unroll
+    for (int j = 0; j < BN / 4; ++j) {                                   // j = 2 i + h: columns 8 i + .., row r0 + 8 h
+        const int row = r0 + 8 * (j & 1), col = n0 + 8 * (j >> 1) + 2 * (lane & 3);
+        const float v0 = acc[2 * j], v1 = acc[2 * j + 1];
+        if (row < M) {
+            __half* yr = y + (size_t)row * N;
+            const __half* rr = res ? res + (size_t)row * N : nullptr;
+            if (pairs && col + 1 < N) {
+                const float2 bb = bias ? make_float2(bias[col], bias[col + 1]) : make_float2(0.f, 0.f);
+                const float2 rv = epi == 2 ? __half22float2(*reinterpret_cast<const __half2*>(rr + col)) : make_float2(0.f, 0.f);
+                *reinterpret_cast<__half2*>(yr + col) =
+                    __halves2half2(epilogue_value(v0, bb.x, rv.x, epi), epilogue_value(v1, bb.y, rv.y, epi));
+            } else {
+                if (col < N) yr[col] = epilogue_value(v0, bias ? bias[col] : 0.f, epi == 2 ? __half2float(rr[col]) : 0.f, epi);
+                if (col + 1 < N)
+                    yr[col + 1] = epilogue_value(v1, bias ? bias[col + 1] : 0.f, epi == 2 ? __half2float(rr[col + 1]) : 0.f, epi);
+            }
+        }
     }
 }
 

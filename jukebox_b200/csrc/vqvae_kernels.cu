@@ -1140,7 +1140,7 @@ extern "C" int jk_conv1d_cl(const jk_conv_args* a, jk_stream_t stream_) {
     static const bool conv_exact = getenv("JK_CONV_EXACT") != nullptr;      // A/B: keep the FMA tile kernel for flagged convs
     if (a->tensor_cores && !conv_exact && (a->c_in == 32 || a->c_in == 64) && (a->c_out == 32 || a->c_out == 64) &&
         (((uintptr_t)a->in | (uintptr_t)a->out | (uintptr_t)a->bias | (uintptr_t)a->res) & 15) == 0) {
-        // tcgen05 + TMA tap-GEMM (vqvae_t5.cu) for stride-1 inputs of >= 128 positions; JK_CONV_T5=0 keeps the mma.sync kernel
+        // wgmma + TMA tap-GEMM (vqvae_t5.cu) for stride-1 inputs of >= 128 positions; JK_CONV_T5=0 keeps the mma.sync kernel
         static const bool t5 = !(getenv("JK_CONV_T5") && atoi(getenv("JK_CONV_T5")) == 0);
         if (t5 && a->in_stride == 1 && a->n_taps <= 3 && a->t_in >= 128 && a->t_out >= 1)
             return jk::conv_t5(a->in, a->t_in, a->c_in, a->out, a->t_out, a->c_out, a->w, a->bias, a->res, a->n_taps, a->tap_off,
@@ -1195,7 +1195,7 @@ extern "C" int jk_resblock_tc(const float* x, float* out, const float* w1, const
         if (C == 64) return launch_resblock_tc<64>(x, out, w1, b1, w2, b2, n, T, dilation, res_scale, (cudaStream_t)stream);
         if (C == 32) return launch_resblock_tc<32>(x, out, w1, b1, w2, b2, n, T, dilation, res_scale, (cudaStream_t)stream);
     }
-    // tcgen05 + TMA version (vqvae_t5.cu): whole 128-position MMA tiles, TMA needs 16-byte aligned rows.  JK_RESBLOCK_T5=0
+    // wgmma + TMA version (vqvae_t5.cu): whole 128-position MMA tiles, TMA needs 16-byte aligned rows.  JK_RESBLOCK_T5=0
     // keeps the mma.sync kernel (A/B runs).
     static const bool t5 = !(getenv("JK_RESBLOCK_T5") && atoi(getenv("JK_RESBLOCK_T5")) == 0);
     if (t5 && (C == 64 || C == 32) && T >= 128 && (((uintptr_t)x | (uintptr_t)out) & 15) == 0)

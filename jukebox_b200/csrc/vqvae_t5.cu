@@ -1,27 +1,23 @@
-// ResConv1DBlock of the VQ-VAE decoder side on the 5th-generation tensor cores (tcgen05 + TMEM), TMA-staged.
+// ResConv1DBlock of the VQ-VAE decoder side on the Hopper tensor cores (wgmma), TMA-staged.
 //
 //   out = x + res_scale * (W2 . relu(W1 * relu(x) + b1) + b2)        (vqvae/resnet.py:27-44: k3 dilated conv, k1 conv)
 //
 // Channels-last fp32 [N, T, C] in and out, C in {32, 64}.  Same arithmetic as resblock_h2_kernel (vqvae_kernels.cu): every
 // product runs as the split-precision triple  hi.w_hi + lo.w_hi + hi.w_lo  of fp16 halves (hi = fp16(v), lo = fp16(v - hi):
-// 22 significant bits) accumulated in fp32 - but the MMAs are tcgen05.mma.kind::f16 with M = 128 positions per
-// instruction and the accumulators live in TMEM, where mma.sync left the legacy tensor path saturated at 38 % of the
-// elapsed cycles (profiles/ncu_resblock_h2_8warps_r02.txt).
+// 22 significant bits) accumulated in fp32 - but the MMAs are warpgroup MMAs (wgmma m64nCk16) reading both operands
+// from swizzled shared memory, where mma.sync needs a ldmatrix per fragment and leaves the legacy tensor path saturated.
 //
-// One persistent CTA per SM walks tiles of 128 positions; five roles, connected by mbarriers only:
-//   warp 0      TMA producer   cp.async.bulk.tensor.3d of the fp32 rows of one tap, [128 rows x C] of clip n starting at
-//                              t0 + (tap - 1) * dilation, into a 2-stage ring.  Rows outside [0, T) arrive as zeros
-//                              (the tensor map's out-of-bounds fill IS the convolution's zero padding).
-//   warps 2-5   converters     fp32 tap tile -> relu -> hi / lo fp16 planes in the K-major, 128-byte-swizzled layout the
+// One persistent CTA per SM walks tiles of 128 positions; three roles, connected by mbarriers only:
+//   last warp   TMA producer   cp.async.bulk.tensor.3d of the fp32 rows of one tap, [128 rows x C] of clip n starting at
+//                              t0 + (tap - 1) * dilation, into a ring.  Rows outside [0, T) arrive as zeros (the tensor
+//                              map's out-of-bounds fill IS the convolution's zero padding).
+//   warps 8..   converters     fp32 tap tile -> relu -> hi / lo fp16 planes in the K-major, 128-byte-swizzled layout the
 //                              tensor core reads (row r, 16-byte chunk j at r * 128 + ((j ^ (r & 7)) << 4)), 2-stage ring
-//   warp 1      MMA issuer     one thread: per tap C / 16 k-steps x 3 products into accumulator 1 (TMEM, 128 lanes x C
-//                              columns); later the k1 conv (hidden tile . W2) into accumulator 2.  tcgen05.commit
-//                              releases the operand slots / publishes the accumulators.  Accumulators are double
-//                              buffered and conv1 of tile i + 1 is issued BEFORE conv2 of tile i, so the tensor pipe
-//                              works while the epilogue warps produce tile i's hidden tile.
-//   warps 6-9   epilogues      (1) tcgen05.ld accumulator 1 -> relu(acc / 2^8 + b1) -> hi / lo planes of the hidden tile
-//                              (the A operand of the k1 conv); (2) accumulator 2 -> x + res_scale * (acc / 2^8 + b2),
-//                              x exact from global memory (an L2 hit: the centre tap has just been loaded).
+//   warps 0-7   consumers      two warpgroups, rows 0-63 and 64-127 of the tile: per tap C / 16 k-steps x 3 products into
+//                              accumulator 1 (registers); then hidden = relu(acc / 2^8 + b1) split into hi / lo fp16
+//                              pairs IN REGISTERS - the accumulator fragment is the A fragment of the next wgmma - and the
+//                              k1 conv (hidden . W2) into accumulator 2; then x + res_scale * (acc / 2^8 + b2) through a
+//                              shared-memory stage so that the residual loads and the stores are coalesced.
 // W1 / W2 are scaled by 2^8 before the split (undone in the epilogues) so that their fp16 remainders stay out of the
 // subnormal range; both are split and laid out (N-major rows, K contiguous, same swizzle) once per CTA.
 #include "common.cuh"
@@ -35,9 +31,9 @@ namespace {
 #ifndef JK_T5_PREFETCH
 #define JK_T5_PREFETCH 1
 #endif
-constexpr int kBM = 128;                  // positions per tile = MMA M
+constexpr int kBM = 128;                  // positions per tile = two wgmma M blocks of 64
 // converter groups of 4 warps (group g converts the taps whose counter is g mod 2): two for C = 32, one for C = 64
-// (A/B on one box, profiles/resblock_t5_variants_r02.txt); JK_T5_CONV_GROUPS overrides both
+// (C = 64 has no shared memory left for a deeper fp32 ring); JK_T5_CONV_GROUPS overrides both
 template <int C>
 struct T5Groups {
 #ifdef JK_T5_CONV_GROUPS
@@ -52,17 +48,16 @@ template <int C>
 struct T5 {
     static constexpr int kWBlock = C * 128;                 // one K block of a weight plane: C rows x 128 bytes
     static constexpr int kW1 = 3 * kWBlock, kW2 = kWBlock;   // bytes per plane
-    static constexpr int kATile = kBM * 128;                 // one operand plane of a tap / hidden tile (128-byte rows)
+    static constexpr int kATile = kBM * 128;                 // one operand plane of a tap tile (128-byte rows)
     static constexpr int kFTile = kBM * C * 4;               // fp32 tap tile as TMA delivers it
     static constexpr int kFS = C == 64 ? 2 : 4;              // stages of the fp32 ring (what shared memory leaves room for)
     static constexpr int offW1h = 0, offW1l = kW1, offW2h = 2 * kW1, offW2l = 2 * kW1 + kW2;
     static constexpr int offA = 2 * kW1 + 2 * kW2;           // [2 stages][hi | lo]
-    static constexpr int offH = offA + 2 * 2 * kATile;       // hidden tile [hi | lo]
-    static constexpr int offF = offH + 2 * kATile;           // [2 stages] fp32
+    static constexpr int offS = offA + 2 * 2 * kATile;       // output stage [128][C] fp32
+    static constexpr int offF = offS + kBM * C * 4;          // [kFS stages] fp32
     static constexpr int offBias = offF + kFS * kFTile;      // b1, b2
     static constexpr int offBar = offBias + 2 * C * 4;
     static constexpr int smem = offBar + 256;
-    static constexpr int tmem_cols = 4 * C;                  // acc1[2], acc2[2]: 256 / 128 columns
 };
 
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
@@ -71,38 +66,6 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
             smem_u32(smem_dst)),
         "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
         : "memory");
-}
-// K-major operand, 128-byte swizzle, 8-row groups 1024 bytes apart (the encoding prefill_gemm.cu runs on)
-__device__ __forceinline__ uint64_t t5_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-__device__ __forceinline__ void t5_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void t5_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void t5_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
 }
 // two values -> packed hi / lo fp16 pairs (a in the low half); values beyond the fp16 range saturate
 __device__ __forceinline__ void t5_split2(float a, float b, uint32_t& hi, uint32_t& lo) {
@@ -114,38 +77,78 @@ __device__ __forceinline__ void t5_split2(float a, float b, uint32_t& hi, uint32
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // byte offset of 16-byte chunk j of row r inside a K-major 128-byte-swizzled plane
 __device__ __forceinline__ uint32_t sw_off(int r, int j) { return (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((j ^ (r & 7)) << 4)); }
+__device__ __forceinline__ void named_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+// scale * (acc / 2^8 + bias) of one consumer warpgroup's 64 rows -> stage[row][C], 16-byte chunks XOR-swizzled with row & 7
+template <int C>
+__device__ __forceinline__ void stage_rows(float* stage, const float (&acc)[C / 2], const float* bias, float scale, int row0, int lane) {
+#pragma unroll
+    for (int j = 0; j < C / 4; ++j) {                     // j = 2 i + h: columns 8 i + 2 (lane % 4) + {0, 1}, row + 8 h
+        const int row = row0 + 8 * (j & 1), col = 8 * (j >> 1) + 2 * (lane & 3);
+        float2 o;
+        o.x = scale * fmaf(acc[2 * j], kWInvT5, bias[col]);
+        o.y = scale * fmaf(acc[2 * j + 1], kWInvT5, bias[col + 1]);
+        *reinterpret_cast<float2*>(stage + row * C + (((col >> 2) ^ (row & 7)) << 2) + (col & 3)) = o;
+    }
+}
+
+// fp32 tap tile -> (relu) -> hi / lo planes of operand slot s: one converter group of 128 threads (ct = 0..127)
+template <int C>
+__device__ __forceinline__ void convert_tap(const uint8_t* fsrc, uint8_t* ah, int a_tile, int ct, bool relu) {
+    constexpr int CH = C / 4, PER = kBM * CH / 128;         // float4 chunks per row, items per thread
+    const float4* f = reinterpret_cast<const float4*>(fsrc);
+    float4 v[PER];
+#pragma unroll
+    for (int j = 0; j < PER; ++j) v[j] = f[ct + j * 128];
+    uint2 h[PER], l[PER];
+#pragma unroll
+    for (int j = 0; j < PER; ++j) {
+        if (relu) { v[j].x = fmaxf(v[j].x, 0.f); v[j].y = fmaxf(v[j].y, 0.f); v[j].z = fmaxf(v[j].z, 0.f); v[j].w = fmaxf(v[j].w, 0.f); }
+        t5_split2(v[j].x, v[j].y, h[j].x, l[j].x);
+        t5_split2(v[j].z, v[j].w, h[j].y, l[j].y);
+    }
+#pragma unroll
+    for (int j = 0; j < PER; ++j) {
+        const int item = ct + j * 128, r = item / CH, c4 = item % CH;
+        const uint32_t o = sw_off(r, c4 >> 1) + (c4 & 1) * 8;
+        *reinterpret_cast<uint2*>(ah + o) = h[j];
+        *reinterpret_cast<uint2*>(ah + a_tile + o) = l[j];
+    }
+}
+
+// accumulate one tap: C_IN / 16 k-steps x 3 products (lo.w_hi, hi.w_lo, hi.w_hi) of this warpgroup's 64 rows
+template <int CI, int CO>
+__device__ __forceinline__ void mma_tap(float (&acc)[CO / 2], uint32_t ah, uint32_t al, uint32_t bh, uint32_t bl) {
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < CI / 16; ++k) {
+        wgmma_ss<CO>(acc, wgmma_desc_sw128(al + k * 32), wgmma_desc_sw128(bh + k * 32));
+        wgmma_ss<CO>(acc, wgmma_desc_sw128(ah + k * 32), wgmma_desc_sw128(bl + k * 32));
+        wgmma_ss<CO>(acc, wgmma_desc_sw128(ah + k * 32), wgmma_desc_sw128(bh + k * 32));
+    }
+    wgmma_commit();
+}
 
 template <int C>
-__global__ void __launch_bounds__(32 * (2 + 4 * T5Groups<C>::value + 4), 1)
+__global__ void __launch_bounds__(32 * (9 + 4 * T5Groups<C>::value), 1)
 resblock_t5_kernel(const __grid_constant__ CUtensorMap map_x, const float* __restrict__ x, float* __restrict__ out,
                    const float* __restrict__ w1, const float* __restrict__ b1, const float* __restrict__ w2,
                    const float* __restrict__ b2, long long T, int dil, float rs, int tiles_per_clip, int total_tiles) {
     using L = T5<C>;
-    constexpr int kGroups = T5Groups<C>::value, kThreadsT5 = 32 * (2 + 4 * kGroups + 4);
+    constexpr int kGroups = T5Groups<C>::value, kThreadsT5 = 32 * (9 + 4 * kGroups), kProducer = 8 + 4 * kGroups;
     extern __shared__ __align__(1024) uint8_t sm[];
     uint64_t* bars = reinterpret_cast<uint64_t*>(sm + L::offBar);
-    uint64_t *f_full = bars, *f_empty = bars + 4, *a_full = bars + 8, *a_empty = bars + 10, *acc1_full = bars + 12,
-             *acc1_empty = bars + 14, *acc2_full = bars + 16, *acc2_empty = bars + 18, *h_full = bars + 20, *h_empty = bars + 21;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 22);
+    uint64_t *f_full = bars, *f_empty = bars + 4, *a_full = bars + 8, *a_empty = bars + 10;
     constexpr int FS = L::kFS;
     float* bias = reinterpret_cast<float*>(sm + L::offBias);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
-    // ---- once per CTA: barriers, TMEM, weights (scaled, split, swizzled), biases ------------------------------------
+    // ---- once per CTA: barriers, weights (scaled, split, swizzled), biases ------------------------------------------
     if (tid == 0) {
         for (int i = 0; i < FS; ++i) { mbar_init(&f_full[i], 1); mbar_init(&f_empty[i], 128); }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&a_full[i], 128); mbar_init(&a_empty[i], 1);
-            mbar_init(&acc1_full[i], 1); mbar_init(&acc1_empty[i], 128);
-            mbar_init(&acc2_full[i], 1); mbar_init(&acc2_empty[i], 128);
-        }
-        mbar_init(h_full, 128); mbar_init(h_empty, 1);
+        for (int i = 0; i < 2; ++i) { mbar_init(&a_full[i], 128); mbar_init(&a_empty[i], 2); }   // a_empty: one arrival per warpgroup
         mbar_fence_init();
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_x)) : "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(L::tmem_cols));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
     }
     for (int i = tid; i < 3 * C * C; i += kThreadsT5) {        // w1[(tap * C + ci) * C + co] -> B1[tap block][row co][k ci]
         const int tap = i / (C * C), ci = (i / C) % C, co = i % C;
@@ -171,18 +174,15 @@ resblock_t5_kernel(const __grid_constant__ CUtensorMap map_x, const float* __res
     }
     for (int i = tid; i < 2 * C; i += kThreadsT5) bias[i] = i < C ? __ldg(b1 + i) : __ldg(b2 + i - C);
     fence_async_smem();                                       // the weight planes are read by the tensor core (async proxy)
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
     const int first = blockIdx.x, stride = gridDim.x;
 
-    if (warp == 0) {
+    if (warp == kProducer) {
         // ================= TMA producer =================
         if (lane == 0) {
             // the rows of the tiles this CTA takes next are pulled into L2 two iterations ahead (every row is read three times,
             // as the centre tap of one tile and the side taps of two others: whoever comes first pays the HBM latency), so
-            // that the ring's loads are L2 hits - two stages of 32 KB cannot cover an HBM round trip
+            // that the ring's loads are L2 hits - a ring of 64 KB cannot cover an HBM round trip
             auto prefetch = [&](int tile) {
                 if (tile >= total_tiles) return;
                 const int nb = tile / tiles_per_clip, t0 = (tile - nb * tiles_per_clip) * kBM;
@@ -207,184 +207,92 @@ resblock_t5_kernel(const __grid_constant__ CUtensorMap map_x, const float* __res
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        if (lane == 0) {
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(C >> 3) << 17) | ((uint32_t)(kBM >> 4) << 24);
-            const uint32_t w1h = smem_u32(sm + L::offW1h), w1l = smem_u32(sm + L::offW1l);
-            const uint32_t w2h = smem_u32(sm + L::offW2h), w2l = smem_u32(sm + L::offW2l);
-            const uint32_t hh = smem_u32(sm + L::offH), hl = hh + L::kATile;
-            auto conv2 = [&](uint32_t j) {      // k1 conv of tile iteration j: hidden tile . W2 -> accumulator 2
-                const uint32_t p = j & 1;
-                mbar_wait(&acc2_empty[p], ((j >> 1) & 1) ^ 1);
-                mbar_wait(h_full, j & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t d = tmem_base + 2 * C + p * C;
-#pragma unroll
-                for (int k = 0; k < C / 16; ++k) {
-                    t5_mma(d, t5_desc(hl + k * 32), t5_desc(w2h + k * 32), idesc, k ? 1u : 0u);
-                    t5_mma(d, t5_desc(hh + k * 32), t5_desc(w2l + k * 32), idesc, 1u);
-                    t5_mma(d, t5_desc(hh + k * 32), t5_desc(w2h + k * 32), idesc, 1u);
-                }
-                t5_commit(h_empty);
-                t5_commit(&acc2_full[p]);
-            };
-            uint32_t kt = 0, it = 0;
-            for (int tile = first; tile < total_tiles; tile += stride, ++it) {
-                const uint32_t p = it & 1;
-                mbar_wait(&acc1_empty[p], ((it >> 1) & 1) ^ 1);
-                const uint32_t d = tmem_base + p * C;
-                for (int tap = 0; tap < 3; ++tap, ++kt) {
-                    const int s = kt & 1;
-                    mbar_wait(&a_full[s], (kt >> 1) & 1);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t ah = smem_u32(sm + L::offA + s * 2 * L::kATile), al = ah + L::kATile;
-                    const uint32_t bh = w1h + tap * L::kWBlock, bl = w1l + tap * L::kWBlock;
-#pragma unroll
-                    for (int k = 0; k < C / 16; ++k) {
-                        t5_mma(d, t5_desc(al + k * 32), t5_desc(bh + k * 32), idesc, (tap | k) ? 1u : 0u);
-                        t5_mma(d, t5_desc(ah + k * 32), t5_desc(bl + k * 32), idesc, 1u);
-                        t5_mma(d, t5_desc(ah + k * 32), t5_desc(bh + k * 32), idesc, 1u);
-                    }
-                    t5_commit(&a_empty[s]);
-                }
-                t5_commit(&acc1_full[p]);
-                if (it > 0) conv2(it - 1);
-            }
-            if (it > 0) conv2(it - 1);
-        }
-    } else if (warp < 2 + 4 * kGroups) {
+    } else if (warp >= 8) {
         // ================= converters: fp32 tap tile -> relu -> hi / lo planes =================
         // kGroups groups of 128 threads; with two groups, group g takes the taps whose counter is g mod 2 - that is the
         // operand slot g and the fp32 slots g (mod 2) - so two taps are converted concurrently and every barrier still
         // sees exactly the 128 arrivals of one group per use
-        const int cg = (warp - 2) >> 2;
-        const int ct = (tid - 64) & 127;                  // 0..127 inside the group
-        constexpr int CH = C / 4;                         // float4 chunks per row
-        constexpr int PER = kBM * CH / 128;               // items per thread
+        const int cg = (warp - 8) >> 2, ct = tid & 127;
         uint32_t kt = 0;
         for (int tile = first; tile < total_tiles; tile += stride) {
             for (int tap = 0; tap < 3; ++tap, ++kt) {
                 if (kGroups == 2 && (int)(kt & 1) != cg) continue;
                 const int s = kt & 1, fs = kt % FS;
                 mbar_wait(&f_full[fs], (kt / FS) & 1);
-                const float4* f = reinterpret_cast<const float4*>(sm + L::offF + fs * L::kFTile);
-                float4 v[PER];
-#pragma unroll
-                for (int j = 0; j < PER; ++j) v[j] = f[ct + j * 128];
-                uint2 h[PER], l[PER];
-#pragma unroll
-                for (int j = 0; j < PER; ++j) {
-                    t5_split2(fmaxf(v[j].x, 0.f), fmaxf(v[j].y, 0.f), h[j].x, l[j].x);
-                    t5_split2(fmaxf(v[j].z, 0.f), fmaxf(v[j].w, 0.f), h[j].y, l[j].y);
-                }
                 mbar_wait(&a_empty[s], ((kt >> 1) & 1) ^ 1);
-                uint8_t* ah = sm + L::offA + s * 2 * L::kATile;
-#pragma unroll
-                for (int j = 0; j < PER; ++j) {
-                    const int item = ct + j * 128, r = item / CH, c4 = item % CH;
-                    const uint32_t o = sw_off(r, c4 >> 1) + (c4 & 1) * 8;
-                    *reinterpret_cast<uint2*>(ah + o) = h[j];
-                    *reinterpret_cast<uint2*>(ah + L::kATile + o) = l[j];
-                }
-                // The fp32 slot is released only here: every loaded value has been consumed by the stores above (an arrive
-                // issued right behind the loads let TMA refill the slot under them - tools/t5_check.py showed O(1) errors in
-                // single 2-row LDS.128 groups), and the proxy fence below also orders this thread's generic reads of the slot
-                // before the async-proxy writes of the refill.
+                convert_tap<C>(sm + L::offF + fs * L::kFTile, sm + L::offA + s * 2 * L::kATile, L::kATile, ct, true);
+                // The fp32 slot is released only here, after every loaded value has been consumed by the stores above (an
+                // arrive right behind the loads would let TMA refill the slot under them); the proxy fence also orders this
+                // thread's generic reads of the slot before the async-proxy writes of the refill.
                 fence_async_smem();
                 mbar_arrive(&a_full[s]);
                 mbar_arrive(&f_empty[fs]);
             }
         }
     } else {
-        // ================= epilogues =================
-        const int q = warp & 3, row = q * 32 + lane;      // TMEM lane quarter of this warp (warp id mod 4); row of the tile
-        const uint32_t lane_base = tmem_base + ((uint32_t)(q * 32) << 16);
-        uint8_t* hh = sm + L::offH;
-        uint32_t it = 0;
-        for (int tile = first; tile < total_tiles; tile += stride, ++it) {
-            const uint32_t p = it & 1;
+        // ================= consumers: conv1, hidden tile, conv2, output =================
+        const int wg = warp >> 2, wt = tid & 127, row0 = wg * 64 + (wt >> 5) * 16 + (lane >> 2);
+        const uint32_t w1h = smem_u32(sm + L::offW1h), w1l = smem_u32(sm + L::offW1l);
+        const uint32_t w2h = smem_u32(sm + L::offW2h), w2l = smem_u32(sm + L::offW2l);
+        float* stage = reinterpret_cast<float*>(sm + L::offS);
+        constexpr int CH4 = C / 4;
+        uint32_t kt = 0;
+        for (int tile = first; tile < total_tiles; tile += stride) {
             const int nb = tile / tiles_per_clip, t0 = (tile - nb * tiles_per_clip) * kBM;
-            // ---- (1) hidden = relu(conv1 / 2^8 + b1) -> hi / lo planes ------------------------------------------
-            mbar_wait(&acc1_full[p], (it >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            uint32_t hi[C / 2], lo[C / 2];
+            float acc[C / 2];
 #pragma unroll
-            for (int c0 = 0; c0 < C; c0 += 32) {
-                uint32_t r[32];
-                t5_ld32(lane_base + p * C + c0, r);
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                for (int e = 0; e < 32; e += 4) {
-                    const float4 bb = *reinterpret_cast<const float4*>(bias + c0 + e);      // one broadcast LDS.128 per 4 columns
-                    const float a0 = fmaxf(fmaf(__uint_as_float(r[e]), kWInvT5, bb.x), 0.f);
-                    const float a1 = fmaxf(fmaf(__uint_as_float(r[e + 1]), kWInvT5, bb.y), 0.f);
-                    const float a2 = fmaxf(fmaf(__uint_as_float(r[e + 2]), kWInvT5, bb.z), 0.f);
-                    const float a3 = fmaxf(fmaf(__uint_as_float(r[e + 3]), kWInvT5, bb.w), 0.f);
-                    t5_split2(a0, a1, hi[(c0 + e) >> 1], lo[(c0 + e) >> 1]);
-                    t5_split2(a2, a3, hi[((c0 + e) >> 1) + 1], lo[((c0 + e) >> 1) + 1]);
+            for (int i = 0; i < C / 2; ++i) acc[i] = 0.f;
+            for (int tap = 0; tap < 3; ++tap, ++kt) {
+                const int s = kt & 1;
+                mbar_wait(&a_full[s], (kt >> 1) & 1);
+                const uint32_t ah = smem_u32(sm + L::offA + s * 2 * L::kATile) + wg * (64 * 128), al = ah + L::kATile;
+                mma_tap<C, C>(acc, ah, al, w1h + tap * L::kWBlock, w1l + tap * L::kWBlock);
+                if (tap > 0) {                                // the previous tap has retired: free its operand slot
+                    wgmma_wait<1>();
+                    if (wt == 0) mbar_arrive(&a_empty[(kt - 1) & 1]);
                 }
             }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            mbar_arrive(&acc1_empty[p]);
-            mbar_wait(h_empty, (it & 1) ^ 1);
+            wgmma_wait<0>();
+            if (wt == 0) mbar_arrive(&a_empty[(kt - 1) & 1]);
+            // ---- hidden = relu(conv1 / 2^8 + b1) -> hi / lo A fragments of the k1 conv -------------------------------
+            uint32_t hh[C / 16][4], hl[C / 16][4];
 #pragma unroll
-            for (int j = 0; j < C / 8; ++j) {
-                const uint32_t o = sw_off(row, j);
-                *reinterpret_cast<uint4*>(hh + o) = make_uint4(hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3]);
-                *reinterpret_cast<uint4*>(hh + L::kATile + o) = make_uint4(lo[4 * j], lo[4 * j + 1], lo[4 * j + 2], lo[4 * j + 3]);
+            for (int j = 0; j < C / 4; ++j) {                 // j = 2 i + h: register 2 (i & 1) + h of k-step i / 2
+                const int col = 8 * (j >> 1) + 2 * (lane & 3);
+                const float a0 = fmaxf(fmaf(acc[2 * j], kWInvT5, bias[col]), 0.f);
+                const float a1 = fmaxf(fmaf(acc[2 * j + 1], kWInvT5, bias[col + 1]), 0.f);
+                t5_split2(a0, a1, hh[j >> 2][j & 3], hl[j >> 2][j & 3]);
             }
-            fence_async_smem();
-            mbar_arrive(h_full);
-            // ---- (2) out = x + res_scale * (conv2 / 2^8 + b2) ---------------------------------------------------
-            // TMEM hands a thread one ROW of the tile; row-per-lane 16-byte global accesses touch 32 different lines per
-            // instruction and saturated the L1 tag stage (ncu: l1tex 80 % of peak, profiles/ncu_resblock_t5_r02a.txt).
-            // So the tile goes through shared memory: res_scale * (acc / 2^8 + b2) row by row into the hidden-tile region
-            // (free between the k1 conv that just read it and the next tile's hidden tile), then all 128 threads add the
-            // residual and store with consecutive lanes on consecutive 16-byte chunks.
-            constexpr int CH4 = C / 4;
-            const int et = tid - 32 * (2 + 4 * kGroups);      // 0..127
+            // this thread's share of the residual rows of its warpgroup (coalesced), requested while the k1 conv runs
             const float* xin = x + ((size_t)nb * T + t0) * C;
-            // this thread's share of the residual rows (coalesced): the first half is requested before the wait for the k1 conv,
-            // the second while the staged tile settles - off the per-tile chain without spilling (168 registers)
-            float4 xres[CH4];
+            float4 xres[CH4 / 2];
 #pragma unroll
             for (int i = 0; i < CH4 / 2; ++i) {
-                const int item = et + i * 128;
+                const int item = wg * 64 * CH4 + wt + i * 128;
                 xres[i] = ((long long)t0 + item / CH4 < T) ? __ldg(reinterpret_cast<const float4*>(xin) + item) : make_float4(0.f, 0.f, 0.f, 0.f);
             }
-            mbar_wait(&acc2_full[p], (it >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            float* stage = reinterpret_cast<float*>(sm + L::offH);      // [128][C] fp32, 16-byte chunks XOR-swizzled with row & 7
+            // ---- k1 conv: hidden . W2 -------------------------------------------------------------------------------
 #pragma unroll
-            for (int c0 = 0; c0 < C; c0 += 32) {
-                uint32_t r[32];
-                t5_ld32(lane_base + 2 * C + p * C + c0, r);
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+            for (int i = 0; i < C / 2; ++i) acc[i] = 0.f;
+            wgmma_fence();
 #pragma unroll
-                for (int e = 0; e < 32; e += 4) {
-                    const float4 bb = *reinterpret_cast<const float4*>(bias + C + c0 + e);
-                    float4 o;
-                    o.x = rs * fmaf(__uint_as_float(r[e]), kWInvT5, bb.x);
-                    o.y = rs * fmaf(__uint_as_float(r[e + 1]), kWInvT5, bb.y);
-                    o.z = rs * fmaf(__uint_as_float(r[e + 2]), kWInvT5, bb.z);
-                    o.w = rs * fmaf(__uint_as_float(r[e + 3]), kWInvT5, bb.w);
-                    *reinterpret_cast<float4*>(stage + row * C + ((((c0 + e) >> 2) ^ (row & 7)) << 2)) = o;
-                }
+            for (int k = 0; k < C / 16; ++k) {
+                wgmma_rs<C>(acc, hl[k], wgmma_desc_sw128(w2h + k * 32));
+                wgmma_rs<C>(acc, hh[k], wgmma_desc_sw128(w2l + k * 32));
+                wgmma_rs<C>(acc, hh[k], wgmma_desc_sw128(w2h + k * 32));
             }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            mbar_arrive(&acc2_empty[p]);
-#pragma unroll
-            for (int i = CH4 / 2; i < CH4; ++i) {
-                const int item = et + i * 128;
-                xres[i] = ((long long)t0 + item / CH4 < T) ? __ldg(reinterpret_cast<const float4*>(xin) + item) : make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-            asm volatile("bar.sync 1, 128;" ::: "memory");
+            wgmma_commit();
+            wgmma_wait<0>();
+            // ---- out = x + res_scale * (conv2 / 2^8 + b2) -----------------------------------------------------------
+            // a thread holds pieces of two rows; the tile goes through shared memory so that the residual loads and the
+            // stores run with consecutive lanes on consecutive 16-byte chunks
+            stage_rows<C>(stage, acc, bias + C, rs, row0, lane);
+            named_sync(1 + wg);
             {
                 float* xo = out + ((size_t)nb * T + t0) * C;
 #pragma unroll
-                for (int i = 0; i < CH4; ++i) {
-                    const int item = et + i * 128, rr = item / CH4, jj = item % CH4;
+                for (int i = 0; i < CH4 / 2; ++i) {
+                    const int item = wg * 64 * CH4 + wt + i * 128, rr = item / CH4, jj = item % CH4;
                     if ((long long)t0 + rr < T) {
                         const float4 v = *reinterpret_cast<const float4*>(stage + rr * C + ((jj ^ (rr & 7)) << 2));
                         const float4 xr = xres[i];
@@ -392,13 +300,8 @@ resblock_t5_kernel(const __grid_constant__ CUtensorMap map_x, const float* __res
                     }
                 }
             }
-            asm volatile("bar.sync 1, 128;" ::: "memory");      // the region becomes the next tile's hidden tile
+            named_sync(1 + wg);                                // the stage rows are rewritten by the next tile
         }
-    }
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(L::tmem_cols));
     }
 }
 
@@ -406,9 +309,9 @@ resblock_t5_kernel(const __grid_constant__ CUtensorMap map_x, const float* __res
 // Tap-GEMM convolution on the same machinery, for the decoder-side convs BETWEEN the residual blocks (the k3 input conv of
 // a DecoderConvBock, the two 2-tap phases of its k4-s2 transposed convs; encdec.py:28-46):
 //   out[t * os + oo, :] = res + scale * (sum_j x[t + off_j, :] . W_j + b),   c_in, c_out in {32, 64}, <= 3 taps, stride-1 input.
-// Roles as in resblock_t5_kernel minus the hidden tile: TMA producer (one tap tile per load), 4 converter warps, MMA issuer
-// (double-buffered accumulator of CO columns), 4 epilogue warps that stage scale * (acc / 2^8 + b) through shared memory and
-// then add the residual / store whole rows with consecutive lanes on consecutive 16-byte chunks.
+// Roles as in resblock_t5_kernel minus the hidden tile: two consumer warpgroups (warps 0-7) that accumulate in registers
+// and stage scale * (acc / 2^8 + b) through shared memory to add the residual / store whole rows coalesced, 4 converter
+// warps (8-11), one TMA producer warp (12).
 // ---------------------------------------------------------------------------------------
 struct ConvT5P {
     const float* in; float* out; const float* w; const float* bias; const float* res;
@@ -431,36 +334,27 @@ struct T5C {
     static constexpr int offBias = offF + kFS * kFTile;
     static constexpr int offBar = offBias + CO * 4;
     static constexpr int smem = offBar + 256;
-    static constexpr int tmem_cols = 2 * CO < 32 ? 32 : 2 * CO;     // 64 or 128: a power of two >= 32
 };
+constexpr int kConvThreads = 416;
 
 template <int CI, int CO>
-__global__ void __launch_bounds__(320, 1)
+__global__ void __launch_bounds__(kConvThreads, 1)
 conv_t5_kernel(const __grid_constant__ CUtensorMap map_x, ConvT5P P, int tiles_per_clip, int total_tiles) {
     using L = T5C<CI, CO>;
     constexpr int FS = L::kFS;
     extern __shared__ __align__(1024) uint8_t sm[];
     uint64_t* bars = reinterpret_cast<uint64_t*>(sm + L::offBar);
-    uint64_t *f_full = bars, *f_empty = bars + 4, *a_full = bars + 8, *a_empty = bars + 10, *acc_full = bars + 12,
-             *acc_empty = bars + 14;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
+    uint64_t *f_full = bars, *f_empty = bars + 4, *a_full = bars + 8, *a_empty = bars + 10;
     float* bias = reinterpret_cast<float*>(sm + L::offBias);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int ntap = P.n_taps;
     if (tid == 0) {
         for (int i = 0; i < FS; ++i) { mbar_init(&f_full[i], 1); mbar_init(&f_empty[i], 128); }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&a_full[i], 128); mbar_init(&a_empty[i], 1);
-            mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 128);
-        }
+        for (int i = 0; i < 2; ++i) { mbar_init(&a_full[i], 128); mbar_init(&a_empty[i], 2); }
         mbar_fence_init();
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_x)) : "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(L::tmem_cols));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    for (int i = tid; i < ntap * CI * CO; i += 320) {         // w[(tap * CI + ci) * CO + co] -> B[tap][row co][k ci]
+    for (int i = tid; i < ntap * CI * CO; i += kConvThreads) {  // w[(tap * CI + ci) * CO + co] -> B[tap][row co][k ci]
         const int tap = i / (CI * CO), ci = (i / CO) % CI, co = i % CO;
         unsigned short h, l;
         const float v = kWScaleT5 * __ldg(P.w + i);
@@ -471,15 +365,12 @@ conv_t5_kernel(const __grid_constant__ CUtensorMap map_x, ConvT5P P, int tiles_p
         *reinterpret_cast<unsigned short*>(sm + L::offWh + o) = h;
         *reinterpret_cast<unsigned short*>(sm + L::offWl + o) = l;
     }
-    for (int i = tid; i < CO; i += 320) bias[i] = P.bias ? __ldg(P.bias + i) : 0.f;
+    for (int i = tid; i < CO; i += kConvThreads) bias[i] = P.bias ? __ldg(P.bias + i) : 0.f;
     fence_async_smem();
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
     const int first = blockIdx.x, stride = gridDim.x;
 
-    if (warp == 0) {
+    if (warp == 12) {
         if (lane == 0) {
             uint32_t kt = 0;
             for (int tile = first; tile < total_tiles; tile += stride) {
@@ -493,103 +384,53 @@ conv_t5_kernel(const __grid_constant__ CUtensorMap map_x, ConvT5P P, int tiles_p
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(CO >> 3) << 17) | ((uint32_t)(kBM >> 4) << 24);
-            const uint32_t wh = smem_u32(sm + L::offWh), wl = smem_u32(sm + L::offWl);
-            uint32_t kt = 0, it = 0;
-            for (int tile = first; tile < total_tiles; tile += stride, ++it) {
-                const uint32_t p = it & 1;
-                mbar_wait(&acc_empty[p], ((it >> 1) & 1) ^ 1);
-                const uint32_t d = tmem_base + p * CO;
-                for (int tap = 0; tap < ntap; ++tap, ++kt) {
-                    const int s = kt & 1;
-                    mbar_wait(&a_full[s], (kt >> 1) & 1);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t ah = smem_u32(sm + L::offA + s * 2 * L::kATile), al = ah + L::kATile;
-                    const uint32_t bh = wh + tap * L::kWBlock, bl = wl + tap * L::kWBlock;
-#pragma unroll
-                    for (int k = 0; k < CI / 16; ++k) {
-                        t5_mma(d, t5_desc(al + k * 32), t5_desc(bh + k * 32), idesc, (tap | k) ? 1u : 0u);
-                        t5_mma(d, t5_desc(ah + k * 32), t5_desc(bl + k * 32), idesc, 1u);
-                        t5_mma(d, t5_desc(ah + k * 32), t5_desc(bh + k * 32), idesc, 1u);
-                    }
-                    t5_commit(&a_empty[s]);
-                }
-                t5_commit(&acc_full[p]);
-            }
-        }
-    } else if (warp < 6) {
-        const int ct = tid - 64;
-        constexpr int CH = CI / 4, PER = kBM * CH / 128;
+    } else if (warp >= 8) {
+        const int ct = tid & 127;
         const bool relu = P.relu_in != 0;
         uint32_t kt = 0;
         for (int tile = first; tile < total_tiles; tile += stride) {
             for (int tap = 0; tap < ntap; ++tap, ++kt) {
                 const int s = kt & 1, fs = kt % FS;
                 mbar_wait(&f_full[fs], (kt / FS) & 1);
-                const float4* f = reinterpret_cast<const float4*>(sm + L::offF + fs * L::kFTile);
-                float4 v[PER];
-#pragma unroll
-                for (int j = 0; j < PER; ++j) v[j] = f[ct + j * 128];
-                uint2 h[PER], l[PER];
-#pragma unroll
-                for (int j = 0; j < PER; ++j) {
-                    if (relu) { v[j].x = fmaxf(v[j].x, 0.f); v[j].y = fmaxf(v[j].y, 0.f); v[j].z = fmaxf(v[j].z, 0.f); v[j].w = fmaxf(v[j].w, 0.f); }
-                    t5_split2(v[j].x, v[j].y, h[j].x, l[j].x);
-                    t5_split2(v[j].z, v[j].w, h[j].y, l[j].y);
-                }
                 mbar_wait(&a_empty[s], ((kt >> 1) & 1) ^ 1);
-                uint8_t* ah = sm + L::offA + s * 2 * L::kATile;
-#pragma unroll
-                for (int j = 0; j < PER; ++j) {
-                    const int item = ct + j * 128, r = item / CH, c4 = item % CH;
-                    const uint32_t o = sw_off(r, c4 >> 1) + (c4 & 1) * 8;
-                    *reinterpret_cast<uint2*>(ah + o) = h[j];
-                    *reinterpret_cast<uint2*>(ah + L::kATile + o) = l[j];
-                }
+                convert_tap<CI>(sm + L::offF + fs * L::kFTile, sm + L::offA + s * 2 * L::kATile, L::kATile, ct, relu);
                 fence_async_smem();
                 mbar_arrive(&a_full[s]);
                 mbar_arrive(&f_empty[fs]);          // only now: the loaded values have been consumed (see resblock_t5_kernel)
             }
         }
     } else {
-        const int q = warp & 3, row = q * 32 + lane, et = tid - 192;
-        const uint32_t lane_base = tmem_base + ((uint32_t)(q * 32) << 16);
+        const int wg = warp >> 2, wt = tid & 127, row0 = wg * 64 + (wt >> 5) * 16 + (lane >> 2);
+        const uint32_t wh = smem_u32(sm + L::offWh), wl = smem_u32(sm + L::offWl);
         float* stage = reinterpret_cast<float*>(sm + L::offS);
         const long long rows_out = P.t_out * P.out_stride;
-        uint32_t it = 0;
-        for (int tile = first; tile < total_tiles; tile += stride, ++it) {
-            const uint32_t p = it & 1;
+        uint32_t kt = 0;
+        for (int tile = first; tile < total_tiles; tile += stride) {
             const int nb = tile / tiles_per_clip, t0 = (tile - nb * tiles_per_clip) * kBM;
-            mbar_wait(&acc_full[p], (it >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+            float acc[CO / 2];
 #pragma unroll
-            for (int c0 = 0; c0 < CO; c0 += 32) {
-                uint32_t r[32];
-                t5_ld32(lane_base + p * CO + c0, r);
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                for (int e = 0; e < 32; e += 4) {
-                    const float4 bb = *reinterpret_cast<const float4*>(bias + c0 + e);
-                    float4 o;
-                    o.x = P.scale * fmaf(__uint_as_float(r[e]), kWInvT5, bb.x);
-                    o.y = P.scale * fmaf(__uint_as_float(r[e + 1]), kWInvT5, bb.y);
-                    o.z = P.scale * fmaf(__uint_as_float(r[e + 2]), kWInvT5, bb.z);
-                    o.w = P.scale * fmaf(__uint_as_float(r[e + 3]), kWInvT5, bb.w);
-                    *reinterpret_cast<float4*>(stage + row * CO + ((((c0 + e) >> 2) ^ (row & 7)) << 2)) = o;
+            for (int i = 0; i < CO / 2; ++i) acc[i] = 0.f;
+            for (int tap = 0; tap < ntap; ++tap, ++kt) {
+                const int s = kt & 1;
+                mbar_wait(&a_full[s], (kt >> 1) & 1);
+                const uint32_t ah = smem_u32(sm + L::offA + s * 2 * L::kATile) + wg * (64 * 128), al = ah + L::kATile;
+                mma_tap<CI, CO>(acc, ah, al, wh + tap * L::kWBlock, wl + tap * L::kWBlock);
+                if (tap > 0) {
+                    wgmma_wait<1>();
+                    if (wt == 0) mbar_arrive(&a_empty[(kt - 1) & 1]);
                 }
             }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            mbar_arrive(&acc_empty[p]);
-            asm volatile("bar.sync 1, 128;" ::: "memory");
+            wgmma_wait<0>();
+            if (wt == 0) mbar_arrive(&a_empty[(kt - 1) & 1]);
+            stage_rows<CO>(stage, acc, bias, P.scale, row0, lane);
+            named_sync(1 + wg);
             {
                 constexpr int CH4 = CO / 4;
                 float* ob = P.out + (size_t)nb * rows_out * CO;
                 const float* rb = P.res ? P.res + (size_t)nb * rows_out * CO : nullptr;
 #pragma unroll 4
-                for (int i = 0; i < CH4; ++i) {
-                    const int item = et + i * 128, rr = item / CH4, jj = item % CH4;
+                for (int i = 0; i < CH4 / 2; ++i) {
+                    const int item = wg * 64 * CH4 + wt + i * 128, rr = item / CH4, jj = item % CH4;
                     const long long t = (long long)t0 + rr;
                     if (t < P.t_out) {
                         float4 v = *reinterpret_cast<const float4*>(stage + rr * CO + ((jj ^ (rr & 7)) << 2));
@@ -602,13 +443,8 @@ conv_t5_kernel(const __grid_constant__ CUtensorMap map_x, ConvT5P P, int tiles_p
                     }
                 }
             }
-            asm volatile("bar.sync 1, 128;" ::: "memory");
+            named_sync(1 + wg);
         }
-    }
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(L::tmem_cols));
     }
 }
 
@@ -653,7 +489,7 @@ int launch_t5(const float* x, float* out, const float* w1, const float* b1, cons
     const long long per_clip = (T + kBM - 1) / kBM, total = per_clip * n;
     JK_REQUIRE(total < (1ll << 31) && T + 4096 < (1ll << 31), "clip too long for 32-bit tile coordinates");
     const unsigned grid = (unsigned)std::min<long long>(total, sms[dev & 63]);
-    resblock_t5_kernel<C><<<grid, 32 * (2 + 4 * T5Groups<C>::value + 4), T5<C>::smem, stream>>>(map, x, out, w1, b1, w2, b2, T, dil, rs, (int)per_clip, (int)total);
+    resblock_t5_kernel<C><<<grid, 32 * (9 + 4 * T5Groups<C>::value), T5<C>::smem, stream>>>(map, x, out, w1, b1, w2, b2, T, dil, rs, (int)per_clip, (int)total);
     JK_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -684,7 +520,7 @@ int launch_conv_t5(const ConvT5P& P, int n, cudaStream_t stream) {
     const long long per_clip = (P.t_out + kBM - 1) / kBM, total = per_clip * n;
     JK_REQUIRE(total < (1ll << 31) && P.t_in + 4096 < (1ll << 31), "clip too long for 32-bit tile coordinates");
     const unsigned grid = (unsigned)std::min<long long>(total, sms[dev & 63]);
-    conv_t5_kernel<CI, CO><<<grid, 320, T5C<CI, CO>::smem, stream>>>(map, P, (int)per_clip, (int)total);
+    conv_t5_kernel<CI, CO><<<grid, kConvThreads, T5C<CI, CO>::smem, stream>>>(map, P, (int)per_clip, (int)total);
     JK_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -128,7 +128,7 @@ class DecodeEngine:
         return out.value
 
     def prefill(self, n, n_positions, *, tokens=None, y_cond=None, x_cond=None, h_out=None):
-        """positions 0..n_positions-1 of all samples through every layer at once (tcgen05 GEMMs);
+        """positions 0..n_positions-1 of all samples through every layer at once (wgmma GEMMs);
         afterwards the engine is at position n_positions."""
         a = _lib.PrefillArgs()
         a.n_samples, a.n_positions = n, n_positions

@@ -170,6 +170,15 @@ TINY_PRIORS = {
 }
 
 
+# logit columns stored per position of a tiny prior: a seeded sample of the vocabulary (all positions, all samples), so that
+# each fixture stays under 1 MB; `pred_cols` holds the column indices and the tests index their own logits with it
+PRED_COLS = 512
+
+
+def sample_cols(bins, seed):
+    return np.sort(np.random.RandomState(seed).choice(bins, min(bins, PRED_COLS), replace=False)).astype(np.int64)
+
+
 def golden_simple_prior(tag, bs=2, seed=4, chunk_size=7):
     from jukebox.hparams import setup_hparams
     from jukebox.make_models import make_vqvae, make_prior
@@ -222,6 +231,8 @@ def golden_simple_prior(tag, bs=2, seed=4, chunk_size=7):
             if enc_kv is not None:
                 arrays["encoder_kv32"] = enc_kv
                 arrays["encoder_kv16"] = enc_kv16.float()
+    cols = sample_cols(arrays["preds32"].shape[-1], seed)
+    arrays.update(pred_cols=cols, preds32=arrays["preds32"][..., cols], preds16=arrays["preds16"][..., cols])
     cfg = dict(tag=tag, vq_name=vq_name, vq_over=vq_over, pr_name=pr_name, pr_over=pr_over, seed=seed,
                chunk_size=chunk_size, n_ctx=int(prior.n_ctx), single_enc_dec=bool(prior.single_enc_dec))
     save(f"prior_{tag}", cfg, named, **arrays)

@@ -32,6 +32,11 @@ class Fixture:
         return sd
 
 
+def logit_cols(fx, a):
+    """the stored logit columns of a fixture that keeps a sample of the vocabulary (`pred_cols`), else all of them"""
+    return a[..., fx["pred_cols"]] if "pred_cols" in fx else a
+
+
 def rel_err(a, b):
     """max|a-b| / max|b|  (the metric SURVEY.md section 8d defines for logits)."""
     a = np.asarray(a, np.float64)

@@ -1,5 +1,5 @@
 """Host-side planning of the decode engine (jk_prior_plan: pure arithmetic, no GPU): K-split units, column ownership,
-shared-memory budget - for the BASELINE configurations on a 148-SM device."""
+shared-memory budget - for the BASELINE configurations on a 132-SM device (H100 SXM)."""
 import ctypes as C
 
 import numpy as np
@@ -19,7 +19,7 @@ CONFIGS = {
 }
 
 
-def plan(name, sms=148):
+def plan(name, sms=132):
     w, depth, heads, n_ctx, blocks, order, prime, enc, bins, mb, _ = CONFIGS[name]
     cfg = _lib.PriorConfig()
     cfg.width, cfg.depth, cfg.heads, cfg.n_state, cfg.mlp_width = w, depth, heads, w // 4, w
@@ -39,7 +39,7 @@ def plan(name, sms=148):
 def test_units_partition_every_conv1d(name):
     cfg, info, cols = plan(name)
     assert info.k_split == CONFIGS[name][-1]
-    assert info.units * info.k_split == 148
+    assert info.units * info.k_split == 132
     assert 2 <= info.ring_slots <= 12 and info.smem_bytes <= 232448
     S, W, M = cfg.n_state, cfg.width, cfg.mlp_width
     for l in range(cfg.depth):
@@ -70,5 +70,5 @@ def test_plan_rejects_bad_geometry():
     cfg, _, _ = plan("tiny")
     cfg.n_state = 24                                             # not a multiple of 16
     info = _lib.PlanInfo()
-    assert _lib.lib().jk_prior_plan(C.byref(cfg), 148, C.byref(info), None, 0) != 0
+    assert _lib.lib().jk_prior_plan(C.byref(cfg), 132, C.byref(info), None, 0) != 0
     assert b"multiples of 16" in _lib.lib().jk_last_error()

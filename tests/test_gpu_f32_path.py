@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-from golden_util import Fixture, rel_err
+from golden_util import Fixture, logit_cols, rel_err
 from test_gpu_transformer import build
 from test_gpu_prior import _load, _cuda, _make_prior
 
@@ -156,7 +156,7 @@ def test_simple_prior_z_forward(tag):
         upto = int(diff[0]) + 1 if diff.numel() else upto
         assert upto > prior.n_tokens
     loss, metrics = prior.z_forward(z, z_conds, y, fp16=False, get_preds=True)
-    preds = metrics["preds"].cpu().numpy()
+    preds = logit_cols(fx, metrics["preds"].cpu().numpy())
     e = rel_err(preds[:, :upto], fx["preds32"][:, :upto])
     print(f"prior_{tag}: z_forward fp32 logits vs reference {e:.2e}; loss {float(loss):.4f} bits")
     assert e < TOL32

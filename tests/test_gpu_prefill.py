@@ -1,4 +1,4 @@
-"""Chunked prefill (jk_prior_prefill: tcgen05 GEMMs over all given positions) against stepping the same
+"""Chunked prefill (jk_prior_prefill: wgmma GEMMs over all given positions) against stepping the same
 tokens one by one through the decode kernel - the equality the reference asserts in its own
 check_chunks (prior/autoregressive.py:330-338) - and against the oracle."""
 import numpy as np
@@ -9,8 +9,8 @@ from golden_util import rel_err
 
 pytestmark = pytest.mark.gpu
 
-# widths are 256 so that every GEMM K (width, n_state = width/4, mlp) is a multiple of the tcgen05 K block;
-# the two paths share every fp16 rounding point and differ in fp32 summation order (TMEM accumulator
+# widths are 256 so that every GEMM K (width, n_state = width/4, mlp) is a multiple of the GEMM K block;
+# the two paths share every fp16 rounding point and differ in fp32 summation order (register accumulator
 # over K blocks vs 8 warps x k16 partials), i.e. the noise floor documented in test_gpu_prior.py
 TOL = 3e-3
 
@@ -59,7 +59,7 @@ CASES = [
     (12, 256, 16, 2, 96, 8, 24, 61),    # given tokens run past the prime and past several blocks (ring layouts)
     (2, 256, 6, 1, 64, 4, None, 33),    # upsampler-like stack, one head
     (0, 256, 3, 4, 48, None, None, 17),  # dense
-    (2, 320, 6, 2, 64, 4, None, 33),    # K tail: n_state 80 is not a multiple of the 64-wide tcgen05 K block (5b: 1200, upsamplers: 480)
+    (2, 320, 6, 2, 64, 4, None, 33),    # K tail: n_state 80 is not a multiple of the 64-wide GEMM K block (5b: 1200, upsamplers: 480)
     (2, 256, 6, 1, 1024, 8, None, 700),  # a long run of given tokens (continuation windows re-prime thousands)
     (2, 4800, 3, 8, 64, 4, None, 33),   # 5b_lyrics geometry: n_state 1200, head_dim 150 - head rows are not 16-byte aligned
     (0, 1024, 2, 1, 160, None, None, 150),  # head_dim 256, dense: several key tiles per query tile

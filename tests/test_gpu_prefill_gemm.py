@@ -1,4 +1,4 @@
-"""tcgen05 + TMA prefill Conv1D (jk_conv1d_prefill_f16) against an fp32 torch reference of the same op."""
+"""wgmma + TMA prefill Conv1D (jk_conv1d_prefill_f16) against an fp32 torch reference of the same op."""
 import ctypes as C
 
 import pytest

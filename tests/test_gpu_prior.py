@@ -4,7 +4,7 @@ import numpy as np
 import pytest
 import torch
 
-from golden_util import Fixture, rel_err
+from golden_util import Fixture, logit_cols, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -103,7 +103,7 @@ def test_simple_prior_conditioning_and_logits(tag):
                 assert e < 4e-3
             _, preds = prior.prior.primed_sample(bs, tokens[:, :-1].clone(), x_cond, y_cond, enc_kv, fp16=True,
                                                  get_preds=True)
-    p = preds.cpu().numpy()
+    p = logit_cols(fx, preds.cpu().numpy())
     e16, e32, ref = rel_err(p, fx["preds16"]), rel_err(p, fx["preds32"]), rel_err(fx["preds16"], fx["preds32"])
     print(f"prior_{tag}: logits vs reference fp16 {e16:.2e}, vs fp32 {e32:.2e} (reference fp16 vs fp32 {ref:.2e})")
     assert e16 < TOL_LOGITS

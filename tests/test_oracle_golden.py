@@ -92,7 +92,7 @@ def test_torch_restatement_is_the_reference_on_the_same_device(tag):
     torch operators, so in fp32 it must reproduce the reference's CPU outputs to 2e-6 on any host.  In fp16 the result
     depends on the host's half-precision GEMM blocking: on the host that wrote the fixtures it is bit-identical up to
     5e-4, on another CPU model (this container has been re-created on different hosts) it shows the same 1.4e-3 ...
-    2.2e-3 order noise that profiles/parity_r02.txt measures on the GPU - hence the 3e-3 bound here."""
+    2.2e-3 order noise that tests/test_gpu_fullsize_golden.py measures on the GPU - hence the 3e-3 bound here."""
     import torch
     from oracle.transformer_torch import TorchDecodeOracle
     fx = Fixture(f"transformer_{tag}")

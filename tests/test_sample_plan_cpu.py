@@ -1,72 +1,35 @@
 """Window planning / stitching of jukebox_b200.sample against the UNMODIFIED reference's own loop
-(jukebox/sample.py:17-96), both driven with the same recording dummy prior on the CPU.  Skipped when the reference
-tree is absent (GPU box)."""
+(jukebox/sample.py:17-96), both driven with the same recording dummy prior on the CPU.  The reference's results
+are stored in tests/golden/sample_level.json (oracle/make_golden_sample_plan.py)."""
 import itertools
+import json
+import os
 
 import pytest
-import torch
 
-from oracle.ref_import import reference_available, load_reference
+from golden_util import GOLDEN
+from oracle.make_golden_sample_plan import CASES, case_key, run_case
 from jukebox_b200.sample import plan_windows, Window
 from jukebox_b200.utils.sample_utils import get_starts
 
-
-class RecordingPrior:
-    """prior.sample appends tokens that encode (call index, position), and records how it was called"""
-
-    def __init__(self, n_ctx):
-        self.n_ctx = n_ctx
-        self.calls = []
-
-    def get_z_conds(self, zs, start, end):
-        return None
-
-    def get_y(self, labels, start):
-        return None
-
-    def sample(self, n_samples, z=None, z_conds=None, y=None, sample_tokens=None, **kw):
-        total = self.n_ctx if sample_tokens is None else sample_tokens
-        self.calls.append((n_samples, z.shape[1], total, tuple(sorted(kw))))
-        new = total - z.shape[1]
-        assert new > 0
-        fresh = 1000 * len(self.calls) + torch.arange(z.shape[1], total).view(1, -1).repeat(n_samples, 1)
-        return torch.cat([z, fresh], dim=1)
+with open(os.path.join(GOLDEN, "sample_level.json")) as _f:
+    REF = json.load(_f)
 
 
-class Hps(dict):
-    __getattr__ = dict.__getitem__
-
-
-CASES = [(total, n_ctx, hop, have, bs, mbs)
-         for total, n_ctx, hop in [(40, 16, 8), (40, 16, 4), (16, 16, 8), (37, 16, 12), (10, 16, 8), (5, 16, 8), (33, 16, 16)]
-         for have in (0, 3, 11, 16, 20) for bs, mbs in ((3, 2), (4, 4))]
-
-
-@pytest.mark.skipif(not reference_available(), reason="reference tree not present")
 @pytest.mark.parametrize("total,n_ctx,hop,have,bs,mbs", CASES)
 def test_sample_level_matches_reference(total, n_ctx, hop, have, bs, mbs):
-    load_reference()
-    import jukebox.sample as ref
     import jukebox_b200.sample as ours
     if total >= n_ctx and have > total:
         pytest.skip("more tokens than the level holds")
-    outs = []
-    for mod in (ref, ours):
-        prior = RecordingPrior(n_ctx)
-        zs = [torch.arange(have).view(1, -1).repeat(bs, 1)]
-        hps = Hps(n_samples=bs)
-        kw = dict(temp=0.9, fp16=True, max_batch_size=mbs)
-        try:
-            zs = mod.sample_level(zs, None, kw, 0, prior, total, hop, hps)
-            outs.append((zs[0].clone(), prior.calls))
-        except Exception as e:          # both sides must fail alike (e.g. negative slices)
-            outs.append(("error", type(e).__name__))
-    if outs[0][0] == "error" if isinstance(outs[0][0], str) else False:
-        assert isinstance(outs[1][0], str)
+    case = (total, n_ctx, hop, have, bs, mbs)
+    ref = REF[case_key(case)]
+    got = json.loads(json.dumps(run_case(ours.sample_level, case)))     # tuples -> lists, as stored
+    if "error" in ref:
+        assert "error" in got, got
         return
-    assert not isinstance(outs[1][0], str), outs[1]
-    assert torch.equal(outs[0][0], outs[1][0])
-    assert outs[0][1] == outs[1][1]
+    assert "error" not in got, got
+    assert got["codes"] == ref["codes"]
+    assert got["calls"] == ref["calls"]
 
 
 def test_plan_windows_shapes():

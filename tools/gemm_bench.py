@@ -1,4 +1,4 @@
-"""Throughput of the tcgen05 prefill Conv1D at the 5b_lyrics c_enc_kv shape (and a square shape), CUDA events."""
+"""Throughput of the wgmma prefill Conv1D at the 5b_lyrics c_enc_kv shape (and a square shape), CUDA events."""
 import json
 import os
 import sys

@@ -1,4 +1,4 @@
-// Micro-benchmarks that inform the decode-engine design (B200): legacy HMMA latency/throughput,
+// Micro-benchmarks that inform the decode-engine design: legacy HMMA latency/throughput,
 // ldmatrix latency, L2 load latency (hit / written-by-another-SM), grid barrier round trip.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>

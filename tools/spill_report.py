@@ -16,7 +16,7 @@ if len(sys.argv) > 1:
 else:
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     o = "/tmp/jk_decode_engine_spill.o"
-    subprocess.run(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
+    subprocess.run(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
                     "-c", os.path.join(root, "jukebox_b200", "csrc", "decode_engine.cu"), "-o", o], check=True)
 sass=subprocess.run(f"cuobjdump -sass {o}", shell=True, capture_output=True, text=True).stdout.splitlines()
 st=[i for i,l in enumerate(sass) if 'Function : ' in l and 'jk_decode_step' in l][0]

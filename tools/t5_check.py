@@ -1,4 +1,4 @@
-"""tcgen05 residual block: bitwise batch independence (n = 4 in one call vs four calls of n = 1), run-to-run determinism and
+"""wgmma residual block: bitwise batch independence (n = 4 in one call vs four calls of n = 1), run-to-run determinism and
 the error pattern against the exact-FMA kernel, by tile row."""
 import os
 import sys
