@@ -83,13 +83,15 @@ typedef struct jk_prior jk_prior;   /* opaque; lives in the caller's arena */
 
 /* How the engine would lay a configuration out on a device with `n_sms` SMs - pure host arithmetic, no device needed
  * (the CPU tests use it; the engine itself always plans for the current device).  cols (optional, uint16 pairs
- * [units][depth][4][2]) receives (first 8-column group, number of groups) of every unit for the four Conv1Ds of a layer. */
+ * [units][depth][4][2]) receives (first 8-column group, number of groups) of every unit for the four Conv1Ds of a layer,
+ * followed by the same pairs of the logits GEMM, [logits_passes][units][2]. */
 typedef struct jk_prior_plan_info {
     int32_t k_split;          /* CTAs per unit: they share the unit's columns and split K                 */
     int32_t units;            /* n_sms / k_split                                                          */
     int32_t ring_slots;       /* 16 KB weight-ring slots per SM                                           */
     int32_t smem_bytes;       /* dynamic shared memory of the decode kernel                               */
     int32_t tile_rows;        /* K/V rows per attention tile                                              */
+    int32_t logits_passes;    /* passes of the tensor-core logits GEMM (0: fp32 FMA logits)               */
     uint64_t arena_bytes;
     uint64_t stream_stride;   /* bytes of the longest per-SM weight stream (+ padding)                    */
 } jk_prior_plan_info;

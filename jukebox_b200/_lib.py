@@ -31,7 +31,8 @@ class LayerWeights(C.Structure):
 
 class PlanInfo(C.Structure):
     _fields_ = [("k_split", C.c_int32), ("units", C.c_int32), ("ring_slots", C.c_int32), ("smem_bytes", C.c_int32),
-                ("tile_rows", C.c_int32), ("arena_bytes", C.c_uint64), ("stream_stride", C.c_uint64)]
+                ("tile_rows", C.c_int32), ("logits_passes", C.c_int32), ("arena_bytes", C.c_uint64),
+                ("stream_stride", C.c_uint64)]
 
 
 class F32Layer(C.Structure):

@@ -56,9 +56,6 @@ using namespace jk;
 #ifndef JK_SKIP_FOREIGN_WAIT
 #define JK_SKIP_FOREIGN_WAIT 1
 #endif
-#ifndef JK_SHFL_STATS
-#define JK_SHFL_STATS 1
-#endif
 #ifndef JK_LOGITS_MMA
 #define JK_LOGITS_MMA 1
 #endif
@@ -422,7 +419,8 @@ struct LogitsRec {
     long long lg_bs;
     const float* lb;            // logit bias of this position or NULL
     long long lb_bs;
-    ushort2 cols;               // column groups of this unit
+    unsigned long long* xp;     // partial-sum exchange of the current pass: xp[pass]
+    ushort2 cols;               // column groups of this unit in the current pass
 };
 __device__ __forceinline__ LogitsRec* sm_lrec() { return reinterpret_cast<LogitsRec*>(jk_smem + 7744); }
 
@@ -456,7 +454,7 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
             g.bias = LD.b_2; g.ln_out = lnb + 1024; g.flag_out = fl + 1; g.kind = 2; g.kin = M;
         } else {       // EPI_LOGITS: [y | y] x [hi(x_out) ; lo(x_out)], see the kernel
             const LogitsRec* lr = sm_lrec();
-            g.in = E->ll_h; g.out = nullptr; g.xp = E->xp[0]; g.K = 2 * W; g.N = E->bins; g.g0 = lr->cols.x; g.ncg = lr->cols.y;
+            g.in = E->ll_h; g.out = nullptr; g.xp = lr->xp; g.K = 2 * W; g.N = E->bins; g.g0 = lr->cols.x; g.ncg = lr->cols.y;
             g.bias = nullptr; g.kind = 2; g.kin = W; g.flag_out = 0;
             g.lg_out = lr->lg_out; g.lg_bs = lr->lg_bs; g.lb = lr->lb; g.lb_bs = lr->lb_bs;
         }
@@ -603,94 +601,6 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
     const bool two_rows = ppc <= 16;
     const int pl = two_rows ? (lane & 15) : lane;
     const int b_first = two_rows ? 2 * warp + (lane >> 4) : warp, b_step = two_rows ? 16 : 8;
-#if JK_SHFL_STATS
-    {
-        // LayerNorm statistics of the rows this epilogue writes (residual epilogues): a row's column pairs sit in one half
-        // warp (or one warp), so the CTA's contribution to the row is reduced with shuffles and published by one lane with
-        // one red per moment - integer adds, so still order independent - straight from the epilogue: no scratch in shared
-        // memory, no serial summing loop, no CTA barriers around it, and the words are on their way ~0.2 us earlier.
-        const bool active = pl < ppc;
-        const int pr = rank * ppc + (active ? pl : 0);  // pair inside the unit
-        const int gc = g.g0 * 8 + 2 * pr;               // global column of the pair
-        const float2 bias = (active && g.bias) ? *reinterpret_cast<const float2*>(g.bias + gc) : make_float2(0.f, 0.f);
-        // warp-uniform trip count (the two half warps of the 16-pair layout hold rows 2w and 2w + 1; only the row index
-        // differs), so that the shuffles below run under the constant full mask: a run-time member mask compiles to
-        // WARPSYNC.COLLECTIVE, which cost 3.5 us per residual epilogue
-        const int bw0 = two_rows ? 2 * warp : warp;
-#pragma unroll 1
-        for (int bw = bw0; bw < B; bw += b_step) {
-            const int b = bw + (two_rows ? (lane >> 4) : 0);
-            const bool valid = b < B;
-            long long fs = 0, fq = 0;
-            if (active && valid) {
-                float s0 = 0.f, s1 = 0.f;
-                if (KS == 1) {
-                    for (int w = 0; w < nwarp; ++w) {
-                        const float2 v = *reinterpret_cast<const float2*>(red + (size_t)(w * 16 + b) * ncp + 2 * pr);
-                        s0 += v.x; s1 += v.y;
-                    }
-                } else {
-                    ulonglong2 v[4];
-                    unsigned spins = 0;
-                    bool again;
-                    do {
-                        again = false;
-#pragma unroll
-                        for (int q = 0; q < 4; ++q)
-                            if (q < KS) v[q] = ll_ld2(xp_unit + ((size_t)q * 16 + b) * kXpCols + 2 * pr);
-#pragma unroll
-                        for (int q = 0; q < 4; ++q)
-                            if (q < KS) again |= !(ll_ok(v[q].x, g.flag_in) && ll_ok(v[q].y, g.flag_in));
-                        if (again) spin_guard(spins);
-                    } while (again);
-#pragma unroll
-                    for (int q = 0; q < 4; ++q)
-                        if (q < KS) { s0 += __uint_as_float((uint32_t)v[q].x); s1 += __uint_as_float((uint32_t)v[q].y); }
-                }
-                const float y0 = h2f_round(s0 + bias.x), y1 = h2f_round(s1 + bias.y);     // Conv1D output, rounded once to fp16
-                __half2 o;
-                if (epi == EPI_QKV) {
-                    o = __floats2half2_rn(y0, y1);
-                } else if (epi == EPI_FC) {                        // quick_gelu (transformer/ops.py:33-35)
-                    o = __floats2half2_rn(quick_gelu_f(y0), quick_gelu_f(y1));
-                } else if (epi != EPI_LOGITS) {
-                    // EPI_PROJ : x1 = fp16(h + a)      EPI_PROJ2 : h = fp16(x1 + m)   (transformer.py:82-83)
-                    const float2 base = res[b * 32 + pl];
-                    const float o0 = h2f_round(base.x + y0), o1 = h2f_round(base.y + y1);
-                    res[b * 32 + pl] = make_float2(o0, o1);
-                    o = __floats2half2_rn(o0, o1);
-                    fs = fx_sum(o0) + fx_sum(o1);
-                    fq = fx_sq(o0) + fx_sq(o1);
-                }
-                if (epi == EPI_LOGITS) {       // fp32 logits (autoregressive.py:226-229): no bias, no rounding
-                    float* lo_ = g.lg_out + (size_t)b * g.lg_bs + gc;      // the caller's strides need not be even
-                    const float* lb_ = g.lb ? g.lb + (size_t)b * g.lb_bs + gc : nullptr;
-                    // bins need not be a multiple of 8 (1b_lyrics: 2127): the last column group is padded with zero weights
-                    if (gc < N) lo_[0] = s0 + (lb_ ? lb_[0] : 0.f);
-                    if (gc + 1 < N) lo_[1] = s1 + (lb_ ? lb_[1] : 0.f);
-                } else {
-                    ll_st(g.out + (size_t)b * (N >> 1) + (gc >> 1), *reinterpret_cast<const uint32_t*>(&o), g.flag_out);
-                }
-            }
-            if (residual) {
-#pragma unroll
-                for (int o = 16; o; o >>= 1) {
-                    if (o < 16 || !two_rows) {
-                        fs += __shfl_xor_sync(0xffffffffu, fs, o);
-                        fq += __shfl_xor_sync(0xffffffffu, fq, o);
-                    }
-                }
-                if (pl == 0 && valid) {
-                    red_add_u64(g.ln_out + 16 * b, (1ull << kCntShift) + (unsigned long long)(kSumBias + fs));
-                    red_add_u64(g.ln_out + 16 * b + 1, (1ull << kCntShift) + (unsigned long long)fq);
-                }
-            }
-        }
-    }
-    STAMP(E, g.pslot, 4);
-    consumer_sync();                       // red region is reused by the next phase
-    return ring;
-#endif
     if (pl < ppc) {
         const int pr = rank * ppc + pl;                 // pair inside the unit
         const int gc = g.g0 * 8 + 2 * pr;               // global column of the pair
@@ -1262,9 +1172,10 @@ __device__ __noinline__ void producer_loop(const EngineDev* E, Ring ring, int do
             }
         }
     }
-    if (do_logits == 2) {       // logits GEMM: one more Conv1D in the stream
-        const int ncg = E->lg_cols[u].y;
-        if (ncg) {
+    if (do_logits == 2) {       // logits GEMM: one more Conv1D per pass in the stream
+        for (int p = 0; p < E->lg_np; ++p) {
+            const int ncg = E->lg_cols[p * E->U + u].y;
+            if (ncg == 0) continue;
             const int nkk = ((2 * E->W) >> E->ks_shift) >> 4, kpc = kpc_of(ncg);
             for (int kk0 = 0; kk0 < nkk; kk0 += kpc) {
                 const int nk = min(kpc, nkk - kk0);
@@ -1656,17 +1567,31 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
     }
     if (wants_logits(A) && logits_on_mma(A)) {
         // logits GEMM: [y | y] (the final residual stream, fp16-exact) x [hi(x_out) ; lo(x_out)] on the tensor cores, through
-        // the same phase code as every Conv1D; the K-split partial sums (hi and lo halves on different ranks) meet in fp32
+        // the same phase code as every Conv1D; the K-split partial sums (hi and lo halves on different ranks) meet in fp32.
+        // Pass p exchanges its partial sums through xp[p], so no pass overwrites words the unit still polls for the pass
+        // before it.  A CTA writes xp[p] (p >= 1) only after its epilogue of pass p - 1 has read the partials of every rank
+        // of its unit: every CTA of the unit is then past the last layer, whose words in xp[p] have all been read.  Each
+        // pass stages [y | y] again: the cross-warp reduction of the previous pass overwrote the tile.
+        // The passes are unrolled (at most 4, compute_layout): a rolled loop around the call made ptxas spill in gemm_phase.
         stage_map_init(2, (2 * E->W) >> E->ks_shift);
-        consumer_sync();
-        if (tid == 0) {
-            LogitsRec* lr = sm_lrec();
-            lr->lg_out = A.logits + (size_t)launch_pos() * A.logits_tstride; lr->lg_bs = A.logits_bstride;
-            lr->lb = (E->add_cond_after && A.x_cond) ? A.logit_bias + (size_t)launch_pos() * A.lb_tstride : nullptr; lr->lb_bs = A.lb_bstride;
-            lr->cols = E->lg_cols[cta_unit()];
+        auto pass_record = [&](int p) {
+            consumer_sync();
+            if (tid == 0) {
+                LogitsRec* lr = sm_lrec();
+                lr->lg_out = A.logits + (size_t)launch_pos() * A.logits_tstride; lr->lg_bs = A.logits_bstride;
+                lr->lb = (E->add_cond_after && A.x_cond) ? A.logit_bias + (size_t)launch_pos() * A.lb_tstride : nullptr; lr->lb_bs = A.lb_bstride;
+                lr->cols = E->lg_cols[p * E->U + cta_unit()];
+                lr->xp = E->xp[p];
+            }
+            consumer_sync();
+        };
+#pragma unroll
+        for (int p = 0; p < 4; ++p) {
+            if (p < E->lg_np) {
+                pass_record(p);
+                ring = gemm_phase(ring, B, EPI_LOGITS, E->depth - 1, (int)nph + p, launch_fbase() + (uint32_t)E->depth + 1);
+            }
         }
-        consumer_sync();
-        ring = gemm_phase(ring, B, EPI_LOGITS, E->depth - 1, (int)nph, launch_fbase() + (uint32_t)E->depth + 1);
     } else if (wants_logits(A)) {
         logits_phase(A, ring, c, launch_pos(), launch_fbase() + (uint32_t)E->depth + 1);
     }
@@ -1736,14 +1661,15 @@ __global__ void pack_gemm_kernel(const T* __restrict__ src, int K, int N, uint8_
 
 // logits GEMM: x_out [bins][W] fp32 -> the same per-CTA fragment streams with K' = 2 W: rows k' < W hold hi = fp16(w),
 // rows k' >= W hold lo = fp16(w - hi) (hi + lo carries 22 significant bits; y is an fp16 value, so y.hi + y.lo is the
-// fp32 product up to 2^-22).  Appended to every CTA's stream after the last layer (lg_goff).
+// fp32 product up to 2^-22).  Appended to every CTA's stream after the last layer (lg_goff), one block per pass:
+// grid (G, passes).
 __global__ void pack_logits_kernel(const float* __restrict__ x_out, int W, int bins, uint8_t* streams,
                                    unsigned long long stream_stride, const ushort2* lg_cols, const uint32_t* lg_goff, int KS) {
-    const int c = blockIdx.x;
-    const ushort2 cg = lg_cols[c / KS];
+    const int c = blockIdx.x, p = blockIdx.y, G = gridDim.x;
+    const ushort2 cg = lg_cols[p * (G / KS) + c / KS];
     const int g0 = cg.x, ncg = cg.y;
     if (ncg == 0) return;
-    uint8_t* dst = streams + (size_t)c * stream_stride + (size_t)lg_goff[c] * 16;
+    uint8_t* dst = streams + (size_t)c * stream_stride + (size_t)lg_goff[p * G + c] * 16;
     const int nkk = ((2 * W) / KS) >> 4, kk_first = (c % KS) * nkk;
     const int total = nkk * ncg * 32;
     for (int i = threadIdx.x; i < total; i += blockDim.x) {
@@ -1822,7 +1748,7 @@ struct Layout {
     std::vector<ushort2> cols;
     std::vector<uint32_t> goff;
     std::vector<int> lrow;
-    int lg_on;                          // logits GEMM planned: its column groups / stream offsets close `cols` / `goff`
+    int lg_on, lg_np;                   // logits GEMM planned, in lg_np passes: its column groups / stream offsets close `cols` / `goff`
     std::vector<size_t> cache_off;      // per layer (K); V follows
     std::vector<size_t> cache_bytes;
     std::vector<int> cache_rows;
@@ -1920,29 +1846,36 @@ int compute_layout(const jk_prior_config& c, int G, Layout& L) {
         }
     }
     // logits GEMM (fifth Conv1D, K' = 2 * width: hi and lo fp16 halves of the fp32 x_out): planned when the K-split is even
-    // (a rank's K slice must not straddle the hi / lo boundary), the doubled slice fits the activation tile and no unit
-    // gets more than 8 column groups.  Its records are appended to `cols` ([U] entries) and `goff` ([G] entries).
-    L.lg_on = 0;
+    // (a rank's K slice must not straddle the hi / lo boundary) and the doubled slice fits the activation tile.  A unit
+    // multiplies at most 8 column groups per pass (the partial-sum exchange holds 64 columns); wider vocabularies take more
+    // passes, each with its own exchange buffer, so at most 4 (1b_lyrics on 132 SMs: 266 groups over 33 units, 2 passes).
+    // Its records are appended to `cols` ([passes][U] entries) and `goff` ([passes][G] entries), pass after pass.
+    L.lg_on = 0; L.lg_np = 0;
     {
         const int groups = (c.bins + 7) / 8;           // a ragged last group is padded with zero weights
         const int Kp = 2 * c.width;
+        const int np = ((groups + U - 1) / U + 7) / 8;
         const bool ok = c.bins > 0 && KS >= 2 && (Kp / 16) % KS == 0 && c.width % (Kp / KS) == 0 &&
-                        (size_t)16 * (Kp / KS + 8) * 2 <= (size_t)65536 && (groups + U - 1) / U <= 8 && !getenv("JK_NO_LOGITS_MMA");
-        L.cols.resize((size_t)U * depth * 4 + U, make_ushort2(0, 0));
-        L.goff.resize((size_t)G * depth * 4 + G, 0);
+                        (size_t)16 * (Kp / KS + 8) * 2 <= (size_t)65536 && np <= 4 && !getenv("JK_NO_LOGITS_MMA");
         if (ok) {
-            L.lg_on = 1;
+            L.lg_on = 1; L.lg_np = np;
+            L.cols.resize((size_t)U * depth * 4 + (size_t)np * U, make_ushort2(0, 0));
+            L.goff.resize((size_t)G * depth * 4 + (size_t)np * G, 0);
             const int base = groups / U, extra = groups % U;
             std::vector<int> n(U, base);
             for (int i = 0; i < U; ++i) order[i] = i;
             std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return cum[a] < cum[b]; });
             for (int i = 0; i < extra; ++i) n[order[i]] += 1;
-            int g0 = 0;
-            for (int u = 0; u < U; ++u) {
-                L.cols[(size_t)U * depth * 4 + u] = make_ushort2((unsigned short)g0, (unsigned short)n[u]);
-                for (int r = 0; r < KS; ++r) L.goff[(size_t)G * depth * 4 + u * KS + r] = (uint32_t)(cum[u] / 16);
-                cum[u] += (unsigned long long)n[u] * (Kp / KS / 16) * 256ull;
-                g0 += n[u];
+            // pass p of unit u: the next min(8, rest) groups of the unit's contiguous range
+            std::vector<int> g0(U, 0);
+            for (int u = 1; u < U; ++u) g0[u] = g0[u - 1] + n[u - 1];
+            for (int p = 0; p < np; ++p) {
+                for (int u = 0; u < U; ++u) {
+                    const int k = std::max(0, std::min(8, n[u] - 8 * p));
+                    L.cols[(size_t)U * depth * 4 + (size_t)p * U + u] = make_ushort2((unsigned short)(g0[u] + 8 * p), (unsigned short)k);
+                    for (int r = 0; r < KS; ++r) L.goff[(size_t)G * depth * 4 + (size_t)p * G + u * KS + r] = (uint32_t)(cum[u] / 16);
+                    cum[u] += (unsigned long long)k * (Kp / KS / 16) * 256ull;
+                }
             }
         }
     }
@@ -2071,9 +2004,10 @@ extern "C" int jk_prior_plan(const jk_prior_config* cfg, int n_sms, jk_prior_pla
     int rc = compute_layout(*cfg, n_sms, L);
     if (rc) return rc;
     out->k_split = L.KS; out->units = L.U; out->ring_slots = L.nslot; out->smem_bytes = L.smem_bytes; out->tile_rows = L.RC;
+    out->logits_passes = L.lg_np;
     out->arena_bytes = (uint64_t)L.total; out->stream_stride = (uint64_t)L.stream_stride;
     if (cols) {
-        const size_t ncols = (size_t)L.U * cfg->depth * 4;       // the layers' records (the logits GEMM's follow in L.cols)
+        const size_t ncols = L.cols.size();                       // the layers' records, then the logits GEMM's
         JK_REQUIRE(cols_len >= ncols * 2, "cols buffer too small: %zu < %zu", cols_len, ncols * 2);
         for (size_t i = 0; i < ncols; ++i) { cols[2 * i] = L.cols[i].x; cols[2 * i + 1] = L.cols[i].y; }
     }
@@ -2120,6 +2054,7 @@ extern "C" int jk_prior_create(const jk_prior_config* cfg, void* arena, size_t a
     p->d_goff = (uint32_t*)(A + L.off_goff);
     E.lrow0 = (const int*)(A + L.off_lrow);
     E.lg_on = L.lg_on; p->lg_on = L.lg_on;
+    E.lg_np = L.lg_np; p->lg_np = L.lg_np;
     E.lg_cols = (const ushort2*)(A + L.off_cols) + (size_t)L.U * cfg->depth * 4;
     E.lg_goff = (const uint32_t*)(A + L.off_goff) + (size_t)G * cfg->depth * 4;
     E.streams = A + L.off_streams; E.stream_stride = L.stream_stride;
@@ -2269,7 +2204,7 @@ extern "C" int jk_prior_set_embeddings(jk_prior* p, const float* x_emb, const fl
     p->host.x_emb = x_emb; p->host.pos_emb = pos_emb; p->host.x_out = x_out; p->host.start_token = start_token;
     JK_CHECK_CUDA(cudaMemcpy(p->dev, &p->host, sizeof(EngineDev), cudaMemcpyHostToDevice));
     if (p->lg_on && x_out) {       // logits GEMM: hi / lo fp16 fragment streams of x_out, behind every CTA's last layer
-        pack_logits_kernel<<<p->G, 256>>>(x_out, p->cfg.width, p->cfg.bins, (uint8_t*)p->host.streams, p->host.stream_stride,
+        pack_logits_kernel<<<dim3(p->G, p->lg_np), 256>>>(x_out, p->cfg.width, p->cfg.bins, (uint8_t*)p->host.streams, p->host.stream_stride,
                                           p->host.lg_cols, p->host.lg_goff, p->host.KS);
         JK_CHECK_CUDA(cudaGetLastError());
         JK_CHECK_CUDA(cudaDeviceSynchronize());

@@ -42,8 +42,9 @@ struct EngineDev {
     const float *x_emb, *pos_emb, *x_out, *start_token;
     const int* lrow0;               // [G+1] logits rows per CTA (prefix)
     // logits as a fifth Conv1D on the tensor cores (decode_engine.cu "logits GEMM"): 0 when the configuration keeps
-    // the fp32 FMA path; column groups per unit [U] and stream offsets per CTA [G] (16-byte units)
-    int lg_on;
+    // the fp32 FMA path.  It runs in lg_np passes of at most 8 column groups per unit (the partial-sum exchange holds 64
+    // columns): column groups per unit [lg_np][U] and stream offsets per CTA [lg_np][G] (16-byte units)
+    int lg_on, lg_np;
     const ushort2* lg_cols;
     const uint32_t* lg_goff;
     LayerDev layer[JK_MAX_DEPTH];
@@ -67,7 +68,7 @@ struct jk_prior {
     int t_host;
     std::vector<ushort2> cols;       // [U][depth][4]
     std::vector<uint32_t> goff;      // [G][depth][4] per-GEMM stream offsets (16-B units)
-    int lg_on;                       // logits GEMM planned (engine.cuh)
+    int lg_on, lg_np;                // logits GEMM planned, and its passes (EngineDev)
     uint32_t* d_goff;
     ushort2* d_cols;
     // arena sub-allocations for per-layer small params

@@ -44,7 +44,7 @@ def main():
     funcs = [l.attn_func for l in ca.transformer._attn_mods]
     pos = min(args.pos, L - 8)
     eng.reset(pos)
-    rows = []
+    rows, clocks = [], []
     for i in range(6):
         eng.step(n, tokens=toks, y_cond=yc, x_cond=xc, logits=lbuf, logit_bias=lb)
         torch.cuda.synchronize()
@@ -52,7 +52,13 @@ def main():
         stamps = prof[: 2 + 5 * depth + 1].astype(np.float64)
         if i >= 2:
             rows.append(np.diff(stamps))
+            # SM clock of this step: CTA 0 enters the proj Conv1D of layer l (clock64 stamp, slot 3 + 5 l) right after it
+            # stamps the end of the attention phase (globaltimer, same slot); the first and the last layer span the step
+            p2 = eng.debug_buffer(6).view(torch.int64).cpu().numpy().reshape(-1, 8).astype(np.float64)
+            a, b = 3, 3 + 5 * (depth - 1)
+            clocks.append((p2[b, 0] - p2[a, 0]) / (stamps[b] - stamps[a]) * 1e3)
     d = np.mean(rows, 0) / 1e3          # us
+    mhz = float(np.mean(clocks))
     print(f"position {pos}, n={n}, depth={depth}: kernel total {d.sum():.1f} us")
     print(f"  embed                : {d[0]:8.2f} us")
     names = ["LN+QKV gemm", "attention", "proj gemm", "LN+FC gemm+gelu", "proj2 gemm"]
@@ -66,7 +72,7 @@ def main():
     print(f"  per layer            : {per.sum(1).mean():8.2f} us")
     # intra-phase stamps of CTA 0 (SM clock cycles): slot = phase index
     p2 = eng.debug_buffer(6).view(torch.int64).cpu().numpy().reshape(-1, 8).astype(np.float64)
-    mhz = 1965.0
+    print(f"  SM clock measured over the step: {mhz:.0f} MHz (min {min(clocks):.0f}, max {max(clocks):.0f} over {len(clocks)} steps)")
     print("  CTA 0, GEMM phases (us): wait+stage | mma+weights | reduce+publish partials | exchange+epilogue")
     for j, nm in ((0, "LN+QKV"), (2, "proj"), (3, "LN+FC"), (4, "proj2")):
         rows = []
@@ -76,10 +82,12 @@ def main():
             rows.append([(s1 - s0), (s2 - s1), (s3 - s2), (s4 - s3)])
         r = np.mean(rows, 0) / mhz
         print(f"     {nm:8s}: {r[0]:6.2f} | {r[1]:6.2f} | {r[2]:6.2f} | {r[3]:6.2f}")
-    sl = 1 + 5 * depth                 # the logits GEMM (when the engine plans one) stamps the slot after the last layer
-    if p2[sl, 4] > p2[sl, 0] > 0:
+    # the logits GEMM (when the engine plans one) stamps the slots after the last layer, one per pass
+    for ip, sl in enumerate(range(1 + 5 * depth, 1 + 5 * depth + 4)):
+        if not p2[sl, 4] > p2[sl, 0] > 0:
+            break
         s0, s1, s2, s3, s4 = p2[sl, :5]
-        print(f"     logits  : {(s1 - s0) / mhz:6.2f} | {(s2 - s1) / mhz:6.2f} | {(s3 - s2) / mhz:6.2f} | {(s4 - s3) / mhz:6.2f}   "
+        print(f"     logits {ip}: {(s1 - s0) / mhz:6.2f} | {(s2 - s1) / mhz:6.2f} | {(s3 - s2) / mhz:6.2f} | {(s4 - s3) / mhz:6.2f}   "
               f"(polled loads in at {(p2[sl, 6] - s0) / mhz:5.2f})")
     print("  CTA 0, staging detail (us from phase entry): statistics ready | own polled loads in | past the statistics barrier | staged + barrier")
     for j, nm in ((0, "LN+QKV"), (2, "proj"), (3, "LN+FC"), (4, "proj2")):
