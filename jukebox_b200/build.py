@@ -36,7 +36,7 @@ def _digest():
 
 
 def build_variant(out, defines):
-    """A/B builds (tools/build_variants.sh): the library with extra -D flags, written to `out` (variants/*.so)."""
+    """A/B builds: the library with extra -D flags, written to `out` (variants/*.so)."""
     cmd = [_nvcc()] + NVCC_FLAGS + ["-D" + d for d in defines] + [os.path.join(CSRC, s) for s in SOURCES] + ["-o", out]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:

@@ -22,17 +22,17 @@
 //     L2 round trip instead of release-counter + acquire-poll + data load, and arrival skew is absorbed word
 //     by word.  Flags are unique per (step, layer), nothing is ever reset.
 //   * LayerNorm statistics need all columns of a row: producers add sum / sum-of-squares of their columns
-//     into 64-bit fixed-point accumulators (exact, order independent) and release-add an arrival counter;
-//     the LN consumers acquire it.  These two all-to-all points per layer are also what makes buffer reuse
-//     safe (see "hazards" below).
+//     into 64-bit fixed-point words (exact, order independent) whose top bits count the contributing CTAs;
+//     the LN consumers poll the words until the count says every CTA has added.  These two all-to-all points
+//     per layer are also what makes buffer reuse safe (see "hazards" below).
 //   * the residual stream never leaves the SM: the CTA that finishes columns c of proj finishes the same
 //     columns of proj2 (and of the embedding), so h / x1 slices live in shared memory.
 //   * KV caches are laid out per attention pattern so that the rows a token attends are one contiguous run
 //     (transpose-block layers store position p at row (p % bc)*blocks + p / bc).
 //
 // Hazards.  A buffer written once per layer may be overwritten for layer l+1 only after every reader of layer
-// l is done.  Every writer first passes an LN statistics wait of layer l+1 (acquire of a counter all G CTAs
-// release-add to AFTER their previous phases, in program order), so all reads of layer l happen-before it.
+// l is done.  Every writer first passes an LN statistics wait of layer l+1 (a statistics word all G CTAs add to
+// AFTER their previous phases, in program order), so all reads of layer l happen-before it.
 // The partial-sum exchange has one buffer per Conv1D index for the same reason.
 //
 // Numerics: activations fp16, accumulation fp32, LayerNorm/softmax fp32 - see oracle/transformer_np.py.
@@ -45,23 +45,6 @@
 #include <math.h>
 
 using namespace jk;
-
-// build-time variants (A/B runs: tools/build_variants.sh); the defaults are the measured winners
-#ifndef JK_MMA_ALL_WARPS
-#define JK_MMA_ALL_WARPS 1
-#endif
-#ifndef JK_QKV_POLL_BATCH
-#define JK_QKV_POLL_BATCH 1
-#endif
-#ifndef JK_SKIP_FOREIGN_WAIT
-#define JK_SKIP_FOREIGN_WAIT 1
-#endif
-#ifndef JK_LOGITS_MMA
-#define JK_LOGITS_MMA 1
-#endif
-#ifndef JK_ATTN_LL_MERGE
-#define JK_ATTN_LL_MERGE 1
-#endif
 
 namespace {
 
@@ -97,26 +80,76 @@ struct StepArgs {
     long long lb_bstride, lb_tstride;
 };
 
+// per-launch record of the logits GEMM in the shared-memory header (written by the kernel before each pass)
+struct LogitsRec {
+    float* lg_out;              // logits of this position
+    long long lg_bs;
+    const float* lb;            // logit bias of this position or NULL
+    long long lb_bs;
+    unsigned long long* xp;     // partial-sum exchange of the current pass: xp[pass]
+    ushort2 cols;               // column groups of this unit in the current pass
+};
+// values of a launch in the shared-memory header (written once by the kernel prologue, see launch_pos())
+struct LaunchVals {
+    int pm, pd;                 // p % block_ctx, p / block_ctx
+    int gmax;                   // CTAs available per (sample, head)
+    int t;                      // position p
+    unsigned step;              // steps executed before this launch
+};
+// thread layout of the activation staging for one K (see stage_map_init)
+struct StageDim {
+    int cw, rgc;
+};
+
 // The one dynamic shared-memory block of the decode kernel.  Every device function derives its
 // pointers from this symbol (never from pointer parameters): that is what lets the compiler emit
 // LDS/STS/ATOMS instead of generic LD/ST (measured: generic loads of the B fragments made the MMA loop
 // 6x slower than the tensor pipe allows).
-//   [0, 192)      ring mbarriers          [256, 512)    LN row statistics + flags
-//   [512, 1024)   descriptor head         [1024, 1536)  two layer records (+ column assignment at +128)
-//   [2048, 6144)  residual-stream slice of this CTA: [16][32] float2
-//   [6144, 7704)  thread layouts of the activation staging (stage_map_init)
 extern __shared__ __align__(1024) uint8_t jk_smem[];
-__device__ __forceinline__ uint64_t* sm_full() { return reinterpret_cast<uint64_t*>(jk_smem); }
-__device__ __forceinline__ uint64_t* sm_empty() { return reinterpret_cast<uint64_t*>(jk_smem) + kMaxSlots; }
-__device__ __forceinline__ float* sm_stats() { return reinterpret_cast<float*>(jk_smem + 256); }
-__device__ __forceinline__ float2* sm_res() { return reinterpret_cast<float2*>(jk_smem + 2048); }
+
+// Its header [0, kHeaderBytes): byte offset and size of every region, in address order.  Only the accessors below
+// address the header.
+constexpr int kHdrBar = 0, kHdrBarBytes = 2 * kMaxSlots * 8;           // ring mbarriers: full[kMaxSlots], empty[kMaxSlots]
+constexpr int kHdrStats = 256, kHdrStatsBytes = 16 * 2 * 4;            // LayerNorm statistics [16 rows] {-mean * rstd, rstd}
+constexpr int kHdrDesc = 512, kHdrDescBytes = 512;                     // descriptor head: EngineDev up to `layer`
+constexpr int kHdrLayer = 1024, kHdrLayerSlot = 256;                   // two layer slots (layer l in slot l & 1): LayerDev,
+constexpr int kHdrColsAt = 128;                                        //   and at +kHdrColsAt this unit's ushort2 cols[4]
+constexpr int kHdrRes = 2048, kHdrResBytes = 16 * 32 * 8;              // residual-stream slice of this CTA: [16][32] float2
+constexpr int kHdrMap = 6144, kHdrMapBytes = 3 * kConsumers * 2;       // staging thread layouts [3 kinds][kConsumers]
+constexpr int kHdrMapDim = 7680, kHdrMapDimBytes = 3 * (int)sizeof(StageDim);
+constexpr int kHdrLaunch = 7712, kHdrLaunchBytes = (int)sizeof(LaunchVals);
+constexpr int kHdrLrec = 7744, kHdrLrecBytes = (int)sizeof(LogitsRec);
+static_assert(offsetof(EngineDev, layer) <= kHdrDescBytes, "descriptor head must fit its shared-memory slot");
+static_assert(sizeof(LayerDev) <= kHdrColsAt && kHdrColsAt + 4 * sizeof(ushort2) <= kHdrLayerSlot,
+              "layer record and column assignment must fit their shared-memory slot");
+static_assert(kHdrBar + kHdrBarBytes <= kHdrStats && kHdrStats + kHdrStatsBytes <= kHdrDesc &&
+              kHdrDesc + kHdrDescBytes <= kHdrLayer && kHdrLayer + 2 * kHdrLayerSlot <= kHdrRes &&
+              kHdrRes + kHdrResBytes <= kHdrMap && kHdrMap + kHdrMapBytes <= kHdrMapDim &&
+              kHdrMapDim + kHdrMapDimBytes <= kHdrLaunch && kHdrLaunch + kHdrLaunchBytes <= kHdrLrec &&
+              kHdrLrec + kHdrLrecBytes <= kHeaderBytes,
+              "shared-memory header regions overlap or exceed kHeaderBytes");
+
+__device__ __forceinline__ uint64_t* sm_full() { return reinterpret_cast<uint64_t*>(jk_smem + kHdrBar); }
+__device__ __forceinline__ uint64_t* sm_empty() { return sm_full() + kMaxSlots; }
+__device__ __forceinline__ float* sm_stats() { return reinterpret_cast<float*>(jk_smem + kHdrStats); }
+__device__ __forceinline__ float2* sm_res() { return reinterpret_cast<float2*>(jk_smem + kHdrRes); }
 __device__ __forceinline__ uint8_t* sm_uni() { return jk_smem + kHeaderBytes; }
 // The engine descriptor lives in global memory; with the shared-memory carve-out at its maximum there is
 // no L1 to cache it, so every `E->field` was an L2 round trip (~300 cycles) on the dependency chain.
 // The head of the descriptor (everything before the per-layer array) and the current / next layer
 // records are therefore copied into shared memory once and read with LDS.
-__device__ __forceinline__ const EngineDev* sm_E() { return reinterpret_cast<const EngineDev*>(jk_smem + 512); }
-__device__ __forceinline__ const LayerDev* sm_layer(int i) { return reinterpret_cast<const LayerDev*>(jk_smem + 1024 + 256 * (i & 1)); }
+__device__ __forceinline__ uint32_t* sm_desc_words() { return reinterpret_cast<uint32_t*>(jk_smem + kHdrDesc); }
+__device__ __forceinline__ const EngineDev* sm_E() { return reinterpret_cast<const EngineDev*>(jk_smem + kHdrDesc); }
+__device__ __forceinline__ uint8_t* sm_layer_slot(int l) { return jk_smem + kHdrLayer + kHdrLayerSlot * (l & 1); }
+__device__ __forceinline__ const LayerDev* sm_layer(int l) { return reinterpret_cast<const LayerDev*>(sm_layer_slot(l)); }
+// (first 8-column group, number of groups) of this unit in layer l's QKV, proj, fc and proj2
+__device__ __forceinline__ ushort2* sm_cols(int l) { return reinterpret_cast<ushort2*>(sm_layer_slot(l) + kHdrColsAt); }
+__device__ __forceinline__ unsigned short* sm_stage_map(int kind) {
+    return reinterpret_cast<unsigned short*>(jk_smem + kHdrMap + 2 * kConsumers * kind);
+}
+__device__ __forceinline__ StageDim* sm_stage_dim(int kind) { return reinterpret_cast<StageDim*>(jk_smem + kHdrMapDim) + kind; }
+__device__ __forceinline__ LaunchVals* sm_launch() { return reinterpret_cast<LaunchVals*>(jk_smem + kHdrLaunch); }
+__device__ __forceinline__ LogitsRec* sm_lrec() { return reinterpret_cast<LogitsRec*>(jk_smem + kHdrLrec); }
 
 // Position in the weight ring.  Only the slot and its parity travel (in registers) through the phase calls; the slot
 // count and slot 0's offset are per-launch constants read from the descriptor in shared memory where they are needed, so
@@ -175,13 +208,6 @@ __device__ __forceinline__ bool ll_ok(unsigned long long w, uint32_t flag) { ret
 __device__ __forceinline__ void spin_guard(unsigned& spins) {
     if (++spins > (1u << 24)) __trap();     // a protocol bug traps instead of hanging the GPU
 }
-// one LL word, polled
-__device__ __forceinline__ uint32_t ll_wait1(const unsigned long long* p, uint32_t flag) {
-    unsigned spins = 0;
-    unsigned long long w = ll_ld1(p);
-    while (!ll_ok(w, flag)) { spin_guard(spins); w = ll_ld1(p); }
-    return (uint32_t)w;
-}
 // a statistics word whose count field says every CTA has contributed
 __device__ __forceinline__ unsigned long long wait_stat_word(const long long* p, int G) {
     unsigned spins = 0;
@@ -239,16 +265,16 @@ __device__ __forceinline__ void publish_stats(long long* ln_out, int B, int ppc)
 // Rows >= B are never written: an MMA output row depends only on its own A row, and those outputs are discarded.
 // How the 256 consumer threads tile a [16 rows][Ks / 8 vectors] slice: cw column vectors per pass x rgc row groups,
 // thread -> (column vector cv, row group rg).  Computed once per launch for the three K of a layer (kind 0: width,
-// 1: n_state, 2: mlp width) and kept in the shared-memory header: [6144 + 512 * kind + 2 * tid] = cv | rg << 8,
-// [7680 + 8 * kind] = {cw, rgc} - so no integer division sits on the path of a phase.
+// 1: n_state, 2: mlp width) and kept in the shared-memory header: sm_stage_map(kind)[tid] = cv | rg << 8,
+// sm_stage_dim(kind) = {cw, rgc} - so no integer division sits on the path of a phase.
 __device__ __forceinline__ void stage_map_init(int kind, int Ks) {
     const int nvec = Ks >> 3, tid = threadIdx.x;
     const int cw = nvec >= kConsumers ? kConsumers : nvec;
     const int rgc = nvec >= kConsumers ? 1 : kConsumers / nvec;
-    reinterpret_cast<unsigned short*>(jk_smem + 6144 + 512 * kind)[tid] = (unsigned short)((tid % cw) | ((tid / cw) << 8));
+    sm_stage_map(kind)[tid] = (unsigned short)((tid % cw) | ((tid / cw) << 8));
     if (tid == 0) {
-        reinterpret_cast<int*>(jk_smem + 7680 + 8 * kind)[0] = cw;
-        reinterpret_cast<int*>(jk_smem + 7680 + 8 * kind)[1] = rgc;
+        sm_stage_dim(kind)->cw = cw;
+        sm_stage_dim(kind)->rgc = rgc;
     }
 }
 
@@ -284,8 +310,8 @@ __device__ __noinline__ void stage_acts(const unsigned long long* in, int K, int
         stats[2 * tid + 1] = rstd;
         STAMP(sm_E(), pslot, 5);
     };
-    const int cw = reinterpret_cast<const int*>(jk_smem + 7680 + 8 * kind)[0], rgc = reinterpret_cast<const int*>(jk_smem + 7680 + 8 * kind)[1];
-    const unsigned tm = reinterpret_cast<const unsigned short*>(jk_smem + 6144 + 512 * kind)[tid];
+    const int cw = sm_stage_dim(kind)->cw, rgc = sm_stage_dim(kind)->rgc;
+    const unsigned tm = sm_stage_map(kind)[tid];
     const int cv = tm & 255, rg = tm >> 8;
     const int row_words = K >> 1;
     bool stats_ready = !ln;
@@ -370,11 +396,9 @@ __device__ __forceinline__ void ldsm4(uint32_t (&r)[4], uint32_t addr) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
                  : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
 }
-// one ring slot worth of k-steps, all of it by ONE warp: the slot's k-steps x column groups are independent MMAs
-// that pipeline back to back (round 1 split every slot over the eight warps - one k-step per warp per slot - and
-// paid the mbarrier wait + LDS -> HMMA latency chain once per slot per warp: 1.2 us for four slots).  NCG (8-column
-// groups of this unit) is a template parameter: with a run-time count the compiler serialised every LDS -> HMMA pair
-// through one register pair (tools/micro/ubench.cu: 4070 vs 1170 cycles for the K = 2048 loop).
+// nk k-steps of one ring slot, by one warp: its k-steps x column groups are independent MMAs that pipeline back to
+// back.  NCG (8-column groups of this unit) is a template parameter: with a run-time count the compiler serialised
+// every LDS -> HMMA pair through one register pair (tools/micro/ubench.cu: 4070 vs 1170 cycles for the K = 2048 loop).
 template <int NCG>
 __device__ __forceinline__ void mma_chunk(float (&acc)[8][4], uint32_t arow, uint32_t sl, int kk0, int nk) {
 #pragma unroll 4
@@ -413,17 +437,6 @@ struct GemmArgs {
     long long lb_bs;
 };
 
-// per-launch record of the logits GEMM in the shared-memory header (written once by the kernel prologue)
-struct LogitsRec {
-    float* lg_out;              // logits of this position
-    long long lg_bs;
-    const float* lb;            // logit bias of this position or NULL
-    long long lb_bs;
-    unsigned long long* xp;     // partial-sum exchange of the current pass: xp[pass]
-    ushort2 cols;               // column groups of this unit in the current pass
-};
-__device__ __forceinline__ LogitsRec* sm_lrec() { return reinterpret_cast<LogitsRec*>(jk_smem + 7744); }
-
 // One Conv1D of layer l (or the logits GEMM), identified by its epilogue.  The argument record is assembled HERE from the
 // descriptor / layer record / column table in shared memory: passed by value it had grown past what the call ABI keeps in
 // registers (896 bytes of stack), and with the shared-memory carve-out at its maximum every local-memory access is an L2
@@ -433,7 +446,7 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
     GemmArgs g;
     {
         const LayerDev& LD = *sm_layer(l);
-        const ushort2* cl = reinterpret_cast<const ushort2*>(jk_smem + 1024 + 256 * (l & 1) + 128);
+        const ushort2* cl = sm_cols(l);
         const int W = E->W, S = E->S, M = E->M;
         long long* lnb = E->lnacc + (size_t)(2 * l) * 512;
         g.epi = epi_; g.pslot = pslot_; g.flag_in = fl; g.flag_out = fl;
@@ -485,7 +498,6 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
     const int kpc = kpc_of(ncg);                          // a power of two
     const int astride = (Ks + 8) * 2;
     const uint32_t arow = smem_u32(uni + (lane & 15) * astride + (lane >> 4) * 16);
-#if JK_MMA_ALL_WARPS
     // The k-steps of this CTA's slice are dealt to the eight warps in contiguous runs (k-step i -> warp i * 8 / nkk), so
     // every warp multiplies - 4 k-steps each for a K = 2048 / KS = 4 phase instead of four warps with a whole slot each and
     // four idle.  EVERY warp still waits for every slot and arrives on its empty barrier, in order: the parity protocol of
@@ -502,7 +514,7 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
     // contiguous runs one warp would own several consecutive slots while the ring delivers them in order, i.e. one warp
     // would multiply at a time (5b_lyrics, one box: 6 192 us per step round robin, 6 691 us with contiguous runs).
     const int nslots_phase = (nkk + kpc - 1) >> (31 - __clz(kpc));
-    const bool in_order = !JK_SKIP_FOREIGN_WAIT || nslots_phase > Ring::nslot();
+    const bool in_order = nslots_phase > Ring::nslot();
     int slot_i = 0;
 #define JK_MMA_LOOP(NCG)                                                                      \
     {                                                                                         \
@@ -517,27 +529,6 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
             ring.advance();                                                                   \
         }                                                                                     \
     }
-#else
-    // slot s of this Conv1D is multiplied by warp s % 8 alone.  EVERY warp still waits for the slot and arrives on its
-    // empty barrier: the parity protocol of the ring only holds while no warp is a whole ring ahead of or behind the
-    // producer (a warp that skipped the handshake of foreign slots aliased phases once a Conv1D had more slots than
-    // the ring: 38 vs 6 for 5b_lyrics).
-#define JK_MMA_LOOP(NCG)                                                                      \
-    {                                                                                         \
-        int owner = 0;                                                                        \
-        _Pragma("unroll 1") for (int kk0 = 0; kk0 < nkk; kk0 += kpc) {                        \
-            mbar_wait(ring.full(), ring.phase);                                                \
-            if (owner == warp) {                                                              \
-                const int nk = min(kpc, nkk - kk0);                                            \
-                mma_chunk<NCG>(acc, arow, smem_u32(ring.data()) + lane * 8, kk0, nk);          \
-            }                                                                                 \
-            __syncwarp();                                                                      \
-            if (lane == 0) mbar_arrive(ring.empty());                                          \
-            owner = (owner + 1) & 7;                                                          \
-            ring.advance();                                                                   \
-        }                                                                                     \
-    }
-#endif
     switch (ncg) {
         case 1: JK_MMA_LOOP(1) break;
         case 2: JK_MMA_LOOP(2) break;
@@ -550,11 +541,7 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
     }
 #undef JK_MMA_LOOP
     STAMP(E, g.pslot, 2);
-#if JK_MMA_ALL_WARPS
     const int nwarp = in_order ? min(8, nslots_phase) : min(8, nkk);       // warps that multiplied at least one k-step
-#else
-    const int nwarp = min(8, (nkk + kpc - 1) >> (31 - __clz(kpc)));       // warps that multiplied at least one slot
-#endif
     float* red = reinterpret_cast<float*>(uni);
     const int ncp = ((nc + 31) & ~31) + 8;
     // partial sums of the unit: [KS ranks][16 rows][64 columns] LL words {fp32, flag}
@@ -785,41 +772,6 @@ __device__ __forceinline__ void attn_out_pair(const EngineDev* E, int b, int h, 
     ll_st(E->ll_a + (((size_t)b * E->S + h * E->dh + d) >> 1), *reinterpret_cast<const uint32_t*>(&o), flag);
 }
 
-// flash-decoding merge of the ns partials of one (sample, head), run by the CTA that finished last.
-// Own function: its registers must not add to attn_item's (see "Register regime" in DESIGN.md).
-__device__ __noinline__ void attn_merge(int item, int ns, int b, int h, uint32_t flag) {
-    const EngineDev* E = sm_E();
-    const int tid = threadIdx.x, dh = E->dh, dhp = E->dh_pad;
-    const float* p0 = E->part + ((size_t)(item * kMaxSplit)) * (dhp + 2);
-    const int st = dhp + 2;
-    const int d = 2 * tid;                  // dims d, d+1 (dh is even, dh <= 512)
-    {
-        // every load of the merge is issued before the first use: ONE L2 round trip instead of three
-        // dependent ones (max pass, sum pass, value pass) on the critical path of the slowest CTAs
-        float m[4], l[4];
-        float2 v[4];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            const bool on = q < ns;
-            m[q] = on ? __ldcg(p0 + (size_t)q * st) : -INFINITY;
-            l[q] = on ? __ldcg(p0 + (size_t)q * st + 1) : 0.f;
-            v[q] = (on && d < dh) ? __ldcg(reinterpret_cast<const float2*>(p0 + (size_t)q * st + 2 + d)) : make_float2(0.f, 0.f);
-        }
-        float M = -INFINITY;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) M = fmaxf(M, m[q]);
-        float Lsum = 0.f, o0 = 0.f, o1 = 0.f;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            if (q < ns) {
-                const float w = expf(m[q] - M);
-                Lsum += l[q] * w; o0 += v[q].x * w; o1 += v[q].y * w;
-            }
-        }
-        if (d < dh) attn_out_pair(E, b, h, d, o0 / Lsum, o1 / Lsum, flag);
-    }
-}
-
 // One (sample, head, part) work item; q_len == 1 (reference factored_attention.py:82-133 and the
 // per-pattern sample branches :135-228).
 //   * q and the current token's k, v come from the QKV Conv1D as LL words (polled: this is the QKV -> attention
@@ -831,13 +783,13 @@ __device__ __noinline__ void attn_merge(int item, int ns, int b, int h, uint32_t
 //   * softmax is flash-style in fp32 (running max / sum), every warp redundantly; P rounded to fp16 as
 //     the reference's w.half(), P.V on the tensor cores (A = P in row 0, B = V via ldmatrix.trans), each
 //     warp owning 16-dim output slices
-//   * parts of one (sample, head) are merged by the last CTA to finish (atomic ticket); the output goes to
-//     the `a` LL buffer, which IS the attention -> proj hand-over
+//   * parts 0 .. ns-2 of one (sample, head) publish their (max, sum, output) as LL words; the last part, which also
+//     holds the current token, polls them and merges (flash-decoding merge); the output goes to the `a` LL buffer,
+//     which IS the attention -> proj hand-over
 __device__ __noinline__ void attn_item(const LayerDev& LD_ref, int b, int h, int s, int ns,
                                        const AttnGeom G, int pslot, uint32_t flag, int pre) {
     const EngineDev* E = sm_E();
     uint8_t* uni = sm_uni();
-    float* stats = sm_stats();
     const LayerDev LD = LD_ref;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int dh = E->dh, dhp = E->dh_pad, S = E->S;
@@ -875,7 +827,6 @@ __device__ __noinline__ void attn_item(const LayerDev& LD_ref, int b, int h, int
     {
         const int hw = dhp >> 1, dw = dh >> 1;
         const int nsel = (LD.attn_func == 6) ? 1 : 3;
-#if JK_QKV_POLL_BATCH
         // up to three words per thread (dh <= 512), ALL issued before the first is examined: one L2 round trip, where a
         // loop of blocking polls paid one per iteration (two for head_dim 256)
         const int total = nsel * hw;
@@ -902,14 +853,6 @@ __device__ __noinline__ void attn_item(const LayerDev& LD_ref, int b, int h, int
             const int i = tid + j * kConsumers;
             if (i < total) reinterpret_cast<uint32_t*>(qh)[i] = wp[j] ? (uint32_t)wv[j] : 0u;
         }
-#else
-        for (int i = tid; i < nsel * hw; i += kConsumers) {
-            const int sel = i / hw, wd = i - sel * hw;
-            uint32_t v = 0u;
-            if (wd < dw) v = ll_wait1(qrow + (size_t)sel * (S >> 1) + wd, flag);
-            reinterpret_cast<uint32_t*>(qh)[sel * hw + wd] = v;
-        }
-#endif
     }
     consumer_sync();
     if (G.wrow >= 0 && last_part) {          // cache the current token's k, v
@@ -1010,25 +953,16 @@ __device__ __noinline__ void attn_item(const LayerDev& LD_ref, int b, int h, int
                         const float inv = 1.f / l_run;
                         if (d < dh) attn_out_pair(E, b, h, d, r0.x * inv, r0.y * inv, flag);
                         if (d + 8 < dh) attn_out_pair(E, b, h, d + 8, r1.x * inv, r1.y * inv, flag);
-                    } else {
-#if JK_ATTN_LL_MERGE
-                        if (last_part) {       // the merging part keeps its own partial in shared memory (osm is free now)
-                            *reinterpret_cast<float2*>(osm + d) = r0;
-                            *reinterpret_cast<float2*>(osm + d + 8) = r1;
-                        } else {               // the others publish theirs as LL words {fp32, flag}
-                            unsigned long long* pl = reinterpret_cast<unsigned long long*>(E->part) +
-                                                     ((size_t)((b * E->H + h) * kMaxSplit + s)) * (dhp + 2) + 2 + d;
-                            const unsigned long long fw = (unsigned long long)flag << 32;
-                            asm volatile(JK_ST_LL ".v2.u64 [%0], {%1,%2};" ::"l"(pl), "l"(fw | __float_as_uint(r0.x)),
-                                         "l"(fw | __float_as_uint(r0.y)) : "memory");
-                            asm volatile(JK_ST_LL ".v2.u64 [%0], {%1,%2};" ::"l"(pl + 8), "l"(fw | __float_as_uint(r1.x)),
-                                         "l"(fw | __float_as_uint(r1.y)) : "memory");
-                        }
-#else
-                        float* part = E->part + ((size_t)((b * E->H + h) * kMaxSplit + s)) * (dhp + 2) + 2;
-                        *reinterpret_cast<float2*>(part + d) = r0;
-                        *reinterpret_cast<float2*>(part + d + 8) = r1;
-#endif
+                    } else if (last_part) {    // the merging part keeps its own partial in shared memory (osm is free now)
+                        *reinterpret_cast<float2*>(osm + d) = r0;
+                        *reinterpret_cast<float2*>(osm + d + 8) = r1;
+                    } else {                   // the others publish theirs as LL words {fp32, flag}
+                        unsigned long long* pl = E->part + ((size_t)((b * E->H + h) * kMaxSplit + s)) * (dhp + 2) + 2 + d;
+                        const unsigned long long fw = (unsigned long long)flag << 32;
+                        asm volatile(JK_ST_LL ".v2.u64 [%0], {%1,%2};" ::"l"(pl), "l"(fw | __float_as_uint(r0.x)),
+                                     "l"(fw | __float_as_uint(r0.y)) : "memory");
+                        asm volatile(JK_ST_LL ".v2.u64 [%0], {%1,%2};" ::"l"(pl + 8), "l"(fw | __float_as_uint(r1.x)),
+                                     "l"(fw | __float_as_uint(r1.y)) : "memory");
                     }
                 }
             }
@@ -1037,82 +971,59 @@ __device__ __noinline__ void attn_item(const LayerDev& LD_ref, int b, int h, int
     }
     STAMP(E, pslot, 3);
     if (ns == 1) return;
-#if JK_ATTN_LL_MERGE
-    // ---- split parts: parts 0 .. ns-2 have published (m, l, o) as LL words; the LAST part (the one that also holds the
-    // current token) polls them and merges - a fixed merger instead of "whoever finishes last": no ticket atomic (an
-    // acq_rel round trip), no second barrier, and the partials arrive word by word like every other hand-over.  Same
-    // order of summation as attn_merge (parts 0 .. ns-1), so the result is bit-identical to the ticket version.
-    {
-        const int item_ = b * E->H + h;
-        unsigned long long* pbase = reinterpret_cast<unsigned long long*>(E->part) + ((size_t)(item_ * kMaxSplit)) * (dhp + 2);
-        if (!last_part) {
-            if (tid == 0) {
-                const unsigned long long fw = (unsigned long long)flag << 32;
-                asm volatile(JK_ST_LL ".v2.u64 [%0], {%1,%2};" ::"l"(pbase + (size_t)s * (dhp + 2)), "l"(fw | __float_as_uint(m_run)),
-                             "l"(fw | __float_as_uint(l_run)) : "memory");
-            }
-            STAMP(E, pslot, 6);
-            return;
-        }
-        consumer_sync();                       // every warp's slice of this part's output is in osm
-        const int d = 2 * tid;
-        if (d < dh) {
-            ulonglong2 ml[3], vv[3];
-            unsigned spins = 0;
-            bool again;
-            do {
-                again = false;
-#pragma unroll
-                for (int q = 0; q < 3; ++q) {
-                    if (q < ns - 1) {
-                        ml[q] = ll_ld2(pbase + (size_t)q * (dhp + 2));
-                        vv[q] = ll_ld2(pbase + (size_t)q * (dhp + 2) + 2 + d);
-                    }
-                }
-#pragma unroll
-                for (int q = 0; q < 3; ++q)
-                    if (q < ns - 1) again |= !(ll_ok(ml[q].x, flag) && ll_ok(ml[q].y, flag) && ll_ok(vv[q].x, flag) && ll_ok(vv[q].y, flag));
-                if (again) spin_guard(spins);
-            } while (again);
-            float M = m_run;
-#pragma unroll
-            for (int q = 0; q < 3; ++q)
-                if (q < ns - 1) M = fmaxf(M, __uint_as_float((uint32_t)ml[q].x));
-            float Lsum = 0.f, o0 = 0.f, o1 = 0.f;
-#pragma unroll
-            for (int q = 0; q < 3; ++q) {
-                if (q < ns - 1) {
-                    const float w = expf(__uint_as_float((uint32_t)ml[q].x) - M);
-                    Lsum += __uint_as_float((uint32_t)ml[q].y) * w;
-                    o0 += __uint_as_float((uint32_t)vv[q].x) * w; o1 += __uint_as_float((uint32_t)vv[q].y) * w;
-                }
-            }
-            {
-                const float w = expf(m_run - M);
-                const float2 own = *reinterpret_cast<const float2*>(osm + d);
-                Lsum += l_run * w; o0 += own.x * w; o1 += own.y * w;
-            }
-            attn_out_pair(E, b, h, d, o0 / Lsum, o1 / Lsum, flag);
+    // ---- split parts: parts 0 .. ns-2 publish (m, l, o) as LL words; the LAST part (the one that also holds the current
+    // token) polls them and merges - a fixed merger: no ticket atomic (an acq_rel round trip), no second barrier, and the
+    // partials arrive word by word like every other hand-over.  Summed in part order 0 .. ns-1: bit-reproducible.
+    unsigned long long* pbase = E->part + ((size_t)((b * E->H + h) * kMaxSplit)) * (dhp + 2);
+    if (!last_part) {
+        if (tid == 0) {
+            const unsigned long long fw = (unsigned long long)flag << 32;
+            asm volatile(JK_ST_LL ".v2.u64 [%0], {%1,%2};" ::"l"(pbase + (size_t)s * (dhp + 2)), "l"(fw | __float_as_uint(m_run)),
+                         "l"(fw | __float_as_uint(l_run)) : "memory");
         }
         STAMP(E, pslot, 6);
         return;
     }
-#endif
-    // ---- split parts: the partial is published, the last finisher merges (flash-decoding merge) ------
-    const int item = b * E->H + h;
-    if (tid == 0) {
-        float* part = E->part + ((size_t)(item * kMaxSplit + s)) * (dhp + 2);
-        part[0] = m_run; part[1] = l_run;
+    consumer_sync();                       // every warp's slice of this part's output is in osm
+    const int d = 2 * tid;
+    if (d < dh) {
+        ulonglong2 ml[3], vv[3];
+        unsigned spins = 0;
+        bool again;
+        do {
+            again = false;
+#pragma unroll
+            for (int q = 0; q < 3; ++q) {
+                if (q < ns - 1) {
+                    ml[q] = ll_ld2(pbase + (size_t)q * (dhp + 2));
+                    vv[q] = ll_ld2(pbase + (size_t)q * (dhp + 2) + 2 + d);
+                }
+            }
+#pragma unroll
+            for (int q = 0; q < 3; ++q)
+                if (q < ns - 1) again |= !(ll_ok(ml[q].x, flag) && ll_ok(ml[q].y, flag) && ll_ok(vv[q].x, flag) && ll_ok(vv[q].y, flag));
+            if (again) spin_guard(spins);
+        } while (again);
+        float M = m_run;
+#pragma unroll
+        for (int q = 0; q < 3; ++q)
+            if (q < ns - 1) M = fmaxf(M, __uint_as_float((uint32_t)ml[q].x));
+        float Lsum = 0.f, o0 = 0.f, o1 = 0.f;
+#pragma unroll
+        for (int q = 0; q < 3; ++q) {
+            if (q < ns - 1) {
+                const float w = expf(__uint_as_float((uint32_t)ml[q].x) - M);
+                Lsum += __uint_as_float((uint32_t)ml[q].y) * w;
+                o0 += __uint_as_float((uint32_t)vv[q].x) * w; o1 += __uint_as_float((uint32_t)vv[q].y) * w;
+            }
+        }
+        {
+            const float w = expf(m_run - M);
+            const float2 own = *reinterpret_cast<const float2*>(osm + d);
+            Lsum += l_run * w; o0 += own.x * w; o1 += own.y * w;
+        }
+        attn_out_pair(E, b, h, d, o0 / Lsum, o1 / Lsum, flag);
     }
-    consumer_sync();
-    if (tid == 0) {      // acq_rel ticket: publishes this CTA's partial, acquires the others' for the merger
-        unsigned ticket;
-        asm volatile("atom.acq_rel.gpu.global.add.u32 %0, [%1], 1;" : "=r"(ticket) : "l"(E->acnt + item) : "memory");
-        stats[48] = (ticket == (unsigned)(ns - 1)) ? 1.f : 0.f;
-        if (ticket == (unsigned)(ns - 1)) E->acnt[item] = 0u;
-    }
-    consumer_sync();
-    if (stats[48] != 0.f) attn_merge(item, ns, b, h, flag);
     STAMP(E, pslot, 6);
 }
 
@@ -1121,7 +1032,6 @@ __device__ __noinline__ void attn_item(const LayerDev& LD_ref, int b, int h, int
 // that phase.  Returns 1 if the tile is on its way.
 __device__ __noinline__ int attn_prefetch(const LayerDev& LD_ref, int B, int c, int t, int pm, int pd, int gmax) {
     const EngineDev* E = sm_E();
-    if (!E->kv_prefetch) return 0;
     const LayerDev LD = LD_ref;
     const AttnGeom G = attn_geom(E, LD, t, pm, pd);
     if (G.R == 0) return 0;
@@ -1309,24 +1219,18 @@ __device__ __noinline__ void logits_phase(const StepArgs& A_ref, Ring& ring_ref,
     }
 }
 
-#ifndef JK_CLEANER_WARP
-#define JK_CLEANER_WARP 1
-#endif
-#ifndef JK_ASYNC_RECORD
-#define JK_ASYNC_RECORD 1
-#endif
 // Housekeeping of the LayerNorm statistics blocks, on warp 9 of CTA 0 (a warp of the producer warpgroup that has nothing
 // else to do).  Block i (0 .. 2 * depth) is used once per launch and must be zero again at the next launch.  It may be
 // cleared once a LATER block is complete: every CTA contributes to block i + 1 only after it has consumed block i
-// (program order + data dependence).  The consumer warps of CTA 0 used to do this between their phases - one polled L2
-// round trip on the critical path of CTA 0 (and so of its unit) twice per layer.  The same warp publishes the position
-// and the step count at the end: the final block is complete only when every CTA is through the stack, and every CTA has
-// read both words long before that.
+// (program order + data dependence).  On the consumer warps of CTA 0 this would put a polled L2 round trip on the
+// critical path of CTA 0 (and so of its unit) twice per layer.  The same warp publishes the position and the step count
+// at the end: the final block is complete only when every CTA is through the stack, and every CTA has read both words
+// long before that.
 __device__ __noinline__ void cleaner_loop() {
     const EngineDev* E = sm_E();
     const int lane = threadIdx.x & 31, G = E->G, nblk = 2 * E->depth;
     const int t = *reinterpret_cast<volatile const int*>(E->t);
-    const unsigned step = *reinterpret_cast<volatile const unsigned*>(E->sync + 64);
+    const unsigned step = *reinterpret_cast<volatile const unsigned*>(E->step);
     for (int i = 1; i <= nblk; ++i) {
         if (lane == 0) wait_stat_word(E->lnacc + (size_t)i * 512, G);
         __syncwarp();
@@ -1335,17 +1239,20 @@ __device__ __noinline__ void cleaner_loop() {
     (E->lnacc + (size_t)nblk * 512)[16 * (lane >> 1) + (lane & 1)] = 0;
     if (lane == 0) {
         *E->t = t + 1;
-        *(E->sync + 64) = step + 1;
+        *E->step = step + 1;
     }
 }
 
 // ---------------------------------------------------------------------------------------
 // Values of a launch that every phase call would otherwise have to keep in a register: ptxas allocates the __noinline__
 // phases inter-procedurally, so each value live across the calls is a register less inside them (on sm_90a, keeping
-// these in registers made gemm_phase spill).  The descriptor fields are re-read from its shared-memory copy; the position
-// and the step count live in header words [7724] and [7728], written by the kernel prologue.
-__device__ __forceinline__ int launch_pos() { return reinterpret_cast<const int*>(jk_smem + 7712)[3]; }
-__device__ __forceinline__ uint32_t launch_step() { return (uint32_t)reinterpret_cast<const int*>(jk_smem + 7712)[4]; }
+// these in registers made gemm_phase spill).  The descriptor fields are re-read from its shared-memory copy; the position,
+// its block coordinates and the step count live in the header's LaunchVals, written by the kernel prologue.
+__device__ __forceinline__ int launch_pos() { return sm_launch()->t; }
+__device__ __forceinline__ int launch_pm() { return sm_launch()->pm; }
+__device__ __forceinline__ int launch_pd() { return sm_launch()->pd; }
+__device__ __forceinline__ int launch_gmax() { return sm_launch()->gmax; }
+__device__ __forceinline__ uint32_t launch_step() { return sm_launch()->step; }
 // LL flags of this launch: launch_fbase() + 1 .. launch_fbase() + depth + 1
 __device__ __forceinline__ uint32_t launch_fbase() { return launch_step() * (uint32_t)(sm_E()->depth + 2); }
 __device__ __forceinline__ int cta_unit() { return (int)blockIdx.x >> sm_E()->ks_shift; }
@@ -1355,22 +1262,20 @@ __device__ __forceinline__ bool wants_logits(const StepArgs& A) { return A.logit
 // x_cond . x_out^T, the logit bias of jkb200.h: the product is linear in the activation)
 __device__ __forceinline__ bool logits_on_mma(const StepArgs& A) {
     const EngineDev* E = sm_E();
-    return JK_LOGITS_MMA && E->lg_on && (!(E->add_cond_after && A.x_cond) || A.logit_bias);
+    return E->lg_on && (!(E->add_cond_after && A.x_cond) || A.logit_bias);
 }
 
 __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const EngineDev* __restrict__ Eg, StepArgs A) {
     const int tid = threadIdx.x, warp = tid >> 5;
     const int c = blockIdx.x;
-    static_assert(offsetof(EngineDev, layer) <= 512, "descriptor head must fit its shared-memory slot");
-    static_assert(sizeof(LayerDev) <= 128, "layer record must fit its shared-memory slot");
     for (int i = tid; i < (int)(offsetof(EngineDev, layer) / 4); i += kThreads)
-        reinterpret_cast<uint32_t*>(jk_smem + 512)[i] = reinterpret_cast<const uint32_t*>(Eg)[i];
+        sm_desc_words()[i] = reinterpret_cast<const uint32_t*>(Eg)[i];
     if (tid < (int)(sizeof(LayerDev) / 4))
-        reinterpret_cast<uint32_t*>(jk_smem + 1024)[tid] = reinterpret_cast<const uint32_t*>(&Eg->layer[0])[tid];
+        reinterpret_cast<uint32_t*>(sm_layer_slot(0))[tid] = reinterpret_cast<const uint32_t*>(&Eg->layer[0])[tid];
     __syncthreads();
     const EngineDev* E = sm_E();
     if (tid >= 32 && tid < 36)
-        reinterpret_cast<uint32_t*>(jk_smem + 1024 + 128)[tid - 32] =
+        reinterpret_cast<uint32_t*>(sm_cols(0))[tid - 32] =
             reinterpret_cast<const uint32_t*>(E->cols + ((size_t)cta_unit() * E->depth + 0) * 4)[tid - 32];
     Ring ring;
     ring.slot = 0; ring.phase = 0;
@@ -1384,48 +1289,24 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
     if (warp >= 8) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
         if (warp == 8) producer_loop(Eg, ring, wants_logits(A) ? (logits_on_mma(A) ? 2 : 1) : 0, c);
-#if JK_CLEANER_WARP
         else if (warp == 9 && c == 0) cleaner_loop();
-#endif
         return;
     }
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     const int B = A.n;
-    // statistics blocks: 2l = input of layer l's LN0, 2l + 1 = input of its LN1, 2 * depth = the final residual stream
-    // (nobody normalises it; its count tells CTA 0 that every CTA is through the stack)
-#define LN_BLOCK(i_) (E->lnacc + (size_t)(i_) * 512)
-    // CTA 0 clears a block for the next launch once a LATER block is complete: every CTA contributes to the later block
-    // only after it has consumed the earlier one (program order + data dependence)
-#if JK_CLEANER_WARP
-#define CLEAR_AFTER(clear_, seen_) do { } while (0)       /* cleaner_loop() on warp 9 of CTA 0 */
-#else
-#define CLEAR_AFTER(clear_, seen_)                                                             \
-    do {                                                                                       \
-        if (c == 0 && tid < 32) {                                                              \
-            if (tid == 0) wait_stat_word(LN_BLOCK(seen_), E->G);                               \
-            __syncwarp();                                                                      \
-            LN_BLOCK(clear_)[16 * (tid >> 1) + (tid & 1)] = 0;                                 \
-        }                                                                                      \
-    } while (0)
-#endif
-    // thread layouts of the activation staging for the three K of a layer (integer divisions: once per launch, not per phase)
-    // per-launch values live in shared memory (not in registers across the phase calls):
-    // [7712] p % block_ctx, [7716] p / block_ctx, [7720] CTAs available per (sample, head), [7724] position t,
-    // [7728] steps executed so far
+    // per-launch values live in shared memory (not in registers across the phase calls)
     if (tid == 0) {
-        int* gq = reinterpret_cast<int*>(jk_smem + 7712);
+        LaunchVals* lv = sm_launch();
         const int t = *reinterpret_cast<volatile const int*>(E->t);
-        gq[0] = E->blocks > 0 ? t % E->bc : 0;
-        gq[1] = E->blocks > 0 ? t / E->bc : 0;
-        gq[2] = max(1, E->G / (B * E->H));
-        gq[3] = t;
+        lv->pm = E->blocks > 0 ? t % E->bc : 0;
+        lv->pd = E->blocks > 0 ? t / E->bc : 0;
+        lv->gmax = max(1, E->G / (B * E->H));
+        lv->t = t;
         // written only at the very end of a launch by CTA 0, after every CTA of that launch has passed an all-to-all
         // point - so every CTA of this launch reads the same value
-        gq[4] = (int)*reinterpret_cast<volatile const unsigned*>(E->sync + 64);
+        lv->step = *reinterpret_cast<volatile const unsigned*>(E->step);
     }
-#define PM (reinterpret_cast<const int*>(jk_smem + 7712)[0])
-#define PD (reinterpret_cast<const int*>(jk_smem + 7712)[1])
-#define GMAX (reinterpret_cast<const int*>(jk_smem + 7712)[2])
+    // thread layouts of the activation staging for the three K of a layer (integer divisions: once per launch, not per phase)
     stage_map_init(0, E->W >> E->ks_shift);
     stage_map_init(1, E->S >> E->ks_shift);
     stage_map_init(2, E->M >> E->ks_shift);
@@ -1457,7 +1338,7 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
     // ---- P0: embedding (autoregressive.py:177-197) or an externally embedded activation ------
     // This CTA embeds exactly the columns of the residual stream it will own for the whole stack.
     {
-        const ushort2 wc = reinterpret_cast<const ushort2*>(jk_smem + 1024 + 128)[1];     // column groups of width-W outputs
+        const ushort2 wc = sm_cols(0)[1];                   // column groups of width-W outputs
         const int ppc = (wc.y * 4) >> E->ks_shift;
         float2* res = sm_res();
         long long* sfx = sm_sfx();
@@ -1486,7 +1367,7 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
             sfx[1024 + b * 32 + pl] = fx_sq(hv.x) + fx_sq(hv.y);
             ll_st(E->ll_h + (((size_t)b * E->W + col) >> 1), *reinterpret_cast<const uint32_t*>(&hh), launch_fbase() + 1);
         }
-        publish_stats(LN_BLOCK(0), B, ppc);
+        publish_stats(E->lnacc, B, ppc);     // statistics block 0: the input of layer 0's LN0
     }
     PHASE_DONE();
 
@@ -1494,41 +1375,30 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
     for (int l = 0; l < E->depth; ++l) {
         const LayerDev& LD = *sm_layer(l);
         const uint32_t fl = launch_fbase() + (uint32_t)l + 1;              // flag of this layer's buffers
-        const int pre = attn_prefetch(LD, B, c, launch_pos(), PM, PD, GMAX);
+        const int pre = attn_prefetch(LD, B, c, launch_pos(), launch_pm(), launch_pd(), launch_gmax());
         // a fresh argument record per phase: nothing of it stays live across the calls in between
         if (l == 1) PROF3(0, 0);
         ring = gemm_phase(ring, B, EPI_QKV, l, (int)nph, fl);
         if (l == 1) PROF3(0, 1);
-        // LN1 statistics of the previous layer: consumed once this layer's LN0 block is complete
-        if (l > 0) CLEAR_AFTER(2 * l - 1, 2 * l);
         // next layer's record + column assignment -> the other shared-memory slot.  The descriptor is in
         // HBM (the weight stream evicts it from L2 every step): issue the loads here so their latency hides
         // behind the attention phase instead of sitting on the dependency chain.
         if (l + 1 < E->depth) {
-#if JK_ASYNC_RECORD
             // cp.async: no register sits between the HBM load and the shared-memory store, so no warp stalls on it here;
             // it is waited for in front of this layer's last Conv1D (whose barriers publish it to the other threads)
             if (tid < (int)(sizeof(LayerDev) / 4))
-                asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(jk_smem + 1024 + 256 * ((l + 1) & 1) + 4 * tid)),
+                asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(sm_layer_slot(l + 1) + 4 * tid)),
                              "l"(reinterpret_cast<const uint32_t*>(&Eg->layer[l + 1]) + tid) : "memory");
             if (tid >= 32 && tid < 36)
-                asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(jk_smem + 1024 + 256 * ((l + 1) & 1) + 128 + 4 * (tid - 32))),
+                asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(sm_cols(l + 1) + (tid - 32))),
                              "l"(reinterpret_cast<const uint32_t*>(E->cols + ((size_t)cta_unit() * E->depth + l + 1) * 4) + (tid - 32)) : "memory");
             asm volatile("cp.async.commit_group;" ::: "memory");
-#else
-            if (tid < (int)(sizeof(LayerDev) / 4))
-                reinterpret_cast<uint32_t*>(jk_smem + 1024 + 256 * ((l + 1) & 1))[tid] =
-                    reinterpret_cast<const uint32_t*>(&Eg->layer[l + 1])[tid];
-            if (tid >= 32 && tid < 36)
-                reinterpret_cast<uint32_t*>(jk_smem + 1024 + 256 * ((l + 1) & 1) + 128)[tid - 32] =
-                    reinterpret_cast<const uint32_t*>(E->cols + ((size_t)cta_unit() * E->depth + l + 1) * 4)[tid - 32];
-#endif
         }
         PHASE_DONE();
         if (l == 1) PROF3(1, 0);
         {
-            const AttnGeom geo = attn_geom(E, LD, launch_pos(), PM, PD);
-            const int ns = attn_nsplit(E, GMAX, geo.R - ((geo.R > 0 && geo.cur) ? 1 : 0));
+            const AttnGeom geo = attn_geom(E, LD, launch_pos(), launch_pm(), launch_pd());
+            const int ns = attn_nsplit(E, launch_gmax(), geo.R - ((geo.R > 0 && geo.cur) ? 1 : 0));
             for (int it = c; it < B * E->H * ns; it += E->G) {
                 const int bh = div_small(it, ns), s = it - bh * ns, ib = bh / E->H;
                 attn_item(LD, ib, bh - ib * E->H, s, ns, geo, (int)nph, fl, pre && it == c);
@@ -1544,19 +1414,15 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
         if (l == 1) PROF3(3, 0);
         ring = gemm_phase(ring, B, EPI_FC, l, (int)nph, fl);
         if (l == 1) PROF3(3, 1);
-        // LN0 statistics of this layer: consumed once its LN1 block is complete
-        CLEAR_AFTER(2 * l, 2 * l + 1);
         PHASE_DONE();
         if (l == 1) PROF3(4, 0);
-#if JK_ASYNC_RECORD
         asm volatile("cp.async.wait_group 0;" ::: "memory");      // the next layer's record (issued a phase and a half ago)
-#endif
         ring = gemm_phase(ring, B, EPI_PROJ2, l, (int)nph, fl);
         if (l == 1) PROF3(4, 1);
         PHASE_DONE();
     }
     if (A.h_out) {      // Transformer.forward boundary: this CTA's slice of the residual stream
-        const ushort2 wc = reinterpret_cast<const ushort2*>(jk_smem + 1024 + 256 * ((E->depth - 1) & 1) + 128)[1];
+        const ushort2 wc = sm_cols(E->depth - 1)[1];
         const int ppc = (wc.y * 4) >> E->ks_shift;
         const float2* res = sm_res();
         const int lane = tid & 31;
@@ -1595,28 +1461,14 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
     } else if (wants_logits(A)) {
         logits_phase(A, ring, c, launch_pos(), launch_fbase() + (uint32_t)E->depth + 1);
     }
-    // the last LN1 block and the final block: clear them once every CTA is through the stack
-    CLEAR_AFTER(2 * E->depth - 1, 2 * E->depth);
     if (c == 0) {
         consumer_sync();
-#if !JK_CLEANER_WARP
-        if (tid < 32) LN_BLOCK(2 * E->depth)[16 * (tid >> 1) + (tid & 1)] = 0;
-#endif
         if (tid == 0) {
             unsigned long long now;
             asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
             if (E->prof_on && nph + 1 < (unsigned)kProfSlots) E->prof[nph + 1] = now;
-#if !JK_CLEANER_WARP
-            *E->t = launch_pos() + 1;
-            *(E->sync + 64) = launch_step() + 1;
-#endif
         }
     }
-#undef LN_BLOCK
-#undef CLEAR_AFTER
-#undef PM
-#undef PD
-#undef GMAX
 #undef PHASE_DONE
 #undef PROF3
 }
@@ -1740,7 +1592,7 @@ __global__ void enc_kv_scatter_kernel(const __half* __restrict__ y, __half* kc, 
 namespace {
 
 struct Layout {
-    size_t off_dev, off_cols, off_goff, off_lrow, off_streams, off_small, off_cache, off_h, off_x1, off_qkv, off_a, off_g, off_xp[4], off_part, off_acnt, off_prof, off_prof2, off_prof3, off_lnacc, off_encx, off_ency, off_wt, off_pf, off_sync, total;
+    size_t off_dev, off_cols, off_goff, off_lrow, off_streams, off_small, off_cache, off_h, off_x1, off_qkv, off_a, off_g, off_xp[4], off_part, off_prof, off_prof2, off_prof3, off_lnacc, off_encx, off_ency, off_wt, off_pf, off_step, total;
     int KS, U;
     size_t wt_per_layer;
     int pf_len, pf_rows;
@@ -1753,7 +1605,7 @@ struct Layout {
     std::vector<size_t> cache_bytes;
     std::vector<int> cache_rows;
     size_t small_per_layer;
-    int dh, dh_pad, bc, prime_pad, uni_bytes, kvpre_bytes, kv_prefetch, nslot, smem_bytes, RC;
+    int dh, dh_pad, bc, prime_pad, uni_bytes, kvpre_bytes, nslot, smem_bytes, RC;
 };
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
@@ -1903,7 +1755,6 @@ int compute_layout(const jk_prior_config& c, int G, Layout& L) {
         if (nslot >= 4 || RC <= 16) break;                  // a deep weight ring matters more than tall K/V tiles
     }
     L.RC = RC;
-    L.kv_prefetch = 0;
     nslot = std::min(nslot, kMaxSlots);
     JK_REQUIRE(nslot >= 2, "not enough shared memory for the weight ring (uni %d bytes)", L.uni_bytes);
     L.nslot = nslot;
@@ -1939,7 +1790,6 @@ int compute_layout(const jk_prior_config& c, int G, Layout& L) {
     L.off_g = off;   off = align_up(off + (size_t)16 * c.mlp_width * 4, 256);
     for (int gi = 0; gi < 4; ++gi) { L.off_xp[gi] = off; off = align_up(off + (size_t)G * 16 * kXpCols * 8, 256); }
     L.off_part = off; off = align_up(off + (size_t)c.max_batch * c.heads * kMaxSplit * (L.dh_pad + 2) * 8, 256);      // LL words
-    L.off_acnt = off; off = align_up(off + (size_t)c.max_batch * c.heads * 4, 256);
     L.off_prof = off; off = align_up(off + (size_t)kProfSlots * 8, 256);
     L.off_prof2 = off; off = align_up(off + (size_t)kProfSlots * 8 * 8, 256);
     L.off_prof3 = off; off = align_up(off + (size_t)5 * 256 * 2 * 8, 256);
@@ -1965,7 +1815,7 @@ int compute_layout(const jk_prior_config& c, int G, Layout& L) {
         L.off_pf = off;
         if (ok) off = align_up(off + (size_t)L.pf_rows * (3 * c.width + 3 * c.n_state + c.n_state + c.mlp_width) * 2, 1024);
     }
-    L.off_sync = off; off += 8192;
+    L.off_step = off; off += 256;                       // step count and position, one 128-byte line each
     L.total = off;
     return 0;
 }
@@ -2040,7 +1890,6 @@ extern "C" int jk_prior_create(const jk_prior_config* cfg, void* arena, size_t a
     E.L = cfg->n_ctx; E.blocks = cfg->blocks; E.bc = L.bc; E.bins = cfg->bins; E.prime_pad = L.prime_pad;
     E.enc_dims = cfg->encoder_dims; E.Bmax = cfg->max_batch; E.add_cond_after = cfg->add_cond_after;
     E.depth = cfg->depth; E.G = G; E.KS = L.KS; E.ks_shift = L.KS == 4 ? 2 : L.KS == 2 ? 1 : 0; E.U = L.U; E.RC = L.RC; E.nslot = L.nslot; E.uni_bytes = L.uni_bytes; E.kvpre_bytes = L.kvpre_bytes; E.small_bytes = (int)L.small_per_layer; E.prof_on = getenv("JK_PROFILE") ? 1 : 0;
-    E.kv_prefetch = getenv("JK_KV_PREFETCH") ? atoi(getenv("JK_KV_PREFETCH")) : 1;
     {
         const int nowait = getenv("JK_NOWAIT") ? atoi(getenv("JK_NOWAIT")) : 0;
         JK_CHECK_CUDA(cudaMemcpyToSymbol(jk_nowait, &nowait, sizeof(int)));
@@ -2062,12 +1911,12 @@ extern "C" int jk_prior_create(const jk_prior_config* cfg, void* arena, size_t a
     E.ll_qkv = (unsigned long long*)(A + L.off_qkv); E.ll_a = (unsigned long long*)(A + L.off_a);
     E.ll_g = (unsigned long long*)(A + L.off_g);
     for (int gi = 0; gi < 4; ++gi) E.xp[gi] = (unsigned long long*)(A + L.off_xp[gi]);
-    E.part = (float*)(A + L.off_part);
-    E.acnt = (unsigned*)(A + L.off_acnt); E.prof = (unsigned long long*)(A + L.off_prof);
+    E.part = (unsigned long long*)(A + L.off_part);
+    E.prof = (unsigned long long*)(A + L.off_prof);
     E.lnacc = (long long*)(A + L.off_lnacc);
     E.prof2 = (long long*)(A + L.off_prof2);
     E.prof3 = (unsigned long long*)(A + L.off_prof3);
-    E.sync = (unsigned*)(A + L.off_sync); E.t = (int*)(E.sync + 96);
+    E.step = (unsigned*)(A + L.off_step); E.t = (int*)(A + L.off_step + 128);
     size_t enc_off = L.off_small + L.small_per_layer * cfg->depth;
     for (int i = 0; i < 4; ++i) { p->bias_ptr[i].resize(cfg->depth); p->ln_ptr[i].resize(cfg->depth); }
     p->enc_w.assign(cfg->depth, nullptr); p->enc_b.assign(cfg->depth, nullptr);
@@ -2085,10 +1934,6 @@ extern "C" int jk_prior_create(const jk_prior_config* cfg, void* arena, size_t a
         for (int i = 0; i < 4; ++i) { p->ln_ptr[i][l] = s; s += cfg->width; }
         LD.b_qkv = p->bias_ptr[0][l]; LD.b_o = p->bias_ptr[1][l]; LD.b_1 = p->bias_ptr[2][l]; LD.b_2 = p->bias_ptr[3][l];
         LD.ln0_g = p->ln_ptr[0][l]; LD.ln0_b = p->ln_ptr[1][l]; LD.ln1_g = p->ln_ptr[2][l]; LD.ln1_b = p->ln_ptr[3][l];
-        if (getenv("JK_DEBUG_PARAMS0") && l > 0) {      // tuning aid: every layer reads layer 0's small parameters (results are garbage)
-            LD.b_qkv = E.layer[0].b_qkv; LD.b_o = E.layer[0].b_o; LD.b_1 = E.layer[0].b_1; LD.b_2 = E.layer[0].b_2;
-            LD.ln0_g = E.layer[0].ln0_g; LD.ln0_b = E.layer[0].ln0_b; LD.ln1_g = E.layer[0].ln1_g; LD.ln1_b = E.layer[0].ln1_b;
-        }
         if (cfg->attn_func[l] == 6) {
             p->enc_w[l] = (__half*)(A + enc_off);
             p->enc_b[l] = (float*)(A + enc_off + (size_t)cfg->width * 2 * cfg->n_state * 2);
@@ -2272,7 +2117,7 @@ extern "C" int jk_prior_step(jk_prior* p, const jk_step_args* a, jk_stream_t str
 
 extern "C" int jk_prior_has_logits_gemm(const jk_prior* p, int* on) {
     JK_REQUIRE(p && on, "null argument");
-    *on = (JK_LOGITS_MMA && p->lg_on) ? 1 : 0;
+    *on = p->lg_on ? 1 : 0;
     return 0;
 }
 

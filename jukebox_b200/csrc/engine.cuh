@@ -22,7 +22,7 @@ struct EngineDev {
     int RC;                         // rows of one shared-memory K (or V) tile of the attention phase
     int ks_shift;                   // log2(KS)
     int KS, U;                      // K-split factor of every Conv1D and the number of column units (G = U * KS)
-    int nslot, uni_bytes, kvpre_bytes, small_bytes, prof_on, kv_prefetch;
+    int nslot, uni_bytes, kvpre_bytes, small_bytes, prof_on;
     float scale2;
     const ushort2* cols;            // [U][depth][4] : (first 8-column group, number of groups) of a unit
     const uint8_t* streams;
@@ -31,14 +31,16 @@ struct EngineDev {
     // written with one 8-byte store and polled by the consumer - no separate flag, no grid barrier
     unsigned long long *ll_h, *ll_x1, *ll_qkv, *ll_a, *ll_g;   // [16][N/2]
     unsigned long long* xp[4];      // K-split partial sums {fp32, flag}: [G][16][64] per Conv1D of a layer
-    float* part;                    // split-KV partials [Bmax*H*kMaxSplit][dh_pad + 2]
-    unsigned* acnt;                 // [Bmax*H] merge tickets
-    long long* lnacc;               // [2*depth][16][2] fixed-point LayerNorm accumulators (sum, sumsq), 128-B apart
+    unsigned long long* part;       // split-KV partials as LL words {fp32, flag}: [Bmax*H][kMaxSplit][m, l, dh_pad outputs]
+    // LayerNorm statistics: 2*depth+1 blocks of 512 words; row r's fixed-point {sum, sumsq} are words 16r and 16r+1
+    // (one 128-B line per row), the contributor count in their top bits.  Block 2l feeds layer l's LN0, 2l+1 its LN1;
+    // block 2*depth (the final residual stream) only tells the housekeeping warp that every CTA is through the stack.
+    long long* lnacc;
     long long* prof2;               // [kProfSlots][8] intra-phase clock64 stamps of CTA 0 (tuning aid)
     unsigned long long* prof3;      // [5][256][2] per-CTA phase entry / exit times of layer 1
     unsigned long long* prof;       // [kProfSlots] phase timestamps of CTA 0 (globaltimer ns)
-    unsigned* sync;                 // [0] LN0 arrivals, [32] LN1 arrivals, [64] steps executed (one 128-B line each)
-    int* t;
+    unsigned* step;                 // steps executed so far (flags of the next launch derive from it)
+    int* t;                         // position of the next step; on its own 128-B line, apart from `step`
     const float *x_emb, *pos_emb, *x_out, *start_token;
     const int* lrow0;               // [G+1] logits rows per CTA (prefix)
     // logits as a fifth Conv1D on the tensor cores (decode_engine.cu "logits GEMM"): 0 when the configuration keeps
