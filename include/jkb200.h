@@ -24,7 +24,7 @@ extern "C" {
 #endif
 
 #define JK_MAX_DEPTH 96
-#define JK_MAX_BATCH 16
+#define JK_MAX_BATCH 32
 
 typedef void* jk_stream_t;          /* cudaStream_t */
 
@@ -43,7 +43,7 @@ int jk_device_sm_count(int* out);
  * its KV cache (transformer/factored_attention.py:230-301, 328-373), MLP + quick_gelu
  * (transformer.py:19-30, ops.py:33-35) -> +cond -> x_out logits (autoregressive.py:226-229).
  *
- * One jk_prior_step call = one token position for up to 16 samples, executed by ONE persistent
+ * One jk_prior_step call = one token position for up to 32 samples, executed by ONE persistent
  * kernel (grid = #SMs) that streams every layer's fp16 weights once through a TMA bulk-copy
  * ring in shared memory.  The position is read from device memory, so the call sequence is
  * CUDA-graph capturable.

@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libjkb200.so")
 
 JK_MAX_DEPTH = 96
-JK_MAX_BATCH = 16
+JK_MAX_BATCH = 32
 
 
 class PriorConfig(C.Structure):

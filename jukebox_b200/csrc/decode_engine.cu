@@ -1,6 +1,6 @@
 // Persistent decode-step engine for Jukebox's autoregressive priors on H100 (sm_90a).
 //
-// One launch = one token position for up to 16 samples through the WHOLE transformer stack
+// One launch = one token position for up to 32 samples through the WHOLE transformer stack
 // (reference: ConditionalAutoregressive2D.sample loop body, prior/autoregressive.py:222-237,
 //  -> Transformer.forward(sample=True), transformer/transformer.py:169-192).
 //
@@ -53,13 +53,18 @@ constexpr int kThreads = 384;          // 2 consumer warpgroups (8 warps) + 1 pr
 constexpr int kSlotBytes = 16384;
 constexpr int kMaxSlots = 12;
 constexpr int kHeaderBytes = 8192;     // barriers, LN statistics, descriptor / layer records, residual slice
-constexpr int kLogitKT = 1024;         // K tile (floats) of the fp32 logits product
+constexpr int kLogitKT = 1024;         // K tile (floats) of the fp32 logits product at 16 rows
 constexpr int kLogitRowsPerChunk = 4;
 constexpr int kLogitRowsPerPass = 16;
 constexpr int kMaxSplit = 4;
 constexpr int kProfSlots = 1024;
 constexpr int kXpCols = 64;            // columns per unit in the partial-sum exchange (8 groups of 8)
-constexpr int kRedBytes = 8 * 16 * 72 * 4;   // cross-warp reduction tile [8 warps][16 rows][<= 72 floats]
+// The decode kernel is instantiated for R = 16 and R = 32 activation rows (the M of the MMAs: one or two m16 tiles
+// against every weight fragment); jk_prior_step launches the 16-row kernel whenever n_samples <= 16.
+// cross-warp reduction tile [8 warps][R rows][<= 72 floats]
+__host__ __device__ constexpr int red_bytes(int R) { return 8 * R * 72 * 4; }
+// K tile of the fp32 logits product: its y tile [R][kt] floats stays at 64 KB
+__host__ __device__ constexpr int logit_kt(int R) { return kLogitKT * 16 / R; }
 // LayerNorm statistics words: [63:52] number of CTAs that have contributed, [51:0] fixed-point value
 constexpr int kCntShift = 52;
 constexpr unsigned long long kValMask = (1ull << kCntShift) - 1;
@@ -110,11 +115,12 @@ extern __shared__ __align__(1024) uint8_t jk_smem[];
 // Its header [0, kHeaderBytes): byte offset and size of every region, in address order.  Only the accessors below
 // address the header.
 constexpr int kHdrBar = 0, kHdrBarBytes = 2 * kMaxSlots * 8;           // ring mbarriers: full[kMaxSlots], empty[kMaxSlots]
-constexpr int kHdrStats = 256, kHdrStatsBytes = 16 * 2 * 4;            // LayerNorm statistics [16 rows] {-mean * rstd, rstd}
+constexpr int kHdrStats = 256, kHdrStatsBytes = 32 * 2 * 4;            // LayerNorm statistics [R rows] {-mean * rstd, rstd}
 constexpr int kHdrDesc = 512, kHdrDescBytes = 512;                     // descriptor head: EngineDev up to `layer`
 constexpr int kHdrLayer = 1024, kHdrLayerSlot = 256;                   // two layer slots (layer l in slot l & 1): LayerDev,
 constexpr int kHdrColsAt = 128;                                        //   and at +kHdrColsAt this unit's ushort2 cols[4]
-constexpr int kHdrRes = 2048, kHdrResBytes = 16 * 32 * 8;              // residual-stream slice of this CTA: [16][32] float2
+constexpr int kHdrRes = 2048, kHdrResBytes = 16 * 32 * 8;              // residual-stream slice of this CTA, see res_ld()
+static_assert(kHdrResBytes == 32 * 32 * 4, "the 32-row residual slice (half2) must fill the 16-row one (float2)");
 constexpr int kHdrMap = 6144, kHdrMapBytes = 3 * kConsumers * 2;       // staging thread layouts [3 kinds][kConsumers]
 constexpr int kHdrMapDim = 7680, kHdrMapDimBytes = 3 * (int)sizeof(StageDim);
 constexpr int kHdrLaunch = 7712, kHdrLaunchBytes = (int)sizeof(LaunchVals);
@@ -132,7 +138,18 @@ static_assert(kHdrBar + kHdrBarBytes <= kHdrStats && kHdrStats + kHdrStatsBytes 
 __device__ __forceinline__ uint64_t* sm_full() { return reinterpret_cast<uint64_t*>(jk_smem + kHdrBar); }
 __device__ __forceinline__ uint64_t* sm_empty() { return sm_full() + kMaxSlots; }
 __device__ __forceinline__ float* sm_stats() { return reinterpret_cast<float*>(jk_smem + kHdrStats); }
-__device__ __forceinline__ float2* sm_res() { return reinterpret_cast<float2*>(jk_smem + kHdrRes); }
+// Entry i = row * 32 + column pair of this CTA's residual-stream slice: [16][32] float2 at 16 rows, [32][32] half2 at
+// 32 rows.  Every value stored is already fp16-rounded, so the half form is exact and the slice keeps its 4 KB.
+template <int R>
+__device__ __forceinline__ float2 res_ld(int i) {
+    if constexpr (R == 16) return reinterpret_cast<const float2*>(jk_smem + kHdrRes)[i];
+    else return __half22float2(reinterpret_cast<const __half2*>(jk_smem + kHdrRes)[i]);
+}
+template <int R>
+__device__ __forceinline__ void res_st(int i, float2 v) {
+    if constexpr (R == 16) reinterpret_cast<float2*>(jk_smem + kHdrRes)[i] = v;
+    else reinterpret_cast<__half2*>(jk_smem + kHdrRes)[i] = __floats2half2_rn(v.x, v.y);
+}
 __device__ __forceinline__ uint8_t* sm_uni() { return jk_smem + kHeaderBytes; }
 // The engine descriptor lives in global memory; with the shared-memory carve-out at its maximum there is
 // no L1 to cache it, so every `E->field` was an L2 round trip (~300 cycles) on the dependency chain.
@@ -240,16 +257,18 @@ __device__ __forceinline__ long long fx_sq(float x) { return __float2ll_rn(fminf
 __device__ __forceinline__ void red_add_u64(long long* p, unsigned long long v) {
     atomicAdd(reinterpret_cast<unsigned long long*>(p), v);
 }
-__device__ __forceinline__ long long* sm_sfx() { return reinterpret_cast<long long*>(sm_uni() + kRedBytes); }
+template <int R>
+__device__ __forceinline__ long long* sm_sfx() { return reinterpret_cast<long long*>(sm_uni() + red_bytes(R)); }
 
-// This CTA's contribution to the statistics block `ln_out` ([16 rows] x {sum, sumsq} adjacent, one 128-byte line per row).
-// sfx: [2][16 rows][32] fixed-point values of the column pairs it wrote.  32 threads each
+// This CTA's contribution to the statistics block `ln_out` ([32 rows] x {sum, sumsq} adjacent, one 128-byte line per row).
+// sfx: [2][32 rows][32] fixed-point values of the column pairs it wrote.  32 threads each
 // reduce one (row, moment) in a fixed order and issue ONE 64-bit red carrying value + count.
+template <int R>
 __device__ __forceinline__ void publish_stats(long long* ln_out, int B, int ppc) {
     const int tid = threadIdx.x;
     consumer_sync();
     if (tid < 2 * B) {
-        const long long* sfx = sm_sfx() + (tid & 1) * 1024;
+        const long long* sfx = sm_sfx<R>() + (tid & 1) * 1024;
         const int row = tid >> 1;
         long long s = (tid & 1) ? 0 : kSumBias;
         for (int i = 0; i < ppc; ++i) s += sfx[row * 32 + i];
@@ -258,12 +277,12 @@ __device__ __forceinline__ void publish_stats(long long* ln_out, int B, int ppc)
     consumer_sync();                       // the scratch is reused by the next phase
 }
 
-// activation staging: LL words of rows [0, B), columns [k0, k0 + Ks) -> shared fp16 [16][Ks+8] (ldmatrix
+// activation staging: LL words of rows [0, B), columns [k0, k0 + Ks) -> shared fp16 [R][Ks+8] (ldmatrix
 // friendly), optionally through LayerNorm (fp32 math, eps 1e-5; reference transformer/ops.py:14-24).
 // Threads are laid out [row group][8-column vector]: a thread keeps ONE column vector (gamma / beta loaded
 // once) and walks rows rg, rg + rgc, ...; four rows = eight 16-byte polled loads in flight per batch.
 // Rows >= B are never written: an MMA output row depends only on its own A row, and those outputs are discarded.
-// How the 256 consumer threads tile a [16 rows][Ks / 8 vectors] slice: cw column vectors per pass x rgc row groups,
+// How the 256 consumer threads tile a [R rows][Ks / 8 vectors] slice: cw column vectors per pass x rgc row groups,
 // thread -> (column vector cv, row group rg).  Computed once per launch for the three K of a layer (kind 0: width,
 // 1: n_state, 2: mlp width) and kept in the shared-memory header: sm_stage_map(kind)[tid] = cv | rg << 8,
 // sm_stage_dim(kind) = {cw, rgc} - so no integer division sits on the path of a phase.
@@ -278,16 +297,17 @@ __device__ __forceinline__ void stage_map_init(int kind, int Ks) {
     }
 }
 
-__device__ __noinline__ void stage_acts(const unsigned long long* in, int K, int k0, int Ks, int B, uint32_t flag, int ln,
-                                        const float* gamma, const float* beta, const long long* lnacc, int kind, int pslot) {
+template <int R>
+__device__ __forceinline__ void stage_acts_body(const unsigned long long* in, int K, int k0, int Ks, int B, uint32_t flag, int ln,
+                                                const float* gamma, const float* beta, const long long* lnacc, int kind, int pslot) {
     const int tid = threadIdx.x;
     uint8_t* acts = sm_uni();
     float* stats = sm_stats();
     const int nvec = Ks >> 3;
     const int astride = (Ks + 8) * 2;
-    // LayerNorm statistics of the 16 rows: lane r polls the two adjacent words (sum, sum of squares) of row r with one
-    // 16-byte load until every CTA has contributed to both (16 pollers per CTA on 16 lines).  Called AFTER this thread's
-    // activation loads are issued: on the 16 polling threads the two latencies overlap instead of adding up.
+    // LayerNorm statistics of the R rows: thread r polls the two adjacent words (sum, sum of squares) of row r with one
+    // 16-byte load until every CTA has contributed to both (R pollers per CTA on R lines).  Called AFTER this thread's
+    // activation loads are issued: on the R polling threads the two latencies overlap instead of adding up.
     auto row_statistics = [&]() {
         const int G = sm_E()->G;
         float mean = 0.f, rstd = 0.f;
@@ -327,7 +347,7 @@ __device__ __noinline__ void stage_acts(const unsigned long long* in, int K, int
             *reinterpret_cast<float4*>(bt + 4) = __ldg(reinterpret_cast<const float4*>(beta + k0 + v * 8 + 4));
         }
 #pragma unroll 1
-        for (int r0 = rg; r0 < 16; r0 += 4 * rgc) {          // uniform trip count per thread group: barrier below
+        for (int r0 = rg; r0 < R; r0 += 4 * rgc) {           // uniform trip count per thread group: barrier below
             ulonglong2 w[4][2];
             auto issue = [&]() {
 #pragma unroll
@@ -341,7 +361,7 @@ __device__ __noinline__ void stage_acts(const unsigned long long* in, int K, int
                 }
             };
             if (act) issue();
-            if (!stats_ready && tid < 16) row_statistics();      // (ln only) while the loads above are in flight
+            if (!stats_ready && tid < R) row_statistics();       // (ln only) while the loads above are in flight
             if (act) {
                 unsigned spins = 0;
                 for (;;) {
@@ -384,7 +404,16 @@ __device__ __noinline__ void stage_acts(const unsigned long long* in, int K, int
             }
         }
     }
-    if (!stats_ready) { if (tid < 16) row_statistics(); consumer_sync(); }
+    if (!stats_ready) { if (tid < R) row_statistics(); consumer_sync(); }
+}
+// The 16-row GEMM phase calls the staging as a function of its own; the 32-row one inlines it.  Called at 32 rows, the
+// staging left gemm_phase too few registers for what it keeps across the call: ptxas put one word (the return address)
+// in local memory, an L2 round trip per phase.  Without the call the staging's registers and the two accumulator sets
+// are simply disjoint live ranges.
+template <int R>
+__device__ __noinline__ void stage_acts(const unsigned long long* in, int K, int k0, int Ks, int B, uint32_t flag, int ln,
+                                        const float* gamma, const float* beta, const long long* lnacc, int kind, int pslot) {
+    stage_acts_body<R>(in, K, k0, Ks, B, flag, ln, gamma, beta, lnacc, kind, pslot);
 }
 
 __device__ __forceinline__ uint2 lds64(uint32_t addr) {
@@ -399,30 +428,36 @@ __device__ __forceinline__ void ldsm4(uint32_t (&r)[4], uint32_t addr) {
 // nk k-steps of one ring slot, by one warp: its k-steps x column groups are independent MMAs that pipeline back to
 // back.  NCG (8-column groups of this unit) is a template parameter: with a run-time count the compiler serialised
 // every LDS -> HMMA pair through one register pair (tools/micro/ubench.cu: 4070 vs 1170 cycles for the K = 2048 loop).
-template <int NCG>
-__device__ __forceinline__ void mma_chunk(float (&acc)[8][4], uint32_t arow, uint32_t sl, int kk0, int nk) {
-#pragma unroll 4
+// MT m16 row tiles (R = 16 * MT rows; tile m starts at arow + m * atile): each B fragment is loaded from the ring slot
+// once and multiplied into MT accumulator sets.  With two tiles one k-step already issues 2 * NCG independent MMAs, and
+// the loop stays rolled: unrolled by 2 it made gemm_phase<32> spill (STL 1 / LDL 2, and STL 11 in the kernel body).
+template <int NCG, int MT>
+__device__ __forceinline__ void mma_chunk(float (&acc)[MT][8][4], uint32_t arow, uint32_t atile, uint32_t sl, int kk0, int nk) {
+#pragma unroll (MT == 1 ? 4 : 1)
     for (int i = 0; i < nk; ++i) {
-        uint32_t a[4];
-        ldsm4(a, arow + (kk0 + i) * 32);
+        uint32_t a[MT][4];
+#pragma unroll
+        for (int m = 0; m < MT; ++m) ldsm4(a[m], arow + m * atile + (kk0 + i) * 32);
         uint2 b[NCG];
 #pragma unroll
         for (int j = 0; j < NCG; ++j) b[j] = lds64(sl + ((i * NCG + j) << 8));
 #pragma unroll
-        for (int j = 0; j < NCG; ++j) mma_16816(acc[j], a, b[j].x, b[j].y);
+        for (int m = 0; m < MT; ++m)
+#pragma unroll
+            for (int j = 0; j < NCG; ++j) mma_16816(acc[m][j], a[m], b[j].x, b[j].y);
     }
 }
 
 // ---------------------------------------------------------------------------------------
 // one Conv1D at decode.  Unit u owns columns [8*g0, 8*(g0+ncg)); this CTA (rank r of the unit) owns the K slice
-// [r*K/KS, (r+1)*K/KS):  partial[16, 8*ncg] = acts[16, K/KS] . Wslice, exchanged inside the unit, and this CTA
+// [r*K/KS, (r+1)*K/KS):  partial[R, 8*ncg] = acts[R, K/KS] . Wslice, exchanged inside the unit, and this CTA
 // finishes column pairs [r*ppc, (r+1)*ppc) of the unit: out = epilogue(sum of the KS partials in rank order).
 // ---------------------------------------------------------------------------------------
 enum { EPI_QKV = 0, EPI_PROJ = 1, EPI_FC = 2, EPI_PROJ2 = 3, EPI_LOGITS = 4 };
 
 struct GemmArgs {
-    const unsigned long long* in;       // LL input [16][K/2]
-    unsigned long long* out;            // LL output [16][N/2]
+    const unsigned long long* in;       // LL input [rows][K/2]
+    unsigned long long* out;            // LL output [rows][N/2]
     unsigned long long* xp;             // partial-sum exchange of this Conv1D index
     int K, N, g0, ncg, ln, epi, pslot;
     uint32_t flag_in, flag_out;
@@ -441,6 +476,7 @@ struct GemmArgs {
 // descriptor / layer record / column table in shared memory: passed by value it had grown past what the call ABI keeps in
 // registers (896 bytes of stack), and with the shared-memory carve-out at its maximum every local-memory access is an L2
 // round trip - the step went from 1.95 to 2.5 ms.
+template <int R>
 __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int pslot_, uint32_t fl) {
     const EngineDev* E = sm_E();
     GemmArgs g;
@@ -480,24 +516,29 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
     const bool residual = (g.epi == EPI_PROJ || g.epi == EPI_PROJ2);
     STAMP(E, g.pslot, 0);
     if (ncg == 0) {                                      // a unit without columns (tiny models) still contributes (count only)
-        if (residual) publish_stats(g.ln_out, B, 0);
+        if (residual) publish_stats<R>(g.ln_out, B, 0);
         return ring;
     }
     const int K = g.K, N = g.N, epi = g.epi;
     const int Ks = K >> ksh;
     // the logits GEMM multiplies [y | y] with [hi(x_out) ; lo(x_out)]: its K runs twice over the kin input columns
     const int k0 = rank * Ks - (rank * Ks >= g.kin ? g.kin : 0);
-    stage_acts(g.in, g.kin, k0, Ks, B, g.flag_in, g.ln, g.gamma, g.beta, g.ln_in, g.kind, g.pslot);
+    if constexpr (R == 16) stage_acts<R>(g.in, g.kin, k0, Ks, B, g.flag_in, g.ln, g.gamma, g.beta, g.ln_in, g.kind, g.pslot);
+    else stage_acts_body<R>(g.in, g.kin, k0, Ks, B, g.flag_in, g.ln, g.gamma, g.beta, g.ln_in, g.kind, g.pslot);
     consumer_sync();
     STAMP(E, g.pslot, 1);
 
-    float acc[8][4];
+    constexpr int MT = R / 16;                            // m16 row tiles
+    float acc[MT][8][4];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) { acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f; }
+    for (int m = 0; m < MT; ++m)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { acc[m][j][0] = acc[m][j][1] = acc[m][j][2] = acc[m][j][3] = 0.f; }
     const int nkk = Ks >> 4;
     const int kpc = kpc_of(ncg);                          // a power of two
     const int astride = (Ks + 8) * 2;
     const uint32_t arow = smem_u32(uni + (lane & 15) * astride + (lane >> 4) * 16);
+    const uint32_t atile = 16 * astride;
     // The k-steps of this CTA's slice are dealt to the eight warps in contiguous runs (k-step i -> warp i * 8 / nkk), so
     // every warp multiplies - 4 k-steps each for a K = 2048 / KS = 4 phase instead of four warps with a whole slot each and
     // four idle.  EVERY warp still waits for every slot and arrives on its empty barrier, in order: the parity protocol of
@@ -523,7 +564,7 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
             if (in_order) { a_ = kk0; b_ = ((slot_i & 7) == warp) ? min(kk0 + kpc, nkk) : kk0; } \
             if (a_ < b_ || in_order) mbar_wait(ring.full(), ring.phase);                       \
             if (a_ < b_)                                                                      \
-                mma_chunk<NCG>(acc, arow, smem_u32(ring.data()) + lane * 8 + (((a_ - kk0) * NCG) << 8), a_, b_ - a_); \
+                mma_chunk<NCG, MT>(acc, arow, atile, smem_u32(ring.data()) + lane * 8 + (((a_ - kk0) * NCG) << 8), a_, b_ - a_); \
             __syncwarp();                                                                      \
             if (lane == 0) mbar_arrive(ring.empty());                                          \
             ring.advance();                                                                   \
@@ -544,20 +585,23 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
     const int nwarp = in_order ? min(8, nslots_phase) : min(8, nkk);       // warps that multiplied at least one k-step
     float* red = reinterpret_cast<float*>(uni);
     const int ncp = ((nc + 31) & ~31) + 8;
-    // partial sums of the unit: [KS ranks][16 rows][64 columns] LL words {fp32, flag}
-    unsigned long long* xp_unit = g.xp + (size_t)(c - rank) * 16 * kXpCols;
+    // partial sums of the unit: [KS ranks][R rows][64 columns] LL words {fp32, flag}
+    unsigned long long* xp_unit = g.xp + (size_t)(c - rank) * R * kXpCols;
     {
         consumer_sync();                   // everyone is done reading the staged activations
-        // cross-warp reduction tile [warps that owned a slot][16 rows][ncp floats]; ncp = 8 mod 32 keeps both the fragment
+        // cross-warp reduction tile [warps that owned a slot][R rows][ncp floats]; ncp = 8 mod 32 keeps both the fragment
         // stores below and the row-wise pair loads of the epilogue free of bank conflicts
         if (warp < nwarp) {
             const int r0 = lane >> 2, c0 = (lane & 3) * 2;
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                if (j < ncg) {
-                    float* d = red + (size_t)(warp * 16) * ncp + j * 8 + c0;
-                    *reinterpret_cast<float2*>(d + r0 * ncp) = make_float2(acc[j][0], acc[j][1]);
-                    *reinterpret_cast<float2*>(d + (r0 + 8) * ncp) = make_float2(acc[j][2], acc[j][3]);
+            for (int m = 0; m < MT; ++m) {
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    if (j < ncg) {
+                        float* d = red + (size_t)(warp * R + m * 16) * ncp + j * 8 + c0;
+                        *reinterpret_cast<float2*>(d + r0 * ncp) = make_float2(acc[m][j][0], acc[m][j][1]);
+                        *reinterpret_cast<float2*>(d + (r0 + 8) * ncp) = make_float2(acc[m][j][2], acc[m][j][3]);
+                    }
                 }
             }
         }
@@ -569,10 +613,10 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
             for (int b = warp; b < B; b += 8) {
                 float s0 = 0.f, s1 = 0.f;
                 for (int w = 0; w < nwarp; ++w) {
-                    const float2 v = *reinterpret_cast<const float2*>(red + (size_t)(w * 16 + b) * ncp + 2 * lane);
+                    const float2 v = *reinterpret_cast<const float2*>(red + (size_t)(w * R + b) * ncp + 2 * lane);
                     s0 += v.x; s1 += v.y;
                 }
-                unsigned long long* dst = xp_unit + ((size_t)rank * 16 + b) * kXpCols + 2 * lane;
+                unsigned long long* dst = xp_unit + ((size_t)rank * R + b) * kXpCols + 2 * lane;
                 const unsigned long long fl = (unsigned long long)g.flag_in << 32;
                 asm volatile(JK_ST_LL ".v2.u64 [%0], {%1,%2};" ::"l"(dst), "l"(fl | __float_as_uint(s0)),
                              "l"(fl | __float_as_uint(s1)) : "memory");
@@ -581,10 +625,9 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
     }
     STAMP(E, g.pslot, 3);
     // ---- ... and finishes its own column pairs ----------------------------------------------------------
-    float2* res = sm_res();
-    long long* sfx = sm_sfx();                                        // [2][16][32] statistics of the pairs written
-    // thread layout: up to 16 pairs per CTA (every K-split configuration): half-warp = sample row (2 * warp + half),
-    // lane & 15 = column pair, one pass; more pairs (KS = 1): lane = pair, rows warp and warp + 8
+    long long* sfx = sm_sfx<R>();                                     // [2][32][32] statistics of the pairs written
+    // thread layout: up to 16 pairs per CTA (every K-split configuration): half-warp = sample row (2 * warp + half, + 16),
+    // lane & 15 = column pair; more pairs (KS = 1): lane = pair, rows warp, warp + 8, ...
     const bool two_rows = ppc <= 16;
     const int pl = two_rows ? (lane & 15) : lane;
     const int b_first = two_rows ? 2 * warp + (lane >> 4) : warp, b_step = two_rows ? 16 : 8;
@@ -597,7 +640,7 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
             float s0 = 0.f, s1 = 0.f;
             if (KS == 1) {
                 for (int w = 0; w < nwarp; ++w) {
-                    const float2 v = *reinterpret_cast<const float2*>(red + (size_t)(w * 16 + b) * ncp + 2 * pr);
+                    const float2 v = *reinterpret_cast<const float2*>(red + (size_t)(w * R + b) * ncp + 2 * pr);
                     s0 += v.x; s1 += v.y;
                 }
             } else {
@@ -610,7 +653,7 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
                     again = false;
 #pragma unroll
                     for (int q = 0; q < 4; ++q)
-                        if (q < KS) v[q] = ll_ld2(xp_unit + ((size_t)q * 16 + b) * kXpCols + 2 * pr);
+                        if (q < KS) v[q] = ll_ld2(xp_unit + ((size_t)q * R + b) * kXpCols + 2 * pr);
 #pragma unroll
                     for (int q = 0; q < 4; ++q)
                         if (q < KS) again |= !(ll_ok(v[q].x, g.flag_in) && ll_ok(v[q].y, g.flag_in));
@@ -635,9 +678,9 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
                 o = __floats2half2_rn(quick_gelu_f(y0), quick_gelu_f(y1));
             } else {
                 // EPI_PROJ : x1 = fp16(h + a)      EPI_PROJ2 : h = fp16(x1 + m)   (transformer.py:82-83)
-                const float2 base = res[b * 32 + pl];
+                const float2 base = res_ld<R>(b * 32 + pl);
                 const float o0 = h2f_round(base.x + y0), o1 = h2f_round(base.y + y1);
-                res[b * 32 + pl] = make_float2(o0, o1);
+                res_st<R>(b * 32 + pl, make_float2(o0, o1));
                 o = __floats2half2_rn(o0, o1);
                 sfx[b * 32 + pl] = fx_sum(o0) + fx_sum(o1);
                 sfx[1024 + b * 32 + pl] = fx_sq(o0) + fx_sq(o1);
@@ -646,7 +689,7 @@ __device__ __noinline__ Ring gemm_phase(Ring ring, int B, int epi_, int l, int p
         }
     }
     STAMP(E, g.pslot, 4);
-    if (residual) publish_stats(g.ln_out, B, ppc);
+    if (residual) publish_stats<R>(g.ln_out, B, ppc);
     else consumer_sync();                  // red region is reused by the next phase
     return ring;
 }
@@ -1052,6 +1095,7 @@ __device__ __noinline__ int attn_prefetch(const LayerDev& LD_ref, int B, int c, 
 // ---------------------------------------------------------------------------------------
 // producer warp: walks this CTA's weight stream (and the logits rows) in consumption order
 // ---------------------------------------------------------------------------------------
+template <int R>
 __device__ __noinline__ void producer_loop(const EngineDev* E, Ring ring, int do_logits, int c) {
     if ((threadIdx.x & 31) != 0) return;
     const uint8_t* src = E->streams + (size_t)c * E->stream_stride;
@@ -1102,8 +1146,8 @@ __device__ __noinline__ void producer_loop(const EngineDev* E, Ring ring, int do
         const int W = E->W;
         for (int pr = r0; pr < r1; pr += kLogitRowsPerPass) {
             const int pe = min(r1, pr + kLogitRowsPerPass);
-            for (int k0 = 0; k0 < W; k0 += kLogitKT) {
-                const int kt = min(kLogitKT, W - k0);
+            for (int k0 = 0; k0 < W; k0 += logit_kt(R)) {
+                const int kt = min(logit_kt(R), W - k0);
                 for (int r = pr; r < pe; r += kLogitRowsPerChunk) {
                     const int nr = min(kLogitRowsPerChunk, pe - r);
                     mbar_wait(ring.empty(), ring.phase ^ 1u);
@@ -1120,7 +1164,10 @@ __device__ __noinline__ void producer_loop(const EngineDev* E, Ring ring, int do
 
 // fp32 logits: logits[b, r] = sum_k y[b, k] * x_out[r, k],  y = float(h) (+ cond)
 // (reference autoregressive.py:226-229: fp32 nn.Linear on the fp32 transformer output)
+// Warp w owns the sample rows [w * R / 8, (w + 1) * R / 8): every x_out row is streamed once whatever R.
+template <int R>
 __device__ __noinline__ void logits_phase(const StepArgs& A_ref, Ring& ring_ref, int c, int t, uint32_t flag) {
+    constexpr int RPW = R / 8;                      // sample rows per warp: 2 or 4
     const EngineDev* E = sm_E();
     uint8_t* uni = sm_uni();
     const StepArgs A = A_ref;
@@ -1128,18 +1175,22 @@ __device__ __noinline__ void logits_phase(const StepArgs& A_ref, Ring& ring_ref,
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int r0 = E->lrow0[c], r1 = E->lrow0[c + 1];
     const int W = E->W, B = A.n;
-    float* ys = reinterpret_cast<float*>(uni);     // [16][kt]
+    float* ys = reinterpret_cast<float*>(uni);     // [R][kt]
     for (int pr = r0; pr < r1; pr += kLogitRowsPerPass) {
         const int pe = min(r1, pr + kLogitRowsPerPass);
-        float acc[kLogitRowsPerPass][2];
+        float acc[kLogitRowsPerPass][RPW];
 #pragma unroll
         for (int i = 0; i < kLogitRowsPerPass; ++i) acc[i][0] = acc[i][1] = 0.f;
-        for (int k0 = 0; k0 < W; k0 += kLogitKT) {
-            const int kt = min(kLogitKT, W - k0);
+        if constexpr (RPW == 4) {
+#pragma unroll
+            for (int i = 0; i < kLogitRowsPerPass; ++i) acc[i][2] = acc[i][3] = 0.f;
+        }
+        for (int k0 = 0; k0 < W; k0 += logit_kt(R)) {
+            const int kt = min(logit_kt(R), W - k0);
             consumer_sync();
             {   // y = float(h) (+ cond): the final residual stream as LL words, 4 halves per 16-byte polled load
                 const int nv = kt >> 2;
-                for (int idx0 = tid; idx0 < 16 * nv; idx0 += 4 * kConsumers) {
+                for (int idx0 = tid; idx0 < R * nv; idx0 += 4 * kConsumers) {
                     ulonglong2 hv[4];
                     unsigned spins = 0;
                     bool again;
@@ -1149,7 +1200,7 @@ __device__ __noinline__ void logits_phase(const StepArgs& A_ref, Ring& ring_ref,
                         for (int u = 0; u < 4; ++u) {
                             const int idx = idx0 + u * kConsumers;
                             const int b = idx / nv, v = idx - b * nv;
-                            if (idx < 16 * nv && b < B) {
+                            if (idx < R * nv && b < B) {
                                 hv[u] = ll_ld2(E->ll_h + (((size_t)b * W + k0 + v * 4) >> 1));
                                 again |= !(ll_ok(hv[u].x, flag) && ll_ok(hv[u].y, flag));
                             }
@@ -1159,7 +1210,7 @@ __device__ __noinline__ void logits_phase(const StepArgs& A_ref, Ring& ring_ref,
 #pragma unroll
                     for (int u = 0; u < 4; ++u) {
                         const int idx = idx0 + u * kConsumers;
-                        if (idx >= 16 * nv) continue;
+                        if (idx >= R * nv) continue;
                         const int b = idx / nv, v = idx - b * nv;
                         float4 y = make_float4(0.f, 0.f, 0.f, 0.f);
                         if (b < B) {
@@ -1178,7 +1229,7 @@ __device__ __noinline__ void logits_phase(const StepArgs& A_ref, Ring& ring_ref,
                 }
             }
             consumer_sync();
-            const float* y0 = ys + (warp * 2) * kt;
+            const float* y0 = ys + (warp * RPW) * kt;
             const float* y1 = y0 + kt;
 #pragma unroll
             for (int rc = 0; rc < kLogitRowsPerPass / kLogitRowsPerChunk; ++rc) {
@@ -1191,12 +1242,21 @@ __device__ __noinline__ void logits_phase(const StepArgs& A_ref, Ring& ring_ref,
                     for (int k = lane * 4; k < kt; k += 128) {      // rolled: this phase runs once per step, its code must stay small
                         float4 a0 = *reinterpret_cast<const float4*>(y0 + k);
                         float4 a1 = *reinterpret_cast<const float4*>(y1 + k);
+                        float4 a2, a3;
+                        if constexpr (RPW == 4) {
+                            a2 = *reinterpret_cast<const float4*>(y1 + kt + k);
+                            a3 = *reinterpret_cast<const float4*>(y1 + 2 * kt + k);
+                        }
 #pragma unroll
                         for (int i = 0; i < kLogitRowsPerChunk; ++i) {
                             if (i < nr) {
                                 float4 w4 = *reinterpret_cast<const float4*>(wsl + i * kt + k);
                                 acc[rc * kLogitRowsPerChunk + i][0] += a0.x * w4.x + a0.y * w4.y + a0.z * w4.z + a0.w * w4.w;
                                 acc[rc * kLogitRowsPerChunk + i][1] += a1.x * w4.x + a1.y * w4.y + a1.z * w4.z + a1.w * w4.w;
+                                if constexpr (RPW == 4) {
+                                    acc[rc * kLogitRowsPerChunk + i][2] += a2.x * w4.x + a2.y * w4.y + a2.z * w4.z + a2.w * w4.w;
+                                    acc[rc * kLogitRowsPerChunk + i][3] += a3.x * w4.x + a3.y * w4.y + a3.z * w4.z + a3.w * w4.w;
+                                }
                             }
                         }
                     }
@@ -1208,12 +1268,17 @@ __device__ __noinline__ void logits_phase(const StepArgs& A_ref, Ring& ring_ref,
         }
 #pragma unroll
         for (int i = 0; i < kLogitRowsPerPass; ++i) {
-            float v0 = warp_sum(acc[i][0]), v1 = warp_sum(acc[i][1]);
+            float v0 = warp_sum(acc[i][0]), v1 = warp_sum(acc[i][1]), v2 = 0.f, v3 = 0.f;
+            if constexpr (RPW == 4) { v2 = warp_sum(acc[i][2]); v3 = warp_sum(acc[i][3]); }
             const int r = pr + i;
             if (lane == 0 && r < pe) {
-                const int b0 = warp * 2;
+                const int b0 = warp * RPW;
                 if (b0 < B) A.logits[(size_t)b0 * A.logits_bstride + (size_t)t * A.logits_tstride + r] = v0;
                 if (b0 + 1 < B) A.logits[(size_t)(b0 + 1) * A.logits_bstride + (size_t)t * A.logits_tstride + r] = v1;
+                if constexpr (RPW == 4) {
+                    if (b0 + 2 < B) A.logits[(size_t)(b0 + 2) * A.logits_bstride + (size_t)t * A.logits_tstride + r] = v2;
+                    if (b0 + 3 < B) A.logits[(size_t)(b0 + 3) * A.logits_bstride + (size_t)t * A.logits_tstride + r] = v3;
+                }
             }
         }
     }
@@ -1226,6 +1291,8 @@ __device__ __noinline__ void logits_phase(const StepArgs& A_ref, Ring& ring_ref,
 // critical path of CTA 0 (and so of its unit) twice per layer.  The same warp publishes the position and the step count
 // at the end: the final block is complete only when every CTA is through the stack, and every CTA has read both words
 // long before that.
+// Lane l clears word l & 1 of rows l / 2 (+ 16): the R rows a launch of R rows adds to.
+template <int R>
 __device__ __noinline__ void cleaner_loop() {
     const EngineDev* E = sm_E();
     const int lane = threadIdx.x & 31, G = E->G, nblk = 2 * E->depth;
@@ -1234,9 +1301,11 @@ __device__ __noinline__ void cleaner_loop() {
     for (int i = 1; i <= nblk; ++i) {
         if (lane == 0) wait_stat_word(E->lnacc + (size_t)i * 512, G);
         __syncwarp();
-        (E->lnacc + (size_t)(i - 1) * 512)[16 * (lane >> 1) + (lane & 1)] = 0;
+#pragma unroll
+        for (int r = 0; r < R; r += 16) (E->lnacc + (size_t)(i - 1) * 512)[16 * (r + (lane >> 1)) + (lane & 1)] = 0;
     }
-    (E->lnacc + (size_t)nblk * 512)[16 * (lane >> 1) + (lane & 1)] = 0;
+#pragma unroll
+    for (int r = 0; r < R; r += 16) (E->lnacc + (size_t)nblk * 512)[16 * (r + (lane >> 1)) + (lane & 1)] = 0;
     if (lane == 0) {
         *E->t = t + 1;
         *E->step = step + 1;
@@ -1265,6 +1334,7 @@ __device__ __forceinline__ bool logits_on_mma(const StepArgs& A) {
     return E->lg_on && (!(E->add_cond_after && A.x_cond) || A.logit_bias);
 }
 
+template <int R>
 __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const EngineDev* __restrict__ Eg, StepArgs A) {
     const int tid = threadIdx.x, warp = tid >> 5;
     const int c = blockIdx.x;
@@ -1288,8 +1358,8 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
     // thread (65536 / 384); the producer warpgroup keeps 40 and hands the rest to the two consumer warpgroups.
     if (warp >= 8) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-        if (warp == 8) producer_loop(Eg, ring, wants_logits(A) ? (logits_on_mma(A) ? 2 : 1) : 0, c);
-        else if (warp == 9 && c == 0) cleaner_loop();
+        if (warp == 8) producer_loop<R>(Eg, ring, wants_logits(A) ? (logits_on_mma(A) ? 2 : 1) : 0, c);
+        else if (warp == 9 && c == 0) cleaner_loop<R>();
         return;
     }
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
@@ -1340,10 +1410,9 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
     {
         const ushort2 wc = sm_cols(0)[1];                   // column groups of width-W outputs
         const int ppc = (wc.y * 4) >> E->ks_shift;
-        float2* res = sm_res();
-        long long* sfx = sm_sfx();
+        long long* sfx = sm_sfx<R>();
         const int lane = tid & 31;
-        for (int b = warp; b < B && lane < ppc; b += 8) {     // lane = column pair, warp = sample row (and row + 8)
+        for (int b = warp; b < B && lane < ppc; b += 8) {     // lane = column pair, warp = sample row (and row + 8, ...)
             const int pl = lane;
             const int col = wc.x * 8 + 2 * (cta_rank() * ppc + pl);
             float2 x;
@@ -1362,12 +1431,12 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
             }
             const __half2 hh = __floats2half2_rn(x.x, x.y);
             const float2 hv = __half22float2(hh);
-            res[b * 32 + pl] = hv;
+            res_st<R>(b * 32 + pl, hv);
             sfx[b * 32 + pl] = fx_sum(hv.x) + fx_sum(hv.y);
             sfx[1024 + b * 32 + pl] = fx_sq(hv.x) + fx_sq(hv.y);
             ll_st(E->ll_h + (((size_t)b * E->W + col) >> 1), *reinterpret_cast<const uint32_t*>(&hh), launch_fbase() + 1);
         }
-        publish_stats(E->lnacc, B, ppc);     // statistics block 0: the input of layer 0's LN0
+        publish_stats<R>(E->lnacc, B, ppc);     // statistics block 0: the input of layer 0's LN0
     }
     PHASE_DONE();
 
@@ -1378,7 +1447,7 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
         const int pre = attn_prefetch(LD, B, c, launch_pos(), launch_pm(), launch_pd(), launch_gmax());
         // a fresh argument record per phase: nothing of it stays live across the calls in between
         if (l == 1) PROF3(0, 0);
-        ring = gemm_phase(ring, B, EPI_QKV, l, (int)nph, fl);
+        ring = gemm_phase<R>(ring, B, EPI_QKV, l, (int)nph, fl);
         if (l == 1) PROF3(0, 1);
         // next layer's record + column assignment -> the other shared-memory slot.  The descriptor is in
         // HBM (the weight stream evicts it from L2 every step): issue the loads here so their latency hides
@@ -1408,27 +1477,26 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
         if (l == 1) PROF3(1, 1);
         PHASE_DONE();
         if (l == 1) PROF3(2, 0);
-        ring = gemm_phase(ring, B, EPI_PROJ, l, (int)nph, fl);
+        ring = gemm_phase<R>(ring, B, EPI_PROJ, l, (int)nph, fl);
         if (l == 1) PROF3(2, 1);
         PHASE_DONE();
         if (l == 1) PROF3(3, 0);
-        ring = gemm_phase(ring, B, EPI_FC, l, (int)nph, fl);
+        ring = gemm_phase<R>(ring, B, EPI_FC, l, (int)nph, fl);
         if (l == 1) PROF3(3, 1);
         PHASE_DONE();
         if (l == 1) PROF3(4, 0);
         asm volatile("cp.async.wait_group 0;" ::: "memory");      // the next layer's record (issued a phase and a half ago)
-        ring = gemm_phase(ring, B, EPI_PROJ2, l, (int)nph, fl);
+        ring = gemm_phase<R>(ring, B, EPI_PROJ2, l, (int)nph, fl);
         if (l == 1) PROF3(4, 1);
         PHASE_DONE();
     }
     if (A.h_out) {      // Transformer.forward boundary: this CTA's slice of the residual stream
         const ushort2 wc = sm_cols(E->depth - 1)[1];
         const int ppc = (wc.y * 4) >> E->ks_shift;
-        const float2* res = sm_res();
         const int lane = tid & 31;
         for (int b = warp; b < B && lane < ppc; b += 8) {
             const int col = wc.x * 8 + 2 * (cta_rank() * ppc + lane);
-            *reinterpret_cast<float2*>(A.h_out + (size_t)b * E->W + col) = res[b * 32 + lane];
+            *reinterpret_cast<float2*>(A.h_out + (size_t)b * E->W + col) = res_ld<R>(b * 32 + lane);
         }
     }
     if (wants_logits(A) && logits_on_mma(A)) {
@@ -1455,11 +1523,11 @@ __global__ void __launch_bounds__(kThreads, 1) jk_decode_step_kernel(const Engin
         for (int p = 0; p < 4; ++p) {
             if (p < E->lg_np) {
                 pass_record(p);
-                ring = gemm_phase(ring, B, EPI_LOGITS, E->depth - 1, (int)nph + p, launch_fbase() + (uint32_t)E->depth + 1);
+                ring = gemm_phase<R>(ring, B, EPI_LOGITS, E->depth - 1, (int)nph + p, launch_fbase() + (uint32_t)E->depth + 1);
             }
         }
     } else if (wants_logits(A)) {
-        logits_phase(A, ring, c, launch_pos(), launch_fbase() + (uint32_t)E->depth + 1);
+        logits_phase<R>(A, ring, c, launch_pos(), launch_fbase() + (uint32_t)E->depth + 1);
     }
     if (c == 0) {
         consumer_sync();
@@ -1606,6 +1674,7 @@ struct Layout {
     std::vector<int> cache_rows;
     size_t small_per_layer;
     int dh, dh_pad, bc, prime_pad, uni_bytes, kvpre_bytes, nslot, smem_bytes, RC;
+    int R;                              // activation rows of the largest kernel this engine launches (16 or 32)
 };
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
@@ -1654,6 +1723,10 @@ int compute_layout(const jk_prior_config& c, int G, Layout& L) {
         L.KS = ks; L.U = G / ks;
     }
     const int KS = L.KS, U = L.U;
+    // Row count of the shared-memory layout: the 32-row kernel's when more than 16 samples may come.  The K split, the
+    // column plan and the streams do not depend on it.
+    L.R = c.max_batch > 16 ? 32 : 16;
+    const int R = L.R;
     L.cols.assign((size_t)U * depth * 4, make_ushort2(0, 0));
     L.goff.assign((size_t)G * depth * 4, 0);
     std::vector<unsigned long long> cum(U, 0);        // bytes per CTA of a unit (all ranks of a unit stream the same amount)
@@ -1698,7 +1771,8 @@ int compute_layout(const jk_prior_config& c, int G, Layout& L) {
         }
     }
     // logits GEMM (fifth Conv1D, K' = 2 * width: hi and lo fp16 halves of the fp32 x_out): planned when the K-split is even
-    // (a rank's K slice must not straddle the hi / lo boundary) and the doubled slice fits the activation tile.  A unit
+    // (a rank's K slice must not straddle the hi / lo boundary) and its [R][2 * width / KS + 8] fp16 tile fits in what the
+    // shared-memory union region holds anyway: 64 KB at 16 rows, the 88 KB of the cross-warp reduction at 32.  A unit
     // multiplies at most 8 column groups per pass (the partial-sum exchange holds 64 columns); wider vocabularies take more
     // passes, each with its own exchange buffer, so at most 4 (1b_lyrics on 132 SMs: 266 groups over 33 units, 2 passes).
     // Its records are appended to `cols` ([passes][U] entries) and `goff` ([passes][G] entries), pass after pass.
@@ -1707,8 +1781,9 @@ int compute_layout(const jk_prior_config& c, int G, Layout& L) {
         const int groups = (c.bins + 7) / 8;           // a ragged last group is padded with zero weights
         const int Kp = 2 * c.width;
         const int np = ((groups + U - 1) / U + 7) / 8;
+        const size_t tile_cap = std::max((size_t)65536, (size_t)red_bytes(R) + 2 * 1024 * 8);
         const bool ok = c.bins > 0 && KS >= 2 && (Kp / 16) % KS == 0 && c.width % (Kp / KS) == 0 &&
-                        (size_t)16 * (Kp / KS + 8) * 2 <= (size_t)65536 && np <= 4 && !getenv("JK_NO_LOGITS_MMA");
+                        (size_t)R * (Kp / KS + 8) * 2 <= tile_cap && np <= 4 && !getenv("JK_NO_LOGITS_MMA");
         if (ok) {
             L.lg_on = 1; L.lg_np = np;
             L.cols.resize((size_t)U * depth * 4 + (size_t)np * U, make_ushort2(0, 0));
@@ -1739,13 +1814,15 @@ int compute_layout(const jk_prior_config& c, int G, Layout& L) {
     for (int cta = 0; cta <= G; ++cta) L.lrow[cta] = (int)((long long)c.bins * cta / G);
 
     const int Kmax = std::max(c.width, std::max(c.n_state, c.mlp_width)) / KS;
-    const int act_rows = c.max_batch > 8 ? 16 : 8;      // rows >= n_samples of the A tile are never read back (see stage_acts)
+    // rows >= n_samples of the A tile are never read back (see stage_acts)
+    const int act_rows = R == 32 ? 32 : c.max_batch > 8 ? 16 : 8;
     const int max_smem = 232448;
     int RC = attn_tile_rows(L.dh_pad), nslot = 0;
     for (;; RC >>= 1) {
         size_t uni = (size_t)act_rows * (Kmax + 8) * 2;
-        uni = std::max(uni, (size_t)16 * kLogitKT * 4);       // also covers the logits GEMM's [16][2 W / KS + 8] fp16 tile (<= 64 KB)
-        uni = std::max(uni, (size_t)kRedBytes + 2 * 1024 * 8);                       // cross-warp reduction + statistics scratch
+        uni = std::max(uni, (size_t)R * logit_kt(R) * 4);    // fp32 logits y tile (64 KB)
+        if (L.lg_on) uni = std::max(uni, (size_t)R * (2 * c.width / KS + 8) * 2);     // the logits GEMM's A tile
+        uni = std::max(uni, (size_t)red_bytes(R) + 2 * 1024 * 8);                     // cross-warp reduction + statistics scratch
         const size_t kv_stage = (size_t)2 * RC * L.dh_pad * 2;                        // one K tile + one V tile
         size_t attn = kv_stage + (size_t)3 * L.dh_pad * 2 + 64 * 4 + (size_t)L.dh_pad * 4 + 64;   // tiles, q/k/v, scores, running output
         uni = std::max(uni, attn);
@@ -1756,11 +1833,17 @@ int compute_layout(const jk_prior_config& c, int G, Layout& L) {
     }
     L.RC = RC;
     nslot = std::min(nslot, kMaxSlots);
+    // More than 16 samples take the 32-row kernel, whose whole [32][K / KS + 8] activation tile must sit in shared memory
+    // next to the K/V tiles and at least 4 ring slots (5b_lyrics: K split 1, 308 KB).
+    JK_REQUIRE(R == 16 || nslot >= 4,
+               "max_batch %d > 16 needs a [32 x %d] fp16 activation tile (%zu bytes: K %d, K split %d) in the %d bytes of "
+               "shared memory per CTA, which leaves %d weight-ring slots (at least 4); this configuration takes at most 16 samples",
+               c.max_batch, Kmax + 8, (size_t)32 * (Kmax + 8) * 2, Kmax * KS, KS, max_smem, std::max(nslot, 0));
     JK_REQUIRE(nslot >= 2, "not enough shared memory for the weight ring (uni %d bytes)", L.uni_bytes);
     L.nslot = nslot;
     L.smem_bytes = kHeaderBytes + L.uni_bytes + L.kvpre_bytes + nslot * kSlotBytes;
     // ldmatrix always addresses 16 A-tile rows; with an 8-row tile rows 8..15 must still lie inside the allocation
-    JK_REQUIRE((size_t)kHeaderBytes + (size_t)16 * (Kmax + 8) * 2 <= (size_t)L.smem_bytes, "A tile exceeds shared memory");
+    JK_REQUIRE((size_t)kHeaderBytes + (size_t)std::max(16, act_rows) * (Kmax + 8) * 2 <= (size_t)L.smem_bytes, "A tile exceeds shared memory");
 
     size_t off = 0;
     L.off_dev = off; off = align_up(off + sizeof(EngineDev), 256);
@@ -1783,12 +1866,12 @@ int compute_layout(const jk_prior_config& c, int G, Layout& L) {
         off += 2 * bytes;
     }
     // LL activation buffers: 8 bytes per fp16 PAIR ({half2, flag})
-    L.off_h = off;   off = align_up(off + (size_t)16 * c.width * 4, 256);
-    L.off_x1 = off;  off = align_up(off + (size_t)16 * c.width * 4, 256);
-    L.off_qkv = off; off = align_up(off + (size_t)16 * 3 * c.n_state * 4, 256);
-    L.off_a = off;   off = align_up(off + (size_t)16 * c.n_state * 4, 256);
-    L.off_g = off;   off = align_up(off + (size_t)16 * c.mlp_width * 4, 256);
-    for (int gi = 0; gi < 4; ++gi) { L.off_xp[gi] = off; off = align_up(off + (size_t)G * 16 * kXpCols * 8, 256); }
+    L.off_h = off;   off = align_up(off + (size_t)R * c.width * 4, 256);
+    L.off_x1 = off;  off = align_up(off + (size_t)R * c.width * 4, 256);
+    L.off_qkv = off; off = align_up(off + (size_t)R * 3 * c.n_state * 4, 256);
+    L.off_a = off;   off = align_up(off + (size_t)R * c.n_state * 4, 256);
+    L.off_g = off;   off = align_up(off + (size_t)R * c.mlp_width * 4, 256);
+    for (int gi = 0; gi < 4; ++gi) { L.off_xp[gi] = off; off = align_up(off + (size_t)G * R * kXpCols * 8, 256); }
     L.off_part = off; off = align_up(off + (size_t)c.max_batch * c.heads * kMaxSplit * (L.dh_pad + 2) * 8, 256);      // LL words
     L.off_prof = off; off = align_up(off + (size_t)kProfSlots * 8, 256);
     L.off_prof2 = off; off = align_up(off + (size_t)kProfSlots * 8 * 8, 256);
@@ -1973,7 +2056,8 @@ extern "C" int jk_prior_create(const jk_prior_config* cfg, void* arena, size_t a
         JK_CHECK_CUDA(cudaGetDevice(&dev));
         JK_CHECK_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
         JK_REQUIRE(L.smem_bytes <= optin, "decode kernel needs %d bytes of shared memory, device allows %d", L.smem_bytes, optin);
-        JK_CHECK_CUDA(cudaFuncSetAttribute(jk_decode_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
+        JK_CHECK_CUDA(cudaFuncSetAttribute(jk_decode_step_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
+        JK_CHECK_CUDA(cudaFuncSetAttribute(jk_decode_step_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
     }
     *out = p;
     return 0;
@@ -2109,8 +2193,10 @@ extern "C" int jk_prior_step(jk_prior* p, const jk_step_args* a, jk_stream_t str
     A.logit_bias = a->logit_bias; A.lb_bstride = a->logit_bias_bstride; A.lb_tstride = a->logit_bias_tstride;
     const EngineDev* E = p->dev;
     void* args[2] = {(void*)&E, (void*)&A};
-    JK_CHECK_CUDA(cudaLaunchCooperativeKernel((const void*)jk_decode_step_kernel, dim3(p->G), dim3(kThreads), args,
-                                              (size_t)p->smem_bytes, stream));
+    // Up to 16 samples take the 16-row kernel even on an engine planned for 32: its layout holds the 16-row one, and one
+    // m16 tile per weight fragment is all those rows need.
+    const void* kernel = a->n_samples <= 16 ? (const void*)jk_decode_step_kernel<16> : (const void*)jk_decode_step_kernel<32>;
+    JK_CHECK_CUDA(cudaLaunchCooperativeKernel(kernel, dim3(p->G), dim3(kThreads), args, (size_t)p->smem_bytes, stream));
     p->t_host += 1;
     return 0;
 }

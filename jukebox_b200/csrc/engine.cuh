@@ -29,8 +29,8 @@ struct EngineDev {
     unsigned long long stream_stride;
     // activations between phases travel as "LL" words (NCCL's low-latency protocol): 8 bytes = {half2 data, u32 flag},
     // written with one 8-byte store and polled by the consumer - no separate flag, no grid barrier
-    unsigned long long *ll_h, *ll_x1, *ll_qkv, *ll_a, *ll_g;   // [16][N/2]
-    unsigned long long* xp[4];      // K-split partial sums {fp32, flag}: [G][16][64] per Conv1D of a layer
+    unsigned long long *ll_h, *ll_x1, *ll_qkv, *ll_a, *ll_g;   // [R][N/2], R = 32 rows when max_batch > 16, else 16
+    unsigned long long* xp[4];      // K-split partial sums {fp32, flag}: [G][R][64] per Conv1D of a layer
     unsigned long long* part;       // split-KV partials as LL words {fp32, flag}: [Bmax*H][kMaxSplit][m, l, dh_pad outputs]
     // LayerNorm statistics: 2*depth+1 blocks of 512 words; row r's fixed-point {sum, sumsq} are words 16r and 16r+1
     // (one 128-B line per row), the contributor count in their top bits.  Block 2l feeds layer l's LN0, 2l+1 its LN1;

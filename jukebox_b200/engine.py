@@ -18,8 +18,8 @@ class DecodeEngine:
         if device.type != "cuda":
             raise RuntimeError("DecodeEngine needs a CUDA device (jukebox_b200 has no CPU path)")
         if max_batch > _lib.JK_MAX_BATCH:
-            raise RuntimeError(f"n_samples {max_batch} > {_lib.JK_MAX_BATCH}: split the batch "
-                               "(sample.py does, via max_batch_size)")
+            raise RuntimeError(f"n_samples {max_batch} > {_lib.JK_MAX_BATCH} (the decode kernel's largest row count): "
+                               "split the batch (sample.py does, via max_batch_size)")
         self.device = device
         cfg = _lib.PriorConfig()
         cfg.width, cfg.depth, cfg.heads, cfg.n_state, cfg.mlp_width = width, depth, heads, n_state, mlp_width

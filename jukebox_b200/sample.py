@@ -10,8 +10,9 @@ continue_sample, upsample, primed_sample, load_codes.  The work itself is organi
   * `LevelRun` owns one level's codes / labels / sampling options and executes windows: slice the context,
     fetch the per-window conditioning from the prior, split the batch into engine-sized pieces
     (`max_batch_size`), call `prior.sample`, append the new tokens.
-  * priors stay on the GPU between levels (180 GB holds all three); `hps.offload_priors` restores the reference's
-    cpu() shuffling.
+  * priors stay on the GPU between levels; `hps.offload_priors` restores the reference's cpu() shuffling.  At
+    `max_batch_size` 32 the decode engines' arenas alone (`jk_prior_plan`, computed) are 23.5 GB for `1b_lyrics` and
+    20.6 GB for each `upsampler_level_*`, 64.7 GB of an 80 GB H100 (INTEGRATION.md lists what that leaves out).
 
 Wav / HTML / alignment output (reference :110-120) is file I/O and out of scope: `_sample` returns the codes and,
 when hps.get('save_dir') is set, writes the reference's `data.pth.tar` resume format per level."""
@@ -127,7 +128,7 @@ def _sample(zs, labels, sampling_kwargs, priors, sample_levels, hps):
         tokens_needed = hps.sample_length // prior.raw_to_tokens
         hop = int(hps.hop_fraction[level] * prior.n_ctx)
         zs = sample_level(zs, labels[level], sampling_kwargs[level], level, prior, tokens_needed, hop, hps)
-        if hps.get('offload_priors', False):      # the reference always did (16 GB cards); 180 GB keeps them
+        if hps.get('offload_priors', False):      # the reference always did (16 GB cards); 80 GB keeps them
             prior.cpu()
             empty_cache()
         audio[level] = prior.decode(zs[level:], start_level=level, bs_chunks=zs[level].shape[0])

@@ -19,22 +19,30 @@ else:
     subprocess.run(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
                     "-c", os.path.join(root, "jukebox_b200", "csrc", "decode_engine.cu"), "-o", o], check=True)
 sass=subprocess.run(f"cuobjdump -sass {o}", shell=True, capture_output=True, text=True).stdout.splitlines()
-st=[i for i,l in enumerate(sass) if 'Function : ' in l and 'jk_decode_step' in l][0]
-ins=[]
-for l in sass[st:]:
-    m=re.match(r'\s*/\*([0-9a-f]{4,6})\*/\s+(.*?);', l)
-    if m: ins.append((int(m.group(1),16), m.group(2)))
-sym=subprocess.run(f"cuobjdump -elf {o} | grep -E '0x[0-9a-f]+ +0x[0-9a-f]+ +0x[0-9a-f]+ .*(stage_acts|attn_pv|attn_scores|attn_item|gemm_phase|logits_phase|attn_prefetch|producer_loop)' | grep -v Value", shell=True, capture_output=True, text=True).stdout
-funcs=[]
-for l in sym.splitlines():
-    f=l.split()
-    name=[k for k in ("stage_acts","attn_pv","attn_scores","attn_item","gemm_phase","logits_phase","attn_prefetch","producer_loop") if k in l][0]
-    funcs.append((int(f[1],16), int(f[2],16), name))
-funcs=sorted(set(funcs))
-for off,size,name in funcs:
-    body=[t for a,t in ins if off<=a<off+size]
-    regs=[int(x) for t in body for x in re.findall(r'\bR(\d+)\b', t)]
-    print(f"{name:14s} n_ins {len(body):5d} maxR {max(regs) if regs else -1:4d} STL {len([t for t in body if t.startswith('STL')]):3d} LDL {len([t for t in body if 'LDL' in t]):3d}")
-kern=[t for a,t in ins if a<funcs[0][0]]
-regs=[int(x) for t in kern for x in re.findall(r'\bR(\d+)\b', t)]
-print(f"{'kernel':14s} n_ins {len(kern):5d} maxR {max(regs):4d} STL {len([t for t in kern if t.startswith('STL')]):3d} LDL {len([t for t in kern if 'LDL' in t]):3d}")
+elf=subprocess.run(f"cuobjdump -elf {o}", shell=True, capture_output=True, text=True).stdout.splitlines()
+NAMES=("stage_acts","attn_pv","attn_scores","attn_item","gemm_phase","logits_phase","attn_prefetch","producer_loop")
+# The kernel is instantiated for 16 and 32 activation rows.  Each instantiation has its own text section holding its
+# copies of the phase functions; the 16-row one is reported under the plain names, the 32-row one with the suffix _r32.
+for rows, suffix in ((16, ""), (32, "_r32")):
+    tag=f"jk_decode_step_kernelILi{rows}E"
+    st=[i for i,l in enumerate(sass) if 'Function : ' in l and tag in l][0]
+    ins=[]
+    for l in sass[st+1:]:
+        if 'Function : ' in l: break
+        m=re.match(r'\s*/\*([0-9a-f]{4,6})\*/\s+(.*?);', l)
+        if m: ins.append((int(m.group(1),16), m.group(2)))
+    syms=[l.split() for l in elf if re.match(r'\s*0x[0-9a-f]+ +(0x[0-9a-f]+|0) +0x[0-9a-f]+ ', l) and 'Value' not in l]
+    shndx=[f[5] for f in syms if len(f) > 6 and tag in f[6] and not f[6].startswith("$")][0]
+    funcs=[]
+    for f in syms:
+        if len(f) > 6 and f[5] == shndx and f[6].startswith("$"):
+            name=[k for k in NAMES if k in f[6]]
+            if name: funcs.append((int(f[1],16), int(f[2],16), name[0]))
+    funcs=sorted(set(funcs))
+    for off,size,name in funcs:
+        body=[t for a,t in ins if off<=a<off+size]
+        regs=[int(x) for t in body for x in re.findall(r'\bR(\d+)\b', t)]
+        print(f"{name+suffix:14s} n_ins {len(body):5d} maxR {max(regs) if regs else -1:4d} STL {len([t for t in body if t.startswith('STL')]):3d} LDL {len([t for t in body if 'LDL' in t]):3d}")
+    kern=[t for a,t in ins if a<funcs[0][0]]
+    regs=[int(x) for t in kern for x in re.findall(r'\bR(\d+)\b', t)]
+    print(f"{'kernel'+suffix:14s} n_ins {len(kern):5d} maxR {max(regs):4d} STL {len([t for t in kern if t.startswith('STL')]):3d} LDL {len([t for t in kern if 'LDL' in t]):3d}")

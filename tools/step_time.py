@@ -23,7 +23,7 @@ with contextlib.redirect_stdout(sys.stderr):
     prior, _ = bench.build_prior(wl)
 ca = prior.prior
 n = int(os.environ.get("JK_N", "16"))
-eng = ca._engine(n)
+eng = ca._engine(int(os.environ.get("JK_ENGINE_N", n)))     # JK_ENGINE_N: an engine planned for more samples than it steps
 L = ca.input_dims
 toks = torch.randint(0, ca.bins, (n, L), device="cuda")
 lbuf = torch.empty(n, ca.bins, device="cuda")
