@@ -173,8 +173,11 @@ int jk_prior_prefill(jk_prior* p, const jk_prefill_args* args, jk_stream_t strea
 int jk_prior_step(jk_prior* p, const jk_step_args* a, jk_stream_t stream);
 /* current position (host copy of the device counter as tracked by the calls made so far) */
 int jk_prior_position(const jk_prior* p, int* t);
-/* debug / test access to the fp16 intermediates of the LAST layer executed:
- * which: 0 = h, 1 = qkv, 2 = attention out, 3 = x1 (x + a), 4 = gelu out.  Returns device ptr. */
+/* profiling buffers of the decode kernel (device ptr and size in halfs; any other `which` is an error):
+ * which: 5 = globaltimer stamps (uint64 per phase), 6 = clock64 stamps (int64 [phase][8]), 7 = globaltimer entry / exit
+ * stamps of every CTA in the five phases of layer 1 (uint64 [5][256][2]).  Written only when the engine was created with JK_PROFILE set.
+ * The activations travel between SMs as flagged words and are not kept: h_out and logits of jk_step_args are the
+ * step's observable outputs. */
 int jk_prior_debug_buffer(const jk_prior* p, int which, const void** ptr, size_t* n_halfs);
 
 /* Conv1D at prefill / training shape on the tensor cores (wgmma + TMA): y[M, N] = x[M, K] . w + b, fp16 in,
