@@ -146,6 +146,17 @@ typedef struct jk_step_args {
     int64_t logit_bias_tstride;
 } jk_step_args;
 
+/* Attention weights of one layer recorded by a prefill call (record_attn in fp16 mode, factored_attention.py:83-105, the
+ * pass lyric alignment reads, align.py:91-96).  w: device fp16 [n_samples][heads][n_positions][ld]; w[b][h][q][k] =
+ * fp16(softmax_fp32(fp16(fp16(q.k) * dh^-1/2))[k]) for key position k of the layer's pattern (for an encoder-decoder layer
+ * k is the encoder row), 0 for every other k; a query without keys (previous-block attention in the first block) is a
+ * row of zeros.  Keys >= ld are not written, so a prime layer can keep just its lyric columns (ld = prime_len). */
+typedef struct jk_attn_record {
+    int32_t layer;
+    int32_t ld;
+    void* w;
+} jk_attn_record;
+
 /* Chunked prefill of the given (prime) tokens: positions 0 .. n_positions-1 of every sample through all
  * layers in one call - the chunked half of ConditionalAutoregressive2D.primed_sample
  * (prior/autoregressive.py:251-359), whose own check_chunks asserts it equals stepping token by token.
@@ -163,10 +174,16 @@ typedef struct jk_prefill_args {
     const float* x_cond;      /* [n_samples, x_cond_len, width] or NULL */
     int64_t x_cond_len;       /* 1 or n_ctx */
     float* h_out;
+    const jk_attn_record* record;   /* n_record distinct layers whose weights this call records, or NULL */
+    int32_t n_record;
 } jk_prefill_args;
 /* positions one prefill call can take; 0 when the configuration has no tensor-core prefill (a GEMM K that
  * is not a multiple of 64, or encoder-decoder layers): step the given tokens instead */
 int jk_prior_prefill_capacity(const jk_prior* p, int* max_positions);
+/* the same number for an engine of this configuration on the current device, from host arithmetic alone (no engine is
+ * built): callers that choose between the prefill and another path ask before building one.  An error when the
+ * configuration cannot make an engine (jk_prior_arena_bytes would fail). */
+int jk_prior_config_prefill_capacity(const jk_prior_config* cfg, int* max_positions);
 int jk_prior_prefill(jk_prior* p, const jk_prefill_args* args, jk_stream_t stream);
 
 /* one token position; increments the device-side position counter */

@@ -57,10 +57,15 @@ class StepArgs(C.Structure):
                 ("logit_bias_bstride", C.c_int64), ("logit_bias_tstride", C.c_int64)]
 
 
+class AttnRecord(C.Structure):
+    _fields_ = [("layer", C.c_int32), ("ld", C.c_int32), ("w", C.c_void_p)]
+
+
 class PrefillArgs(C.Structure):
     _fields_ = [("n_samples", C.c_int32), ("n_positions", C.c_int32), ("tokens", C.c_void_p),
                 ("tok_stride", C.c_int64), ("y_cond", C.c_void_p), ("x_cond", C.c_void_p),
-                ("x_cond_len", C.c_int64), ("h_out", C.c_void_p)]
+                ("x_cond_len", C.c_int64), ("h_out", C.c_void_p), ("record", C.POINTER(AttnRecord)),
+                ("n_record", C.c_int32)]
 
 
 class ConvArgs(C.Structure):
@@ -88,6 +93,7 @@ SIGNATURES = {
     "jk_prior_set_encoder_kv": (_I, [_P, _P, _I, _P]),
     "jk_prior_step": (_I, [_P, C.POINTER(StepArgs), _P]),
     "jk_prior_prefill_capacity": (_I, [_P, C.POINTER(C.c_int)]),
+    "jk_prior_config_prefill_capacity": (_I, [C.POINTER(PriorConfig), C.POINTER(C.c_int)]),
     "jk_prior_prefill": (_I, [_P, C.POINTER(PrefillArgs), _P]),
     "jk_prior_position": (_I, [_P, C.POINTER(C.c_int)]),
     "jk_prior_has_logits_gemm": (_I, [_P, C.POINTER(C.c_int)]),

@@ -1930,6 +1930,17 @@ extern "C" int jk_prior_arena_bytes(const jk_prior_config* cfg, size_t* bytes) {
     return 0;
 }
 
+extern "C" int jk_prior_config_prefill_capacity(const jk_prior_config* cfg, int* max_positions) {
+    JK_REQUIRE(cfg && max_positions, "null argument");
+    int G = device_sms();
+    JK_REQUIRE(G > 0, "no CUDA device (the decode engine has no CPU path)");
+    Layout L;
+    int rc = compute_layout(*cfg, G, L);
+    if (rc) return rc;
+    *max_positions = L.pf_len;
+    return 0;
+}
+
 extern "C" int jk_prior_plan(const jk_prior_config* cfg, int n_sms, jk_prior_plan_info* out, uint16_t* cols, size_t cols_len) {
     JK_REQUIRE(cfg && out, "null argument");
     JK_REQUIRE(n_sms >= 1 && n_sms <= 1024, "n_sms %d out of range", n_sms);

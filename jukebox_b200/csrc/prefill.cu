@@ -113,30 +113,32 @@ __device__ __forceinline__ int fwd_key(const AttnFwd& A, int p, int j) {
 
 constexpr int kFwdThreads = 128;
 
-__global__ void __launch_bounds__(kFwdThreads) attn_fwd_kernel(AttnFwd A) {
-    extern __shared__ float fsm[];
-    float* qs = fsm;                 // [dh]
-    float* sc = fsm + A.dh;          // [nk]
-    __shared__ float red[kFwdThreads / 32];
-    const int p = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int dh = A.dh, S = A.S;
-    const size_t row = (size_t)b * A.P + p;
-    const __half* q = A.qkv + row * A.q_stride + h * dh;
-    __half* out = A.a + row * S + h * dh;
+// K / V rows of head h of sample b: key j of the pattern is row fwd_key(.., j) of kbase / vbase, `kstride` halfs apart
+struct FwdKV {
+    const __half* kbase;
+    const __half* vbase;
+    size_t kstride;
+};
+__device__ __forceinline__ FwdKV fwd_kv(const AttnFwd& A, int h, int b) {
     const bool enc = A.attn_func == 6;
-    const __half* kbase = enc ? A.kc + ((size_t)b * A.H + h) * A.enc_rows * A.dhp : A.qkv + (size_t)b * A.P * 3 * S + S + h * dh;
-    const __half* vbase = enc ? A.vc + ((size_t)b * A.H + h) * A.enc_rows * A.dhp : kbase + S;
-    const size_t kstride = enc ? (size_t)A.dhp : (size_t)3 * S;
-    const int nk = fwd_nkeys(A, p);
-    if (nk == 0) {
-        for (int d = tid; d < dh; d += kFwdThreads) out[d] = __float2half_rn(0.f);
-        return;
-    }
+    const int S = A.S;
+    FwdKV R;
+    R.kbase = enc ? A.kc + ((size_t)b * A.H + h) * A.enc_rows * A.dhp : A.qkv + (size_t)b * A.P * 3 * S + S + h * A.dh;
+    R.vbase = enc ? A.vc + ((size_t)b * A.H + h) * A.enc_rows * A.dhp : R.kbase + S;
+    R.kstride = enc ? (size_t)A.dhp : (size_t)3 * S;
+    return R;
+}
+
+// scores of query p over its nk > 0 keys -> sc[j], fp16(fp16(q.k) * dh^-1/2); returns the row max (one CTA of kFwdThreads)
+__device__ __forceinline__ float fwd_row_scores(const AttnFwd& A, const FwdKV& R, int p, int h, int b, int nk, float* qs,
+                                                float* sc, float* red) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int dh = A.dh;
+    const __half* q = A.qkv + ((size_t)b * A.P + p) * A.q_stride + h * dh;
     for (int d = tid; d < dh; d += kFwdThreads) qs[d] = ldh(q + d);
     __syncthreads();
     for (int j = warp; j < nk; j += kFwdThreads / 32) {
-        const __half* k = kbase + (size_t)fwd_key(A, p, j) * kstride;
+        const __half* k = R.kbase + (size_t)fwd_key(A, p, j) * R.kstride;
         float dot = 0.f;
         for (int d = lane; d < dh; d += 32) dot = fmaf(qs[d], ldh(k + d), dot);
         dot = warp_sum(dot);
@@ -150,6 +152,25 @@ __global__ void __launch_bounds__(kFwdThreads) attn_fwd_kernel(AttnFwd A) {
     __syncthreads();
     mx = fmaxf(fmaxf(red[0], red[1]), fmaxf(red[2], red[3]));
     __syncthreads();
+    return mx;
+}
+
+__global__ void __launch_bounds__(kFwdThreads) attn_fwd_kernel(AttnFwd A) {
+    extern __shared__ float fsm[];
+    float* qs = fsm;                 // [dh]
+    float* sc = fsm + A.dh;          // [nk]
+    __shared__ float red[kFwdThreads / 32];
+    const int p = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int dh = A.dh, S = A.S;
+    __half* out = A.a + ((size_t)b * A.P + p) * S + h * dh;
+    const FwdKV R = fwd_kv(A, h, b);
+    const int nk = fwd_nkeys(A, p);
+    if (nk == 0) {
+        for (int d = tid; d < dh; d += kFwdThreads) out[d] = __float2half_rn(0.f);
+        return;
+    }
+    const float mx = fwd_row_scores(A, R, p, h, b, nk, qs, sc, red);
     float l = 0.f;
     for (int j = tid; j < nk; j += kFwdThreads) {
         const float e = expf(sc[j] - mx);
@@ -163,9 +184,34 @@ __global__ void __launch_bounds__(kFwdThreads) attn_fwd_kernel(AttnFwd A) {
     for (int d = tid; d < dh; d += kFwdThreads) {
         float o = 0.f;
         for (int j = 0; j < nk; ++j) {
-            o = fmaf(sc[j], ldh(vbase + (size_t)fwd_key(A, p, j) * kstride + d), o);
+            o = fmaf(sc[j], ldh(R.vbase + (size_t)fwd_key(A, p, j) * R.kstride + d), o);
         }
         out[d] = __float2half_rn(o * inv);
+    }
+}
+
+// recorded weights of query p (see attn_record_mma_kernel) for the head geometries the tensor-core kernels do not take
+// (dh > 256: the released upsamplers' 480): w[b][h][p][key] = fp16(exp(s - max) / sum) for keys < ld
+__global__ void __launch_bounds__(kFwdThreads) attn_record_kernel(AttnFwd A, __half* __restrict__ w, int ld) {
+    extern __shared__ float fsm[];
+    float* qs = fsm;                 // [dh]
+    float* sc = fsm + A.dh;          // [nk]
+    __shared__ float red[kFwdThreads / 32];
+    const int p = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int nk = fwd_nkeys(A, p);
+    if (nk == 0) return;             // a row without keys stays as the caller zeroed it
+    const float mx = fwd_row_scores(A, fwd_kv(A, h, b), p, h, b, nk, qs, sc, red);
+    float l = 0.f;
+    for (int j = tid; j < nk; j += kFwdThreads) l += expf(sc[j] - mx);
+    l = warp_sum(l);
+    if (lane == 0) red[warp] = l;
+    __syncthreads();
+    const float inv = 1.f / (red[0] + red[1] + red[2] + red[3]);
+    __half* wrow = w + (((size_t)b * A.H + h) * A.P + p) * ld;
+    for (int j = tid; j < nk; j += kFwdThreads) {
+        const int k = fwd_key(A, p, j);
+        if (k < ld) wrow[k] = __float2half_rn(expf(sc[j] - mx) * inv);
     }
 }
 
@@ -208,10 +254,149 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
     return *reinterpret_cast<const uint32_t*>(&h);
 }
 
+// Pieces of the tensor-core attention shared by the forward kernel and the record kernel below.
 // W16: head rows are 16-byte aligned (dh % 8 == 0) -> 16-byte cp.async chunks; else (5b_lyrics: dh 150) 4-byte words
+constexpr int kBQ = 64, kBK = 32;
+
+// the tile of 64 queries i0.. of one sequence -> shared memory (zero rows / columns beyond nq / dh) -> this warp's A fragments
+template <int DH, bool W16>
+__device__ __forceinline__ void load_q_frags(uint32_t (&qf)[DH / 16][4], __half* qs, const AttnFwd& A, const SeqGeom& G,
+                                             size_t rowbase, int i0, int h) {
+    constexpr int XS = DH + 8;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int dh = A.dh, nv = dh >> 3;                       // 16-byte chunks per row
+    if (W16) {
+        for (int i = tid; i < kBQ * (DH / 8); i += 128) {
+            const int r = i / (DH / 8), c = i % (DH / 8);
+            uint4 v = make_uint4(0, 0, 0, 0);
+            if (i0 + r < G.nq && c < nv)
+                v = *reinterpret_cast<const uint4*>(A.qkv + (rowbase + G.q0 + (size_t)(i0 + r) * G.qs) * A.q_stride + h * dh + c * 8);
+            *reinterpret_cast<uint4*>(qs + r * XS + c * 8) = v;
+        }
+    } else {
+        for (int i = tid; i < kBQ * (DH / 2); i += 128) {
+            const int r = i / (DH / 2), c = i % (DH / 2);
+            uint32_t v = 0;
+            if (i0 + r < G.nq && 2 * c < dh)
+                v = *reinterpret_cast<const uint32_t*>(A.qkv + (rowbase + G.q0 + (size_t)(i0 + r) * G.qs) * A.q_stride + h * dh + c * 2);
+            *reinterpret_cast<uint32_t*>(qs + r * XS + c * 2) = v;
+        }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < DH / 16; ++k) ldmatrix_x4(qf[k], qs + (warp * 16 + (lane & 15)) * XS + k * 16 + (lane >> 4) * 8);
+}
+
+// the keys a tile of queries attends: K / V rows kbase + j * kstride, j < nk
+struct KeyRange {
+    const __half* kbase;
+    const __half* vbase;
+    size_t kstride;
+    int nk;
+};
+__device__ __forceinline__ KeyRange key_range(const AttnFwd& A, const SeqGeom& G, size_t rowbase, int i0, int h, int b, bool enc) {
+    KeyRange R;
+    // keys beyond the last query of this tile are never needed
+    int nk = G.nk;
+    if (!enc && nk > 0) {
+        const long long qmax = G.q0 + (long long)(min(i0 + kBQ, G.nq) - 1) * G.qs;
+        const long long jm = qmax >= G.k0 ? (qmax - G.k0) / G.ks + 1 : 0;
+        nk = (int)min((long long)nk, jm);
+    }
+    const int S = A.S;
+    if (enc) {
+        R.kbase = A.kc + ((size_t)b * A.H + h) * A.enc_rows * A.dhp; R.vbase = A.vc + ((size_t)b * A.H + h) * A.enc_rows * A.dhp;
+        R.kstride = (size_t)A.dhp;
+    } else {
+        R.kbase = A.qkv + (rowbase + (size_t)(nk > 0 ? G.k0 : 0)) * 3 * S + S + h * A.dh; R.vbase = R.kbase + S;
+        R.kstride = (size_t)3 * S * G.ks;
+    }
+    R.nk = nk;
+    return R;
+}
+
+// keys j0 .. j0 + 31 (and their values when KV) -> shared memory; rows beyond nk and columns beyond dh are zero
+template <int DH, bool W16, bool KV>
+__device__ __forceinline__ void stage_keys(__half* ks, __half* vs, const KeyRange& R, int j0, int dh) {
+    constexpr int XS = DH + 8;
+    const int tid = threadIdx.x, nv = dh >> 3;
+    if (W16) {
+        for (int i = tid; i < kBK * (DH / 8); i += 128) {
+            const int r = i / (DH / 8), c = i % (DH / 8);
+            if (j0 + r < R.nk && c < nv) {
+                cp16(ks + r * XS + c * 8, R.kbase + (size_t)(j0 + r) * R.kstride + c * 8);
+                if (KV) cp16(vs + r * XS + c * 8, R.vbase + (size_t)(j0 + r) * R.kstride + c * 8);
+            } else {
+                *reinterpret_cast<uint4*>(ks + r * XS + c * 8) = make_uint4(0, 0, 0, 0);
+                if (KV) *reinterpret_cast<uint4*>(vs + r * XS + c * 8) = make_uint4(0, 0, 0, 0);
+            }
+        }
+        asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
+    } else {
+#pragma unroll 4
+        for (int i = tid; i < kBK * (DH / 2); i += 128) {
+            const int r = i / (DH / 2), c = i % (DH / 2);
+            uint32_t kv = 0, vv = 0;
+            if (j0 + r < R.nk && 2 * c < dh) {
+                kv = *reinterpret_cast<const uint32_t*>(R.kbase + (size_t)(j0 + r) * R.kstride + c * 2);
+                if (KV) vv = *reinterpret_cast<const uint32_t*>(R.vbase + (size_t)(j0 + r) * R.kstride + c * 2);
+            }
+            *reinterpret_cast<uint32_t*>(ks + r * XS + c * 2) = kv;
+            if (KV) *reinterpret_cast<uint32_t*>(vs + r * XS + c * 2) = vv;
+        }
+    }
+}
+
+// S = Q K^T of this warp's 16 query rows x the 32 staged keys, with the reference's roundings
+// (score = fp16(fp16(q.k) * dh^-1/2)); keys outside the pattern (j >= nk, or after the query) are -inf.
+// sc[n][e]: key j0 + n*8 + 2*t4 + (e & 1) of query row qp0 (e < 2) or qp1 (e >= 2)
+template <int DH>
+__device__ __forceinline__ void tile_scores(float (&sc)[kBK / 8][4], const uint32_t (&qf)[DH / 16][4], const __half* ks,
+                                            const SeqGeom& G, int j0, int nk, long long qp0, long long qp1, bool enc, float scale2) {
+    constexpr int XS = DH + 8;
+    const int lane = threadIdx.x & 31, t4 = lane & 3;
+#pragma unroll
+    for (int n = 0; n < kBK / 8; ++n) sc[n][0] = sc[n][1] = sc[n][2] = sc[n][3] = 0.f;
+#pragma unroll
+    for (int k = 0; k < DH / 16; ++k) {
+#pragma unroll
+        for (int np = 0; np < kBK / 16; ++np) {
+            uint32_t kf[4];
+            ldmatrix_x4(kf, ks + (np * 16 + (lane & 7) + ((lane >> 4) << 3)) * XS + k * 16 + ((lane >> 3) & 1) * 8);
+            mma_16816(sc[2 * np], qf[k], kf[0], kf[1]);
+            mma_16816(sc[2 * np + 1], qf[k], kf[2], kf[3]);
+        }
+    }
+#pragma unroll
+    for (int n = 0; n < kBK / 8; ++n)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const int j = j0 + n * 8 + 2 * t4 + (e & 1);
+            const long long kp = G.k0 + (long long)j * G.ks;
+            const bool ok = j < nk && (enc || kp <= (e >= 2 ? qp1 : qp0));
+            sc[n][e] = ok ? h2f_round(h2f_round(sc[n][e]) * scale2) : -INFINITY;
+        }
+}
+
+// the running row max / row sum (fp32, from the unrounded exponentials) of quad-shared rows after one tile of scores;
+// returns the rescale factors of the previous sums
+__device__ __forceinline__ void online_max(const float (&sc)[kBK / 8][4], float& m0, float& m1, float& c0, float& c1) {
+    float mx0 = m0, mx1 = m1;
+#pragma unroll
+    for (int n = 0; n < kBK / 8; ++n)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            if (e >= 2) mx1 = fmaxf(mx1, sc[n][e]); else mx0 = fmaxf(mx0, sc[n][e]);
+        }
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+    c0 = expf(m0 - mx0); c1 = expf(m1 - mx1);
+    m0 = mx0; m1 = mx1;
+}
+
 template <int DH, bool W16>
 __global__ void __launch_bounds__(128) attn_fwd_mma_kernel(AttnFwd A, AttnSeqs Q) {
-    constexpr int XS = DH + 8, BQ = 64, BK = 32;
+    constexpr int XS = DH + 8, BQ = kBQ, BK = kBK;
     extern __shared__ __align__(16) __half asm_[];
     __half* qs = asm_;                       // [BQ][XS]
     __half* ks = qs + BQ * XS;               // [BK][XS]
@@ -223,113 +408,27 @@ __global__ void __launch_bounds__(128) attn_fwd_mma_kernel(AttnFwd A, AttnSeqs Q
     const SeqGeom G = seq_geom(Q, seq);
     const int i0 = qt * BQ;
     if (i0 >= G.nq) return;
-    const int dh = A.dh, S = A.S, nv = dh >> 3;              // 16-byte chunks per row
+    const int dh = A.dh, S = A.S;
     const bool enc = A.attn_func == 6;
     const size_t rowbase = (size_t)b * A.P;
-    // ---- Q tile -> shared memory (zero rows / columns beyond nq / dh) ----
-    if (W16) {
-        for (int i = tid; i < BQ * (DH / 8); i += 128) {
-            const int r = i / (DH / 8), c = i % (DH / 8);
-            uint4 v = make_uint4(0, 0, 0, 0);
-            if (i0 + r < G.nq && c < nv)
-                v = *reinterpret_cast<const uint4*>(A.qkv + (rowbase + G.q0 + (size_t)(i0 + r) * G.qs) * A.q_stride + h * dh + c * 8);
-            *reinterpret_cast<uint4*>(qs + r * XS + c * 8) = v;
-        }
-    } else {
-        for (int i = tid; i < BQ * (DH / 2); i += 128) {
-            const int r = i / (DH / 2), c = i % (DH / 2);
-            uint32_t v = 0;
-            if (i0 + r < G.nq && 2 * c < dh)
-                v = *reinterpret_cast<const uint32_t*>(A.qkv + (rowbase + G.q0 + (size_t)(i0 + r) * G.qs) * A.q_stride + h * dh + c * 2);
-            *reinterpret_cast<uint32_t*>(qs + r * XS + c * 2) = v;
-        }
-    }
-    __syncthreads();
     uint32_t qf[DH / 16][4];
-#pragma unroll
-    for (int k = 0; k < DH / 16; ++k) ldmatrix_x4(qf[k], qs + (warp * 16 + (lane & 15)) * XS + k * 16 + (lane >> 4) * 8);
+    load_q_frags<DH, W16>(qf, qs, A, G, rowbase, i0, h);
     float o[DH / 8][4];
 #pragma unroll
     for (int n = 0; n < DH / 8; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
     float m0 = -1e30f, m1 = -1e30f, l0 = 0.f, l1 = 0.f;
     const int qi0 = i0 + warp * 16 + g, qi1 = qi0 + 8;                  // this lane's two query rows (sequence indices)
     const long long qp0 = G.q0 + (long long)qi0 * G.qs, qp1 = G.q0 + (long long)qi1 * G.qs;
-    // keys beyond the last query of this tile are never needed
-    int nk = G.nk;
-    if (!enc && nk > 0) {
-        const long long qmax = G.q0 + (long long)(min(i0 + BQ, G.nq) - 1) * G.qs;
-        const long long jm = qmax >= G.k0 ? (qmax - G.k0) / G.ks + 1 : 0;
-        nk = (int)min((long long)nk, jm);
-    }
-    const __half* kbase;
-    const __half* vbase;
-    size_t kstride;
-    if (enc) {
-        kbase = A.kc + ((size_t)b * A.H + h) * A.enc_rows * A.dhp; vbase = A.vc + ((size_t)b * A.H + h) * A.enc_rows * A.dhp;
-        kstride = (size_t)A.dhp;
-    } else {
-        kbase = A.qkv + (rowbase + (size_t)(nk > 0 ? G.k0 : 0)) * 3 * S + S + h * dh; vbase = kbase + S; kstride = (size_t)3 * S * G.ks;
-    }
-    for (int j0 = 0; j0 < nk; j0 += BK) {
+    const KeyRange R = key_range(A, G, rowbase, i0, h, b, enc);
+    for (int j0 = 0; j0 < R.nk; j0 += BK) {
         __syncthreads();                                                // the previous tile's fragment reads are done
-        if (W16) {
-            for (int i = tid; i < BK * (DH / 8); i += 128) {
-                const int r = i / (DH / 8), c = i % (DH / 8);
-                if (j0 + r < nk && c < nv) {
-                    cp16(ks + r * XS + c * 8, kbase + (size_t)(j0 + r) * kstride + c * 8);
-                    cp16(vs + r * XS + c * 8, vbase + (size_t)(j0 + r) * kstride + c * 8);
-                } else {
-                    *reinterpret_cast<uint4*>(ks + r * XS + c * 8) = make_uint4(0, 0, 0, 0);
-                    *reinterpret_cast<uint4*>(vs + r * XS + c * 8) = make_uint4(0, 0, 0, 0);
-                }
-            }
-            asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
-        } else {
-#pragma unroll 4
-            for (int i = tid; i < BK * (DH / 2); i += 128) {
-                const int r = i / (DH / 2), c = i % (DH / 2);
-                uint32_t kv = 0, vv = 0;
-                if (j0 + r < nk && 2 * c < dh) {
-                    kv = *reinterpret_cast<const uint32_t*>(kbase + (size_t)(j0 + r) * kstride + c * 2);
-                    vv = *reinterpret_cast<const uint32_t*>(vbase + (size_t)(j0 + r) * kstride + c * 2);
-                }
-                *reinterpret_cast<uint32_t*>(ks + r * XS + c * 2) = kv;
-                *reinterpret_cast<uint32_t*>(vs + r * XS + c * 2) = vv;
-            }
-        }
+        stage_keys<DH, W16, true>(ks, vs, R, j0, dh);
         __syncthreads();
-        // ---- S = Q K^T for this warp's 16 rows x 32 keys ----
         float sc[BK / 8][4];
-#pragma unroll
-        for (int n = 0; n < BK / 8; ++n) sc[n][0] = sc[n][1] = sc[n][2] = sc[n][3] = 0.f;
-#pragma unroll
-        for (int k = 0; k < DH / 16; ++k) {
-#pragma unroll
-            for (int np = 0; np < BK / 16; ++np) {
-                uint32_t kf[4];
-                ldmatrix_x4(kf, ks + (np * 16 + (lane & 7) + ((lane >> 4) << 3)) * XS + k * 16 + ((lane >> 3) & 1) * 8);
-                mma_16816(sc[2 * np], qf[k], kf[0], kf[1]);
-                mma_16816(sc[2 * np + 1], qf[k], kf[2], kf[3]);
-            }
-        }
-        // ---- mask, the reference's roundings, online softmax ----
-        float mx0 = m0, mx1 = m1;
-#pragma unroll
-        for (int n = 0; n < BK / 8; ++n)
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const int j = j0 + n * 8 + 2 * t4 + (e & 1);
-                const long long kp = G.k0 + (long long)j * G.ks;
-                const bool row1 = e >= 2;
-                const bool ok = j < nk && (enc || kp <= (row1 ? qp1 : qp0));
-                const float v = ok ? h2f_round(h2f_round(sc[n][e]) * A.scale2) : -INFINITY;
-                sc[n][e] = v;
-                if (row1) mx1 = fmaxf(mx1, v); else mx0 = fmaxf(mx0, v);
-            }
-        mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
-        mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
-        const float c0 = expf(m0 - mx0), c1 = expf(m1 - mx1);
-        m0 = mx0; m1 = mx1;
+        tile_scores<DH>(sc, qf, ks, G, j0, R.nk, qp0, qp1, enc, A.scale2);
+        // ---- online softmax ----
+        float c0, c1;
+        online_max(sc, m0, m1, c0, c1);
         float r0 = 0.f, r1 = 0.f;
         uint32_t pf[BK / 16][4];
 #pragma unroll
@@ -368,23 +467,102 @@ __global__ void __launch_bounds__(128) attn_fwd_mma_kernel(AttnFwd A, AttnSeqs Q
     }
 }
 
+// ---- recorded attention weights (record_attn, factored_attention.py:83-105 in fp16 mode) ----------------------------------
+// w[b][h][q][k] = fp16(softmax_fp32(score)[k]) for every key k < ld of the query's pattern, score as above.  The weights are
+// normalised BEFORE the fp16 rounding, so the forward kernel's unnormalised P cannot serve: the same tiles and key staging
+// run twice, the first pass for the row max and row sum, the second for the write.  Entries outside the pattern are
+// zeroed by the caller (cudaMemsetAsync), and so are rows without keys.
 template <int DH, bool W16>
-int launch_attn_mma(const AttnFwd& A, const AttnSeqs& Q, int nseq, int n, cudaStream_t stream) {
-    constexpr size_t smem = (size_t)(64 + 2 * 32) * (DH + 8) * 2;
-    static bool attr_set[64] = {};
+__global__ void __launch_bounds__(128) attn_record_mma_kernel(AttnFwd A, AttnSeqs Q, __half* __restrict__ w, int ld) {
+    constexpr int XS = DH + 8;
+    extern __shared__ __align__(16) __half asm_[];
+    __half* qs = asm_;                       // [kBQ][XS]
+    __half* ks = qs + kBQ * XS;              // [kBK][XS]
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int g = lane >> 2, t4 = lane & 3;
+    const int seq = blockIdx.x / Q.tiles_per_seq, qt = blockIdx.x - seq * Q.tiles_per_seq;
+    const int h = blockIdx.y, b = blockIdx.z;
+    const SeqGeom G = seq_geom(Q, seq);
+    const int i0 = qt * kBQ;
+    if (i0 >= G.nq) return;
+    const bool enc = A.attn_func == 6;
+    const size_t rowbase = (size_t)b * A.P;
+    uint32_t qf[DH / 16][4];
+    load_q_frags<DH, W16>(qf, qs, A, G, rowbase, i0, h);
+    const int qi0 = i0 + warp * 16 + g, qi1 = qi0 + 8;
+    const long long qp0 = G.q0 + (long long)qi0 * G.qs, qp1 = G.q0 + (long long)qi1 * G.qs;
+    const KeyRange R = key_range(A, G, rowbase, i0, h, b, enc);
+    // ---- pass 1: row max and row sum ----
+    float m0 = -1e30f, m1 = -1e30f, l0 = 0.f, l1 = 0.f;
+    for (int j0 = 0; j0 < R.nk; j0 += kBK) {
+        __syncthreads();
+        stage_keys<DH, W16, false>(ks, nullptr, R, j0, A.dh);
+        __syncthreads();
+        float sc[kBK / 8][4];
+        tile_scores<DH>(sc, qf, ks, G, j0, R.nk, qp0, qp1, enc, A.scale2);
+        float c0, c1;
+        online_max(sc, m0, m1, c0, c1);
+        float r0 = 0.f, r1 = 0.f;
+#pragma unroll
+        for (int n = 0; n < kBK / 8; ++n) {
+            r0 += expf(sc[n][0] - m0) + expf(sc[n][1] - m0);
+            r1 += expf(sc[n][2] - m1) + expf(sc[n][3] - m1);
+        }
+        r0 += __shfl_xor_sync(0xffffffffu, r0, 1); r0 += __shfl_xor_sync(0xffffffffu, r0, 2);
+        r1 += __shfl_xor_sync(0xffffffffu, r1, 1); r1 += __shfl_xor_sync(0xffffffffu, r1, 2);
+        l0 = l0 * c0 + r0; l1 = l1 * c1 + r1;
+    }
+    // ---- pass 2: fp16(exp(s - max) / sum) of the keys below ld ----
+    const float inv0 = l0 > 0.f ? 1.f / l0 : 0.f, inv1 = l1 > 0.f ? 1.f / l1 : 0.f;
+    __half* w0 = w + (((size_t)b * A.H + h) * A.P + (size_t)qp0) * ld;
+    __half* w1 = w + (((size_t)b * A.H + h) * A.P + (size_t)qp1) * ld;
+    for (int j0 = 0; j0 < R.nk && G.k0 + (long long)j0 * G.ks < ld; j0 += kBK) {
+        __syncthreads();
+        stage_keys<DH, W16, false>(ks, nullptr, R, j0, A.dh);
+        __syncthreads();
+        float sc[kBK / 8][4];
+        tile_scores<DH>(sc, qf, ks, G, j0, R.nk, qp0, qp1, enc, A.scale2);
+#pragma unroll
+        for (int n = 0; n < kBK / 8; ++n)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const bool row1 = e >= 2;
+                const long long kp = G.k0 + (long long)(j0 + n * 8 + 2 * t4 + (e & 1)) * G.ks;
+                if ((row1 ? qi1 : qi0) < G.nq && kp < ld && sc[n][e] != -INFINITY)
+                    (row1 ? w1 : w0)[kp] = __float2half_rn(expf(sc[n][e] - (row1 ? m1 : m0)) * (row1 ? inv1 : inv0));
+            }
+    }
+}
+
+// w == nullptr: the forward (attn_fwd_mma_kernel); else the recorded weights of the layer (attn_record_mma_kernel)
+template <int DH, bool W16>
+int launch_attn_mma(const AttnFwd& A, const AttnSeqs& Q, int nseq, int n, __half* w, int ld, cudaStream_t stream) {
+    const dim3 grid((unsigned)(nseq * Q.tiles_per_seq), A.H, n);
+    static bool attr_set[2][64] = {};
     int dev = 0;
     JK_CHECK_CUDA(cudaGetDevice(&dev));
-    if (!attr_set[dev & 63]) {
-        JK_CHECK_CUDA(cudaFuncSetAttribute((attn_fwd_mma_kernel<DH, W16>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set[dev & 63] = true;
+    if (!w) {
+        constexpr size_t smem = (size_t)(kBQ + 2 * kBK) * (DH + 8) * 2;
+        if (!attr_set[0][dev & 63]) {
+            JK_CHECK_CUDA(cudaFuncSetAttribute((attn_fwd_mma_kernel<DH, W16>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            attr_set[0][dev & 63] = true;
+        }
+        attn_fwd_mma_kernel<DH, W16><<<grid, 128, smem, stream>>>(A, Q);
+    } else {
+        constexpr size_t smem = (size_t)(kBQ + kBK) * (DH + 8) * 2;
+        if (!attr_set[1][dev & 63]) {
+            JK_CHECK_CUDA(cudaFuncSetAttribute((attn_record_mma_kernel<DH, W16>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            attr_set[1][dev & 63] = true;
+        }
+        attn_record_mma_kernel<DH, W16><<<grid, 128, smem, stream>>>(A, Q, w, ld);
     }
-    attn_fwd_mma_kernel<DH, W16><<<dim3((unsigned)(nseq * Q.tiles_per_seq), A.H, n), 128, smem, stream>>>(A, Q);
     JK_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 
-// returns 1 if the tensor-core kernel took the layer, 0 if the shape is left to attn_fwd_kernel, < 0 on error
-int attn_forward_mma(const AttnFwd& A, int n, cudaStream_t stream) {
+// the layer's attention (w == nullptr) or its recorded weights on the tensor cores: returns 1 if the tensor-core kernel
+// took the layer, 0 if the shape is left to attn_fwd_kernel / attn_record_kernel, < 0 on error
+int attn_mma(const AttnFwd& A, int n, __half* w, int ld, cudaStream_t stream) {
     static const bool off = getenv("JK_PREFILL_SCALAR_ATTN") != nullptr;
     if (off || A.dh % 2 != 0 || A.dh > 256) return 0;
     const bool w16 = A.dh % 8 == 0 && A.S % 8 == 0 && A.dhp % 8 == 0;
@@ -398,11 +576,11 @@ int attn_forward_mma(const AttnFwd& A, int n, cudaStream_t stream) {
     }
     Q.tiles_per_seq = (maxq + 63) / 64;
     int rc;
-    if (!w16) rc = A.dh <= 160 ? launch_attn_mma<160, false>(A, Q, nseq, n, stream) : launch_attn_mma<256, false>(A, Q, nseq, n, stream);
-    else if (A.dh <= 32) rc = launch_attn_mma<32, true>(A, Q, nseq, n, stream);
-    else if (A.dh <= 64) rc = launch_attn_mma<64, true>(A, Q, nseq, n, stream);
-    else if (A.dh <= 128) rc = launch_attn_mma<128, true>(A, Q, nseq, n, stream);
-    else rc = launch_attn_mma<256, true>(A, Q, nseq, n, stream);
+    if (!w16) rc = A.dh <= 160 ? launch_attn_mma<160, false>(A, Q, nseq, n, w, ld, stream) : launch_attn_mma<256, false>(A, Q, nseq, n, w, ld, stream);
+    else if (A.dh <= 32) rc = launch_attn_mma<32, true>(A, Q, nseq, n, w, ld, stream);
+    else if (A.dh <= 64) rc = launch_attn_mma<64, true>(A, Q, nseq, n, w, ld, stream);
+    else if (A.dh <= 128) rc = launch_attn_mma<128, true>(A, Q, nseq, n, w, ld, stream);
+    else rc = launch_attn_mma<256, true>(A, Q, nseq, n, w, ld, stream);
     return rc ? rc : 1;
 }
 
@@ -462,6 +640,16 @@ extern "C" int jk_prior_prefill(jk_prior* p, const jk_prefill_args* a, jk_stream
     JK_REQUIRE(a->x_cond_len == 0 || a->x_cond_len == 1 || a->x_cond_len == c.n_ctx, "x_cond_len must be 1 or n_ctx");
     const int W = c.width, S = c.n_state, Mw = c.mlp_width, H = c.heads;
     const int rows = n * P;
+    JK_REQUIRE(a->n_record >= 0 && (a->n_record == 0 || a->record), "record: %d layers but no table", a->n_record);
+    const jk_attn_record* rec[JK_MAX_DEPTH] = {};     // per layer: its entry of a->record, or NULL
+    for (int i = 0; i < a->n_record; ++i) {
+        const jk_attn_record& r = a->record[i];
+        JK_REQUIRE(r.layer >= 0 && r.layer < c.depth, "record: layer %d out of range (depth %d)", r.layer, c.depth);
+        JK_REQUIRE(!rec[r.layer], "record: layer %d listed twice", r.layer);
+        JK_REQUIRE(r.ld >= 1, "record: layer %d has ld %d (>= 1 keys per row)", r.layer, r.ld);
+        JK_REQUIRE(r.w, "record: layer %d has no output buffer", r.layer);
+        rec[r.layer] = &r;
+    }
     {
         const size_t cnt = (size_t)rows * W;
         embed_rows_kernel<<<(unsigned)((cnt + 255) / 256), 256, 0, stream>>>(
@@ -476,6 +664,7 @@ extern "C" int jk_prior_prefill(jk_prior* p, const jk_prefill_args* a, jk_stream
     JK_CHECK_CUDA(cudaGetDevice(&dev));
     if (!attr_set[dev & 63]) {
         JK_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+        JK_CHECK_CUDA(cudaFuncSetAttribute(attn_record_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
         attr_set[dev & 63] = true;
     }
     JK_REQUIRE(fwd_smem <= 64 * 1024, "prefill attention tile too large");
@@ -491,11 +680,21 @@ extern "C" int jk_prior_prefill(jk_prior* p, const jk_prefill_args* a, jk_stream
         A.qkv = p->pf_qkv; A.a = p->pf_a; A.P = P; A.S = S; A.H = H; A.dh = E.dh; A.bc = E.bc; A.attn_func = LD.attn_func;
         A.prime = E.prime_pad; A.scale2 = E.scale2; A.q_stride = q_stride; A.kc = LD.kc; A.vc = LD.vc; A.enc_rows = E.enc_dims;
         A.dhp = E.dh_pad;
-        rc = attn_forward_mma(A, n, stream);            // tensor cores when the head geometry allows (dh % 8 == 0, dh <= 256)
+        rc = attn_mma(A, n, nullptr, 0, stream);        // tensor cores when the head geometry allows (dh even, dh <= 256)
         if (rc < 0) return rc;
         if (rc == 0) {
             attn_fwd_kernel<<<dim3(P, H, n), kFwdThreads, fwd_smem, stream>>>(A);
             JK_CHECK_CUDA(cudaGetLastError());
+        }
+        if (const jk_attn_record* r = rec[l]) {         // reads q / K only: before the next layer overwrites pf_qkv
+            __half* w = (__half*)r->w;
+            JK_CHECK_CUDA(cudaMemsetAsync(w, 0, (size_t)n * H * P * r->ld * sizeof(__half), stream));
+            rc = attn_mma(A, n, w, r->ld, stream);
+            if (rc < 0) return rc;
+            if (rc == 0) {
+                attn_record_kernel<<<dim3(P, H, n), kFwdThreads, fwd_smem, stream>>>(A, w, r->ld);
+                JK_CHECK_CUDA(cudaGetLastError());
+            }
         }
         if (!enc) {
             const size_t cnt = (size_t)rows * S;

@@ -11,6 +11,31 @@ from . import _lib
 from ._lib import lib, check, ptr, stream_ptr
 
 
+def prior_config(*, width, depth, heads, n_state, mlp_width, n_ctx, blocks, attn_funcs, bins=0, prime_len=0,
+                 encoder_dims=0, max_batch=16, add_cond_after=True):
+    """the jk_prior_config of an engine (include/jkb200.h)"""
+    cfg = _lib.PriorConfig()
+    cfg.width, cfg.depth, cfg.heads, cfg.n_state, cfg.mlp_width = width, depth, heads, n_state, mlp_width
+    cfg.n_ctx, cfg.blocks, cfg.bins = n_ctx, blocks or 0, bins
+    cfg.prime_len, cfg.encoder_dims = prime_len or 0, encoder_dims or 0
+    cfg.max_batch, cfg.add_cond_after = max_batch, int(bool(add_cond_after))
+    assert len(attn_funcs) == depth <= _lib.JK_MAX_DEPTH
+    for i, f in enumerate(attn_funcs):
+        cfg.attn_func[i] = f
+    return cfg
+
+
+def config_prefill_capacity(device, **kw):
+    """positions one prefill call of an engine built with DecodeEngine(**kw) could take, without building it; 0 when
+    that configuration has no prefill or cannot make an engine at all (jk_prior_config_prefill_capacity)"""
+    if kw.get("max_batch", 16) > _lib.JK_MAX_BATCH:
+        return 0
+    out = C.c_int(0)
+    with torch.cuda.device(device):
+        rc = lib().jk_prior_config_prefill_capacity(C.byref(prior_config(**kw)), C.byref(out))
+    return out.value if rc == 0 else 0
+
+
 class DecodeEngine:
     def __init__(self, *, width, depth, heads, n_state, mlp_width, n_ctx, blocks, attn_funcs,
                  bins=0, prime_len=0, encoder_dims=0, max_batch=16, add_cond_after=True, device=None):
@@ -21,14 +46,9 @@ class DecodeEngine:
             raise RuntimeError(f"n_samples {max_batch} > {_lib.JK_MAX_BATCH} (the decode kernel's largest row count): "
                                "split the batch (sample.py does, via max_batch_size)")
         self.device = device
-        cfg = _lib.PriorConfig()
-        cfg.width, cfg.depth, cfg.heads, cfg.n_state, cfg.mlp_width = width, depth, heads, n_state, mlp_width
-        cfg.n_ctx, cfg.blocks, cfg.bins = n_ctx, blocks or 0, bins
-        cfg.prime_len, cfg.encoder_dims = prime_len or 0, encoder_dims or 0
-        cfg.max_batch, cfg.add_cond_after = max_batch, int(bool(add_cond_after))
-        assert len(attn_funcs) == depth <= _lib.JK_MAX_DEPTH
-        for i, f in enumerate(attn_funcs):
-            cfg.attn_func[i] = f
+        cfg = prior_config(width=width, depth=depth, heads=heads, n_state=n_state, mlp_width=mlp_width, n_ctx=n_ctx,
+                           blocks=blocks, attn_funcs=attn_funcs, bins=bins, prime_len=prime_len,
+                           encoder_dims=encoder_dims, max_batch=max_batch, add_cond_after=add_cond_after)
         self.cfg = cfg
         self.max_batch = max_batch
         with torch.cuda.device(device):
@@ -127,9 +147,13 @@ class DecodeEngine:
         check(lib().jk_prior_prefill_capacity(self.handle, C.byref(out)))
         return out.value
 
-    def prefill(self, n, n_positions, *, tokens=None, y_cond=None, x_cond=None, h_out=None):
+    def prefill(self, n, n_positions, *, tokens=None, y_cond=None, x_cond=None, h_out=None, record=None):
         """positions 0..n_positions-1 of all samples through every layer at once (wgmma GEMMs);
-        afterwards the engine is at position n_positions."""
+        afterwards the engine is at position n_positions.
+
+        record: {layer: w} - fp16 CUDA tensors [n, heads, n_positions, ld] that receive the layer's normalised attention
+        weights (keys by absolute position, or encoder row for an encoder-decoder layer; keys >= ld are dropped; zeros
+        outside the layer's pattern).  See jk_attn_record in include/jkb200.h."""
         a = _lib.PrefillArgs()
         a.n_samples, a.n_positions = n, n_positions
         a.tokens = ptr(tokens)
@@ -138,6 +162,16 @@ class DecodeEngine:
         a.x_cond = ptr(x_cond)
         a.x_cond_len = x_cond.shape[1] if x_cond is not None else 1
         a.h_out = ptr(h_out)
+        if record:
+            table = (_lib.AttnRecord * len(record))()
+            for e, (layer, w) in zip(table, record.items()):
+                if (w.dtype != torch.float16 or w.dim() != 4 or tuple(w.shape[:3]) != (n, self.cfg.heads, n_positions)
+                        or w.device != self.device or not w.is_contiguous()):
+                    raise RuntimeError(f"record[{layer}]: need a contiguous fp16 tensor [{n}, {self.cfg.heads}, "
+                                       f"{n_positions}, ld] on {self.device}, got {w.dtype} {tuple(w.shape)} on {w.device}"
+                                       f"{'' if w.is_contiguous() else ' (strided)'}")
+                e.layer, e.ld, e.w = int(layer), w.shape[3], ptr(w)
+            a.record, a.n_record = table, len(record)
         with torch.cuda.device(self.device):
             check(lib().jk_prior_prefill(self.handle, C.byref(a), stream_ptr()))
         self.position = n_positions

@@ -155,7 +155,9 @@ class ConditionalAutoregressive2D(nn.Module):
         separated enc-dec priors, prior.py:285-301), else (loss in bits per token, preds | acts | None).
 
         fp16=True runs the causal stack through the fp16 decode engine (prefill kernels); fp16=False runs the fp32
-        forward-mode path (csrc/f32_path.cu).  No gradients: training is out of scope, the loss is an evaluation."""
+        forward-mode path (csrc/f32_path.cu).  With attention recording on (Transformer.set_record_attn), fp16=True
+        records in the same prefill when the window fits one prefill call (D <= prefill_capacity), else it takes the
+        fp32 path.  No gradients: training is out of scope, the loss is an evaluation."""
         with t.no_grad():
             x = self.preprocess(x)
             N, D = x.shape
@@ -163,7 +165,11 @@ class ConditionalAutoregressive2D(nn.Module):
             assert (0 <= x).all() and (x < self.bins).all()
             x_cond, y_cond = self._check_conds(N, x_cond, y_cond)
             x = x.contiguous()
-            if fp16 and not self.transformer._record_layers:
+            if fp16 and self.transformer._record_layers:     # asked before an engine is built: else the fp32 path
+                self.transformer.configure_engine(bins=0 if self.only_encode else self.bins,
+                                                  add_cond_after=self.add_cond_after_transformer)
+                fp16 = 1 < D <= self.transformer.prefill_capacity(N)
+            if fp16:
                 acts = self._acts_fp16(x, x_cond, y_cond, encoder_kv)
             else:
                 from ..transformer import f32
@@ -191,17 +197,23 @@ class ConditionalAutoregressive2D(nn.Module):
 
     def _acts_fp16(self, x, x_cond, y_cond, encoder_kv):
         """the causal stack over given tokens on the fp16 decode engine: position by position it computes exactly the
-        forward pass (reference check_sample, factored_attention.py:424-455)"""
+        forward pass (reference check_sample, factored_attention.py:424-455).  The recorded layers' attention weights come
+        from the prefill (fp16, Transformer.store_ws)."""
         N, D = x.shape
+        tr = self.transformer
         eng = self._engine(N)
-        self.transformer.del_cache()
-        if any(b.attn_func == 6 for b in self.transformer._attn_mods):
+        tr.del_cache()
+        if any(b.attn_func == 6 for b in tr._attn_mods):
             assert encoder_kv is not None
             eng.set_encoder_kv(encoder_kv)
         acts = t.empty(N, D, self.width, dtype=t.float32, device=x.device)
         if 1 < D <= eng.prefill_capacity:
-            eng.prefill(N, D, tokens=x, y_cond=y_cond, x_cond=x_cond, h_out=acts)
+            ws = {i: t.empty(N, tr.n_head, D, tr.record_ld(i), dtype=t.float16, device=x.device) for i in tr._record_layers}
+            eng.prefill(N, D, tokens=x, y_cond=y_cond, x_cond=x_cond, h_out=acts, record=ws)
+            if ws:
+                tr.store_ws(ws)
         else:
+            assert not tr._record_layers, "attention is recorded by the prefill"
             for i in range(D):
                 out = t.empty(N, self.width, dtype=t.float32, device=x.device)
                 eng.step(N, tokens=x, y_cond=y_cond, x_cond=x_cond, h_out=out)

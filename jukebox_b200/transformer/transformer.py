@@ -111,15 +111,10 @@ class Transformer(nn.Module):
         if dev.type != "cuda":
             raise RuntimeError("Transformer.forward(sample=True) needs the module on a CUDA device: "
                                "jukebox_b200 has no CPU path (use the oracle in tests)")
-        if self._engine is None or self._engine.max_batch < n_samples or self._engine.device != dev:
+        if not self._engine_fits(n_samples, dev):
             if self.res_scale_unsupported():
                 raise NotImplementedError("res_scale=True priors are not supported by the decode engine yet")
-            l0 = self._attn_mods[0]
-            eng = DecodeEngine(width=self.n_in, depth=self.n_depth, heads=self.n_head, n_state=l0.attn.n_state,
-                               mlp_width=l0.mlp.c_fc.n_out, n_ctx=self.n_ctx, blocks=self.blocks,
-                               attn_funcs=[l.attn_func for l in self._attn_mods],
-                               prime_len=self.prime_len, encoder_dims=self.encoder_dims,
-                               max_batch=max(1, n_samples), device=dev, **self._engine_cfg)
+            eng = DecodeEngine(device=dev, **self._engine_kwargs(n_samples))
             for i, blk in enumerate(self._attn_mods):
                 eng.load_layer(i, blk)
             self._engine = eng
@@ -128,15 +123,41 @@ class Transformer(nn.Module):
                 l.attn.del_cache()
         return self._engine
 
+    def _engine_fits(self, n_samples, dev):
+        return self._engine is not None and self._engine.max_batch >= n_samples and self._engine.device == dev
+
+    def _engine_kwargs(self, n_samples):
+        l0 = self._attn_mods[0]
+        return dict(width=self.n_in, depth=self.n_depth, heads=self.n_head, n_state=l0.attn.n_state,
+                    mlp_width=l0.mlp.c_fc.n_out, n_ctx=self.n_ctx, blocks=self.blocks,
+                    attn_funcs=[l.attn_func for l in self._attn_mods], prime_len=self.prime_len,
+                    encoder_dims=self.encoder_dims, max_batch=max(1, n_samples), **self._engine_cfg)
+
+    def prefill_capacity(self, n_samples):
+        """positions one fp16 prefill of n_samples can take, without building an engine when none is built yet: 0 when
+        this stack has no prefill, or no engine for this configuration / batch (more than JK_MAX_BATCH samples)"""
+        from ..engine import config_prefill_capacity
+        dev = self._attn_mods[0].ln_0.weight.device
+        if self._engine_fits(n_samples, dev):
+            return self._engine.prefill_capacity
+        if dev.type != "cuda" or self.res_scale_unsupported():
+            return 0
+        return config_prefill_capacity(dev, **self._engine_kwargs(n_samples))
+
     def res_scale_unsupported(self):
         return any(l.res_scale != 1.0 for l in self._attn_mods)
 
     # ---- reference surface --------------------------------------------------------------
     def set_record_attn(self, record_attn):
         """record_attn: False / True / a collection of layer indices (reference transformer.py:146-163).  Recorded
-        weights are produced by the forward-mode fp32 path and appear in `self.ws` after the next forward call, one
-        [n, heads, queries, keys] tensor per recorded layer, keys indexed by absolute position (for dense and enc-dec
-        layers - the ones alignment reads, prior.py:327-344 - that is the reference's own layout)."""
+        weights appear in `self.ws` after the next whole-sequence forward, one [n, heads, queries, keys] tensor per
+        recorded layer, keys indexed by absolute position (encoder row for an enc-dec layer; a prime layer keeps its
+        music queries x lyric keys, [:, :, prime_len:, :prime_len]) - the reference's own layout.  Zeros outside a
+        layer's pattern.  Which pass records them:
+          ConditionalAutoregressive2D.forward(fp16=True) with a window that fits one prefill (prefill_capacity): the fp16
+              prefill, fp16 weights fp16(softmax_fp32(fp16(fp16(q.k) * dh^-1/2))) - the reference's fp16 mode;
+          any other whole-sequence forward (fp16=False, Transformer.forward(sample=False), longer windows): the fp32
+              forward-mode path, fp32 weights."""
         def _on(layer_idx):
             if isinstance(record_attn, bool):
                 return record_attn
@@ -170,19 +191,29 @@ class Transformer(nn.Module):
         out, ws = path.run(x, encoder_kv, 0, record=self._record_layers)
         path.reset()
         if self._record_layers:
-            for i in self._record_layers:      # prime layers keep music queries x lyric keys (factored_attention.py:103-105)
-                if self._attn_mods[i].attn_func == 7:
-                    ws[i] = ws[i][:, :, self.prime_len:, :self.prime_len]
-            self.ws = [ws[i] for i in self._record_layers]
-            for i in self._record_layers:
-                self._attn_mods[i].attn.w = ws[i]
+            self.store_ws(ws)
         return out
+
+    def record_ld(self, layer):
+        """keys per recorded row of `layer`: encoder rows (enc-dec), the lyric prefix (prime), else the context"""
+        f = self._attn_mods[layer].attn_func
+        return self.encoder_dims if f == 6 else self.prime_len if f == 7 else self.n_ctx
+
+    def store_ws(self, ws):
+        """ws: {layer: [n, heads, n_ctx, keys]} weights of the recorded layers -> self.ws / attn.w"""
+        for i in self._record_layers:          # prime layers keep music queries x lyric keys (factored_attention.py:103-105)
+            if self._attn_mods[i].attn_func == 7:
+                ws[i] = ws[i][:, :, self.prime_len:, :self.prime_len]
+        self.ws = [ws[i] for i in self._record_layers]
+        for i in self._record_layers:
+            self._attn_mods[i].attn.w = ws[i]
 
     def forward(self, x, encoder_kv=None, sample=False, fp16=False, fp16_out=False):
         assert x.dim() == 3 and x.shape[2] == self.n_in
         if not sample or not fp16:
-            # forward mode (any fp16 flag: computed in fp32, a superset of the reference's fp16 precision) and fp32
-            # sampling: csrc/f32_path.cu
+            # forward mode over activations (any fp16 flag: computed in fp32, a superset of the reference's fp16
+            # precision; the fp16 prefill starts from tokens, ConditionalAutoregressive2D._acts_fp16) and fp32 sampling:
+            # csrc/f32_path.cu
             out = self._forward_f32(x, encoder_kv, sample)
             return out.half() if fp16_out else out
         n, l = x.shape[0], x.shape[1]
