@@ -240,6 +240,21 @@ typedef struct jk_conv_args {
 } jk_conv_args;
 int jk_conv1d_cl(const jk_conv_args* a, jk_stream_t stream);
 
+/* Wide decoder-side convolutions on the tensor cores (wgmma + TMA): the convs of the upsampler Conditioner
+ * (prior/conditioners.py:8-48), c_in and c_out multiples of 64 with one of them above 64.  Same arithmetic contract as
+ * tensor_cores = 1 above: every product is the fp16 x 3 split hi.w_hi + lo.w_hi + hi.w_lo with the weights scaled by 2^8
+ * before the split, fp32 accumulation, free summation order.
+ * jk_pack_conv_weight_split turns a packed fp32 weight [k, c_in, c_out] (jk_pack_conv_weight, or one phase of a
+ * transposed conv) into the layout the kernel streams: [hi | lo][c_out][k * c_in] fp16, jk_conv_weight_split_bytes bytes
+ * of device memory (16-byte aligned).  Do it once per weight load.
+ * jk_conv1d_tc_wide computes exactly what jk_conv1d_cl documents, reading the weight from w_split (a->w is read only
+ * when JK_CONV_EXACT is set, which runs the exact FMA kernel instead); a->tensor_cores is ignored.  It takes in_stride 1,
+ * 1..3 taps, t_in >= 128 and 16-byte aligned in / out / bias / res, and returns an error naming the constraint otherwise:
+ * callers keep jk_conv1d_cl for those shapes. */
+int jk_conv_weight_split_bytes(int k, int c_in, int c_out, size_t* bytes);
+int jk_pack_conv_weight_split(const float* packed, void* split, int k, int c_in, int c_out, jk_stream_t stream);
+int jk_conv1d_tc_wide(const jk_conv_args* a, const void* w_split, jk_stream_t stream);
+
 /* ResConv1DBlock (vqvae/resnet.py:27-44): out = x + res_scale * (W2.relu(W1 *_dil relu(x) + b1) + b2)
  * x, out [n, T, C] (x != out); w1 packed [3, C, Cs]; w2 packed [1, Cs, C].  For C == Cs in {32, 64} (every
  * ResConv1DBlock of the reference's VQ-VAEs) this is ONE launch with the hidden activation kept in shared memory and

@@ -104,6 +104,9 @@ SIGNATURES = {
     "jk_vq_argmin": (_I, [_P, _P, _P, _P, _L, _I, _I, _P]),
     "jk_vq_gather": (_I, [_P, _P, _P, _L, _I, _I, _P]),
     "jk_conv1d_cl": (_I, [C.POINTER(ConvArgs), _P]),
+    "jk_conv_weight_split_bytes": (_I, [_I, _I, _I, C.POINTER(C.c_size_t)]),
+    "jk_pack_conv_weight_split": (_I, [_P, _P, _I, _I, _I, _P]),
+    "jk_conv1d_tc_wide": (_I, [C.POINTER(ConvArgs), _P, _P]),
     "jk_resblock_cl": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _L, _I, _I, _I, _F, _P]),
     "jk_resblock_tc": (_I, [_P, _P, _P, _P, _P, _P, _I, _L, _I, _I, _F, _P]),
     "jk_pack_conv_weight": (_I, [_P, _P, _I, _I, _I, _I, _P]),

@@ -1103,6 +1103,10 @@ int conv_t5(const float* in, long long t_in, int c_in, float* out, long long t_o
             cudaStream_t stream);                                                 // vqvae_t5.cu
 int resblock_t5(const float* x, float* out, const float* w1, const float* b1, const float* w2, const float* b2, int n,
                 long long T, int C, int dil, float rs, cudaStream_t stream);      // vqvae_t5.cu
+int conv_wide_t5(const float* in, long long t_in, int c_in, float* out, long long t_out, int c_out, const void* w_split,
+                 const float* bias, const float* res, int n_taps, const int* tap_off, int out_stride, int out_offset,
+                 int relu_in, float scale, int n, cudaStream_t stream);       // vqvae_t5.cu
+int pack_conv_weight_split(const float* packed, void* split, int k, int c_in, int c_out, cudaStream_t stream);   // vqvae_t5.cu
 }
 
 extern "C" int jk_conv1d_cl(const jk_conv_args* a, jk_stream_t stream_) {
@@ -1214,6 +1218,42 @@ extern "C" int jk_pack_conv_weight(const float* w, float* packed, int c_out, int
     pack_conv_weight_kernel<<<(total + 255) / 256, 256, 0, stream>>>(w, packed, c_out, c_in, k, transposed);
     JK_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+extern "C" int jk_conv_weight_split_bytes(int k, int c_in, int c_out, size_t* bytes) {
+    JK_REQUIRE(bytes, "null argument");
+    JK_REQUIRE(k >= 1 && c_in >= 1 && c_out >= 1, "k, c_in and c_out must be positive");
+    *bytes = (size_t)2 * k * c_in * c_out * 2;
+    return 0;
+}
+
+extern "C" int jk_pack_conv_weight_split(const float* packed, void* split, int k, int c_in, int c_out, jk_stream_t stream) {
+    JK_REQUIRE(packed && split, "null argument");
+    JK_REQUIRE(k >= 1 && c_in >= 1 && c_out >= 1, "k, c_in and c_out must be positive");
+    return jk::pack_conv_weight_split(packed, split, k, c_in, c_out, (cudaStream_t)stream);
+}
+
+extern "C" int jk_conv1d_tc_wide(const jk_conv_args* a, const void* w_split, jk_stream_t stream) {
+    JK_REQUIRE(a && a->in && a->out && w_split, "null argument");
+    static const bool conv_exact = getenv("JK_CONV_EXACT") != nullptr;      // A/B: the exact FMA kernel, as for narrow convs
+    if (conv_exact) {
+        JK_REQUIRE(a->w, "jk_conv1d_tc_wide: JK_CONV_EXACT needs the packed fp32 weight in w");
+        jk_conv_args e = *a;
+        e.tensor_cores = 0;
+        return jk_conv1d_cl(&e, stream);
+    }
+    JK_REQUIRE(a->c_in % 64 == 0 && a->c_out % 64 == 0 && a->c_in > 0 && a->c_out > 0 && (a->c_in > 64 || a->c_out > 64),
+               "jk_conv1d_tc_wide: c_in and c_out must be multiples of 64 and one of them above 64 (got %d -> %d)", a->c_in, a->c_out);
+    JK_REQUIRE(a->in_stride == 1, "jk_conv1d_tc_wide: the input stride must be 1 (got %d)", a->in_stride);
+    JK_REQUIRE(a->n_taps >= 1 && a->n_taps <= 3, "jk_conv1d_tc_wide: n_taps must be 1..3 (got %d)", a->n_taps);
+    JK_REQUIRE(a->t_in >= 128, "jk_conv1d_tc_wide: t_in must be at least 128 positions (got %lld)", (long long)a->t_in);
+    JK_REQUIRE(a->n >= 1 && a->n <= 65535, "jk_conv1d_tc_wide: batch out of range");
+    JK_REQUIRE(a->out_stride >= 1 && a->out_offset >= 0 && a->out_offset < a->out_stride, "jk_conv1d_tc_wide: bad output stride / offset");
+    JK_REQUIRE((((uintptr_t)a->in | (uintptr_t)a->out | (uintptr_t)a->bias | (uintptr_t)a->res | (uintptr_t)w_split) & 15) == 0,
+               "jk_conv1d_tc_wide: in, out, bias, res and w_split must be 16-byte aligned");
+    if (a->t_out == 0) return 0;
+    return jk::conv_wide_t5(a->in, a->t_in, a->c_in, a->out, a->t_out, a->c_out, w_split, a->bias, a->res, a->n_taps, a->tap_off,
+                            a->out_stride, a->out_offset, a->relu_in, a->scale, a->n, (cudaStream_t)stream);
 }
 
 extern "C" int jk_layernorm_f32(const float* x, const float* g, const float* b, float* y, int64_t rows, int width,

@@ -448,6 +448,212 @@ conv_t5_kernel(const __grid_constant__ CUtensorMap map_x, ConvT5P P, int tiles_p
     }
 }
 
+// ---------------------------------------------------------------------------------------
+// Wide tap-GEMM convolution on the same roles, for c_in, c_out multiples of 64 with one of them above 64 (the upsampler
+// Conditioner's 512 / 1024 / 1920 channels, prior/conditioners.py):
+//   out[t * os + oo, co0 .. co0 + BN) = res + scale * (sum_tap sum_ci x[t + off_tap, ci] . W[tap, ci, co] + b)
+// K = taps x c_in no longer fits one operand tile and the weights no longer fit in shared memory, so
+//   - a work item is 128 positions x BN output channels (BN = 128, or 64 when c_out is an odd multiple of 64).  Items are
+//     numbered position-tile major: the CTAs that work on the channel tiles of one position tile at the same time share
+//     its activation rows in L2;
+//   - the K loop runs over the 64-channel blocks of every tap through a kS-stage ring.  A stage holds the fp32 block
+//     [128 positions x 64 channels] as TMA delivers it - the converters turn it IN PLACE into its hi / lo fp16 planes
+//     (16 KB each) - and the hi / lo planes of the weight block [BN x 64], which TMA loads with the 128-byte swizzle
+//     straight from the split weight that jk_pack_conv_weight_split made once per weight load ([hi | lo][c_out][taps *
+//     c_in] fp16 of 2^8 w);
+//   - every K block's 12 wgmmas go into a zeroed partial accumulator that is then added to the item's fp32 sum with
+//     ordinary (round-to-nearest) adds.  The tensor core's own accumulation rounds each k16 step's sum towards zero, and
+//     over K = 5760 that bias grows to ~2e-5 of the output scale; promoted every 64 channels it stays at the exact
+//     kernel's level.  The second accumulator is what the register reallocation below pays for;
+//   - the epilogue writes scale * (acc / 2^8 + b) (+ res) from the accumulator fragments: the four lanes of a quad cover
+//     32 contiguous bytes of one row (whole sectors, also for the row-strided phases of a transposed conv), and shared
+//     memory is left to the ring.
+// Roles, four warpgroups: consumers 0-1 (rows 0-63 / 64-127 of the item, 184 registers), converters (warps 8-11, 104
+// registers), TMA producer (warp 12; warps 13-15 only hand their registers back, 40 each).
+// ---------------------------------------------------------------------------------------
+struct ConvWideP {
+    const float* bias; const float* res; float* out;
+    long long t_out;
+    int c_in, c_out, n_taps, tap_off[3], out_stride, out_offset, relu_in;
+    float scale;
+};
+
+template <int BN>
+struct T5W {
+    static constexpr int kS = BN == 128 ? 3 : 4;             // ring stages (what 227 KB of shared memory leaves room for)
+    static constexpr int kA = kBM * 64 * 4;                  // fp32 block; after conversion hi plane | lo plane (16 KB each)
+    static constexpr int kAPlane = kBM * 128;
+    static constexpr int kB = BN * 128;                      // one weight plane: BN rows x 64 fp16
+    static constexpr int kStage = kA + 2 * kB;
+    static constexpr int offBar = kS * kStage;
+    static constexpr int smem = offBar + 128 + 1024;         // barriers, and slack to align the ring to 1024 bytes
+};
+
+__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
+            smem_u32(smem_dst)),
+        "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+        : "memory");
+}
+
+// fp32 block [128][64] at st -> (relu) -> hi plane at st, lo plane at st + 16 KB, by the 128 converter threads: every
+// value is read into registers before the group barrier, so the planes can overwrite the block they come from
+__device__ __forceinline__ void convert_block_inplace(uint8_t* st, int ct, bool relu) {
+    constexpr int CH = 16, PER = kBM * CH / 128;            // float4 chunks per row, items per thread
+    const float4* f = reinterpret_cast<const float4*>(st);
+    float4 v[PER];
+#pragma unroll
+    for (int j = 0; j < PER; ++j) v[j] = f[ct + j * 128];
+    uint2 h[PER], l[PER];
+#pragma unroll
+    for (int j = 0; j < PER; ++j) {
+        if (relu) { v[j].x = fmaxf(v[j].x, 0.f); v[j].y = fmaxf(v[j].y, 0.f); v[j].z = fmaxf(v[j].z, 0.f); v[j].w = fmaxf(v[j].w, 0.f); }
+        t5_split2(v[j].x, v[j].y, h[j].x, l[j].x);
+        t5_split2(v[j].z, v[j].w, h[j].y, l[j].y);
+    }
+    named_sync(1);
+#pragma unroll
+    for (int j = 0; j < PER; ++j) {
+        const int item = ct + j * 128, r = item / CH, c4 = item % CH;
+        const uint32_t o = sw_off(r, c4 >> 1) + (c4 & 1) * 8;
+        *reinterpret_cast<uint2*>(st + o) = h[j];
+        *reinterpret_cast<uint2*>(st + kBM * 128 + o) = l[j];
+    }
+}
+
+constexpr int kWideThreads = 512;
+
+template <int BN>
+__global__ void __launch_bounds__(kWideThreads, 1)
+conv_wide_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w, ConvWideP P,
+                 int tiles_per_clip, int n_tiles_n, int total_items) {
+    using L = T5W<BN>;
+    constexpr int S = L::kS;
+    extern __shared__ __align__(1024) uint8_t sm_raw[];
+    uint8_t* sm = sm_raw + ((1024u - (smem_u32(sm_raw) & 1023u)) & 1023u);   // TMA's 128-byte swizzle needs 1024-byte stages
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sm + L::offBar);
+    uint64_t *full = bars, *conv = bars + S, *empty = bars + 2 * S;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int kb_per_tap = P.c_in / 64, n_kb = P.n_taps * kb_per_tap;
+    if (tid == 0) {
+        // full: the producer's expect_tx (activation + weight bytes); conv: the 128 converter threads; empty: one arrival
+        // per consumer warpgroup once its MMAs on the stage have retired
+        for (int i = 0; i < S; ++i) { mbar_init(&full[i], 1); mbar_init(&conv[i], 128); mbar_init(&empty[i], 2); }
+        mbar_fence_init();
+        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_x)) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_w)) : "memory");
+    }
+    __syncthreads();
+    const int first = blockIdx.x, stride = gridDim.x;
+
+    // register reallocation (setmaxnreg, whole warpgroups): the block launches with 128 per thread (65536 / 512);
+    // 2 x 128 x 184 + 128 x 104 + 128 x 40 = 65536
+    if (warp >= 12) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (warp == 12 && lane == 0) {
+            uint32_t kt = 0;
+            for (int item = first; item < total_items; item += stride) {
+                const int mt = item / n_tiles_n, co0 = (item - mt * n_tiles_n) * BN;
+                const int nb = mt / tiles_per_clip, t0 = (mt - nb * tiles_per_clip) * kBM;
+                for (int kb = 0; kb < n_kb; ++kb, ++kt) {
+                    const int s = kt % S, tap = kb / kb_per_tap, c0 = (kb - tap * kb_per_tap) * 64;
+                    mbar_wait(&empty[s], ((kt / S) & 1) ^ 1);
+                    mbar_expect_tx(&full[s], (uint32_t)L::kStage);
+                    const int off = tap == 0 ? P.tap_off[0] : tap == 1 ? P.tap_off[1] : P.tap_off[2];
+                    uint8_t* st = sm + s * L::kStage;
+                    // rows outside [0, T) of clip nb - a whole block of them when the dilation exceeds T - arrive as zeros
+                    tma_load_3d(st, &map_x, c0, t0 + off, nb, &full[s]);
+                    tma_load_2d(st + L::kA, &map_w, tap * P.c_in + c0, co0, &full[s]);
+                    tma_load_2d(st + L::kA + L::kB, &map_w, tap * P.c_in + c0, P.c_out + co0, &full[s]);
+                }
+            }
+        }
+    } else if (warp >= 8) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 104;");
+        const int ct = tid & 127;
+        const bool relu = P.relu_in != 0;
+        uint32_t kt = 0;
+        for (int item = first; item < total_items; item += stride) {
+            for (int kb = 0; kb < n_kb; ++kb, ++kt) {
+                const int s = kt % S;
+                mbar_wait(&full[s], (kt / S) & 1);
+                convert_block_inplace(sm + s * L::kStage, ct, relu);
+                fence_async_smem();                   // the planes are read by the tensor core (async proxy)
+                mbar_arrive(&conv[s]);
+            }
+        }
+    } else {
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 184;");
+        const int wg = warp >> 2, wt = tid & 127, rq = wg * 64 + (wt >> 5) * 16 + (lane >> 2);
+        const uint32_t ring = smem_u32(sm);
+        uint32_t kt = 0;
+        for (int item = first; item < total_items; item += stride) {
+            const int mt = item / n_tiles_n, co0 = (item - mt * n_tiles_n) * BN;
+            const int nb = mt / tiles_per_clip, t0 = (mt - nb * tiles_per_clip) * kBM;
+            float acc[BN / 2];
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+            for (int kb = 0; kb < n_kb; ++kb, ++kt) {
+                const int s = kt % S;
+                const uint32_t ph = (kt / S) & 1;
+                mbar_wait(&full[s], ph);              // weight planes (TMA)
+                mbar_wait(&conv[s], ph);              // activation planes (converters)
+                const uint32_t st = ring + s * L::kStage, ah = st + wg * (64 * 128), al = ah + L::kAPlane;
+                float part[BN / 2];
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) part[i] = 0.f;
+                mma_tap<64, BN>(part, ah, al, st + L::kA, st + L::kA + L::kB);
+                wgmma_wait<0>();
+                if (wt == 0) mbar_arrive(&empty[s]);  // the block has retired: free its stage
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+            }
+            // ---- out = res + scale * (acc / 2^8 + b), straight from the fragments ----
+            const long long rows_out = P.t_out * P.out_stride;
+            float* ob = P.out + (size_t)nb * rows_out * P.c_out + co0;
+            const float* rb = P.res ? P.res + (size_t)nb * rows_out * P.c_out + co0 : nullptr;
+            const float* bb = P.bias ? P.bias + co0 : nullptr;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const long long t = (long long)t0 + rq + 8 * h;
+                if (t < P.t_out) {
+                    const size_t ro = (size_t)(t * P.out_stride + P.out_offset) * P.c_out;
+#pragma unroll
+                    for (int i = 0; i < BN / 8; ++i) {
+                        const int col = 8 * i + 2 * (lane & 3);
+                        const float2 b = bb ? __ldg(reinterpret_cast<const float2*>(bb + col)) : make_float2(0.f, 0.f);
+                        float2 o;
+                        o.x = P.scale * fmaf(acc[4 * i + 2 * h], kWInvT5, b.x);
+                        o.y = P.scale * fmaf(acc[4 * i + 2 * h + 1], kWInvT5, b.y);
+                        if (rb) {
+                            const float2 r = __ldg(reinterpret_cast<const float2*>(rb + ro + col));
+                            o.x += r.x; o.y += r.y;
+                        }
+                        *reinterpret_cast<float2*>(ob + ro + col) = o;
+                    }
+                }
+            }
+        }
+    }
+}
+
+// packed fp32 [k, c_in, c_out] -> [hi | lo][c_out][k * c_in] fp16 of 2^8 w (row co, column tap * c_in + ci)
+__global__ void pack_split_kernel(const float* __restrict__ packed, unsigned short* __restrict__ split, int K, int c_out) {
+    const long long total = (long long)K * c_out;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int kk = (int)(i / c_out), co = (int)(i % c_out);   // coalesced reads of the packed weight
+        unsigned short h, l;
+        const float v = kWScaleT5 * __ldg(packed + i);
+        asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(h) : "f"(v));
+        const float rem = v - __half2float(__ushort_as_half(h));
+        asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(l) : "f"(rem));
+        const size_t o = (size_t)co * K + kk;
+        split[o] = h;
+        split[(size_t)K * c_out + o] = l;
+    }
+}
+
 typedef CUresult (*EncodeTiledFnT5)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -524,6 +730,49 @@ int launch_conv_t5(const ConvT5P& P, int n, cudaStream_t stream) {
     JK_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
+
+template <int BN>
+int launch_conv_wide(const float* in, long long t_in, const void* w_split, const ConvWideP& P, int n, cudaStream_t stream) {
+    EncodeTiledFnT5 enc = t5_encode();
+    JK_REQUIRE(enc, "cuTensorMapEncodeTiled is not available from the driver");
+    CUtensorMap map_x, map_w;
+    {
+        cuuint64_t dims[3] = {(cuuint64_t)P.c_in, (cuuint64_t)t_in, (cuuint64_t)n};
+        cuuint64_t strides[2] = {(cuuint64_t)P.c_in * 4, (cuuint64_t)t_in * P.c_in * 4};
+        cuuint32_t box[3] = {64, (cuuint32_t)kBM, 1};
+        cuuint32_t estr[3] = {1, 1, 1};
+        CUresult r = enc(&map_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(in), dims, strides, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        JK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for a [%d, %lld, %d] fp32 tensor", (int)r, n, t_in, P.c_in);
+    }
+    {
+        const long long K = (long long)P.n_taps * P.c_in;
+        cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)2 * P.c_out};
+        cuuint64_t strides[1] = {(cuuint64_t)K * 2};
+        cuuint32_t box[2] = {64, (cuuint32_t)BN};
+        cuuint32_t estr[2] = {1, 1};
+        CUresult r = enc(&map_w, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(w_split), dims, strides, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        JK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for a [2 x %d, %lld] fp16 split weight", (int)r, P.c_out, K);
+    }
+    static bool attr_set[64] = {};
+    static int sms[64] = {};
+    int dev = 0;
+    JK_CHECK_CUDA(cudaGetDevice(&dev));
+    if (!attr_set[dev & 63]) {
+        JK_CHECK_CUDA(cudaFuncSetAttribute(conv_wide_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, T5W<BN>::smem));
+        JK_CHECK_CUDA(cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
+        attr_set[dev & 63] = true;
+    }
+    const long long per_clip = (P.t_out + kBM - 1) / kBM, n_tiles_n = P.c_out / BN, total = per_clip * n * n_tiles_n;
+    JK_REQUIRE(total < (1ll << 31) && t_in + 4096 < (1ll << 31), "clip too long for 32-bit tile coordinates");
+    const unsigned grid = (unsigned)std::min<long long>(total, sms[dev & 63]);
+    conv_wide_kernel<BN><<<grid, kWideThreads, T5W<BN>::smem, stream>>>(map_x, map_w, P, (int)per_clip, (int)n_tiles_n, (int)total);
+    JK_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
 }  // namespace
 
 namespace jk {
@@ -548,6 +797,25 @@ int conv_t5(const float* in, long long t_in, int c_in, float* out, long long t_o
     if (c_in == 32 && c_out == 64) return launch_conv_t5<32, 64>(P, n, stream);
     if (c_in == 32 && c_out == 32) return launch_conv_t5<32, 32>(P, n, stream);
     JK_REQUIRE(false, "conv_t5: channels must be 32 or 64 (got %d -> %d)", c_in, c_out);
+    return 0;
+}
+// jk_conv1d_tc_wide (vqvae_kernels.cu) dispatches here once it has checked the shape: c_in, c_out multiples of 64,
+// stride-1 input, <= 3 taps, t_in >= 128, 16-byte aligned pointers; w_split from pack_conv_weight_split
+int conv_wide_t5(const float* in, long long t_in, int c_in, float* out, long long t_out, int c_out, const void* w_split,
+                 const float* bias, const float* res, int n_taps, const int* tap_off, int out_stride, int out_offset,
+                 int relu_in, float scale, int n, cudaStream_t stream) {
+    ConvWideP P;
+    P.bias = bias; P.res = res; P.out = out; P.t_out = t_out; P.c_in = c_in; P.c_out = c_out; P.n_taps = n_taps;
+    for (int i = 0; i < 3; ++i) P.tap_off[i] = i < n_taps ? tap_off[i] : 0;
+    P.out_stride = out_stride; P.out_offset = out_offset; P.relu_in = relu_in; P.scale = scale;
+    if (c_out % 128 == 0) return launch_conv_wide<128>(in, t_in, w_split, P, n, stream);
+    return launch_conv_wide<64>(in, t_in, w_split, P, n, stream);
+}
+int pack_conv_weight_split(const float* packed, void* split, int k, int c_in, int c_out, cudaStream_t stream) {
+    const long long total = (long long)k * c_in * c_out;
+    const unsigned blocks = (unsigned)std::min<long long>((total + 255) / 256, 65535);
+    pack_split_kernel<<<blocks, 256, 0, stream>>>(packed, static_cast<unsigned short*>(split), k * c_in, c_out);
+    JK_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 }  // namespace jk

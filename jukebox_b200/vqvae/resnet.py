@@ -39,6 +39,8 @@ class ResConv1DBlock(nn.Module):
                 check(lib().jk_resblock_cl(ptr(x), ptr(out), None, ptr(w1), ptr(b1), ptr(w2), ptr(b2), n, T, C_, c3.n_out,
                                            c3.dilation, float(self.res_scale), stream_ptr()))
             return out
+        # two launches through an [n, T, Cs] temporary; with tensor_cores set, the wide shapes of the upsampler
+        # Conditioner (multiples of 64 channels, one above 64) run both on the wgmma kernel (jk_conv1d_tc_wide)
         h = c3(x, relu_in=True)
         return c1(h, relu_in=True, res=x, scale=self.res_scale)
 
@@ -69,7 +71,7 @@ class Resnet1D(nn.Module):
 
 def use_tensor_cores(module, on=True):
     """switch every ResConv1DBlock and channels-last conv below `module` to the split-precision tensor-core kernels
-    (jk_resblock_tc, jk_conv1d_cl with tensor_cores = 1) - decoder-side stacks only"""
+    (jk_resblock_tc, jk_conv1d_cl with tensor_cores = 1, jk_conv1d_tc_wide) - decoder-side stacks only"""
     for m in module.modules():
         if hasattr(m, "tensor_cores"):
             m.tensor_cores = bool(on)
