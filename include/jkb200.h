@@ -270,6 +270,20 @@ int jk_resblock_cl(const float* x, float* out, float* tmp, const float* w1, cons
 int jk_resblock_tc(const float* x, float* out, const float* w1, const float* b1, const float* w2, const float* b2,
                    int n, int64_t T, int C, int dilation, float res_scale, jk_stream_t stream);
 
+/* Spectral losses of VQVAE.forward (utils/audio_utils.py:80-131), one fused kernel: no spectrogram reaches memory.
+ * Per clip n of two mono signals a, b [n, T] fp32 (torch.stft semantics of audio_utils.py:80-84: center=True with
+ * reflect padding of n_fft/2, `window` = the periodic Hann of win_length centred in n_fft at (n_fft - win_length)/2,
+ * onesided, 1 + T/hop frames):
+ *   resid[n]  = sum over frames and bins of (|STFT(a_n)| - |STFT(b_n)|)^2
+ *   norm_a[n] = sum over frames and bins of  |STFT(a_n)|^2            (both float64)
+ * n_fft a power of two in [256, 4096], 1 <= win_length <= n_fft, hop >= 1, T > n_fft/2; anything else is an error.
+ * workspace: device memory of jk_stft_workspace_bytes(n, T, n_fft, hop) bytes (8-byte aligned; 0 for invalid sizes).
+ * The result is bitwise deterministic and the same for a clip whatever the batch it is computed in. */
+int     jk_stft_mag_diff(const float* a, const float* b, const float* window, double* resid, double* norm_a,
+                         int n, int64_t T, int n_fft, int hop, int win_length,
+                         void* workspace, size_t workspace_bytes, jk_stream_t stream);
+size_t  jk_stft_workspace_bytes(int n, int64_t T, int n_fft, int hop);
+
 /* Token sampling of the autoregressive loop (prior/autoregressive.py:233-235, 343-345):
  *   tokens[r, position] ~ Categorical(logits = logits[r, :] / temp),  r = 0..n-1
  * one launch per position.  logits: fp32 rows `logits_stride` floats apart (entries of -inf carry no

@@ -107,6 +107,8 @@ SIGNATURES = {
     "jk_conv_weight_split_bytes": (_I, [_I, _I, _I, C.POINTER(C.c_size_t)]),
     "jk_pack_conv_weight_split": (_I, [_P, _P, _I, _I, _I, _P]),
     "jk_conv1d_tc_wide": (_I, [C.POINTER(ConvArgs), _P, _P]),
+    "jk_stft_mag_diff": (_I, [_P, _P, _P, _P, _P, _I, _L, _I, _I, _I, _P, C.c_size_t, _P]),
+    "jk_stft_workspace_bytes": (C.c_size_t, [_I, _L, _I, _I]),
     "jk_resblock_cl": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _L, _I, _I, _I, _F, _P]),
     "jk_resblock_tc": (_I, [_P, _P, _P, _P, _P, _P, _I, _L, _I, _I, _F, _P]),
     "jk_pack_conv_weight": (_I, [_P, _P, _I, _I, _I, _I, _P]),

@@ -1,7 +1,9 @@
-"""Codebook quantise / dequantise (reference: jukebox/vqvae/bottleneck.py:88-147, 181-199).
+"""Codebook quantise / dequantise (reference: jukebox/vqvae/bottleneck.py:88-147, 181-215).
 
-Only the sampling-time surface is built (encode / decode); k-means EMA updates (`update_k`,
-`forward` with losses) are training and out of scope."""
+The sampling-time surface (encode / decode) and the evaluation-mode forward, which VQVAE.forward uses to measure a
+model: quantise, dequantise, commit loss, no codebook update.  Tensors are channels-last [N, T, emb_width] (the
+reference's are NCT).  The k-means EMA updates (`update_k=True`, a Bottleneck in training mode) are training and out of
+scope."""
 import torch as t
 import torch.nn as nn
 
@@ -48,8 +50,21 @@ class BottleneckBlock(nn.Module):
         N, T = x_l.shape
         return self.dequantise(x_l).view(N, T, self.emb_width)
 
-    def forward(self, x, update_k=True):
-        raise NotImplementedError("codebook EMA training is out of scope (SURVEY.md section 2.1 #4)")
+    def forward(self, x, update_k=False):
+        """x: [N, T, emb_width] -> (codes [N, T], decoder input [N, T, emb_width], commit_loss, dict(fit, pn))
+        (bottleneck.py:168-193 with update_k False)"""
+        if update_k:
+            raise NotImplementedError("codebook EMA training is out of scope (SURVEY.md section 2.1 #4)")
+        N, T, w = x.shape
+        assert w == self.emb_width, f"Expected {w} to be {self.emb_width}"
+        x = x.float().reshape(N * T, w)
+        prenorm = t.norm(x - t.mean(x)) / x.numel() ** 0.5
+        x_l, min_distance = self.quantise(x)
+        fit = t.mean(min_distance)
+        x_d = self.dequantise(x_l)
+        commit_loss = t.norm(x_d - x) ** 2 / x.numel()
+        x_d = x + (x_d - x)          # the reference's straight-through form, same rounding
+        return x_l.view(N, T), x_d.view(N, T, w), commit_loss, dict(fit=fit, pn=prenorm)
 
 
 class Bottleneck(nn.Module):
@@ -65,3 +80,14 @@ class Bottleneck(nn.Module):
         if end_level is None:
             end_level = self.levels
         return [blk.decode(z) for blk, z in zip(self.level_blocks[start_level:end_level], zs)]
+
+    def forward(self, xs):
+        """evaluation mode only (bottleneck.py:200-215 with self.training False): no codebook update and, as in the
+        reference, no per-level metrics"""
+        zs, xs_quantised, commit_losses = [], [], []
+        for blk, x in zip(self.level_blocks, xs):
+            z, x_quantised, commit_loss, _ = blk(x, update_k=self.training)
+            zs.append(z)
+            xs_quantised.append(x_quantised.detach())
+            commit_losses.append(commit_loss)
+        return zs, xs_quantised, commit_losses, []

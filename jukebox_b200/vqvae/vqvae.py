@@ -1,4 +1,4 @@
-"""VQVAE.encode / decode on the GPU (reference: jukebox/vqvae/vqvae.py:44-144).
+"""VQVAE.encode / decode and the evaluation-mode forward on the GPU (reference: jukebox/vqvae/vqvae.py:21-228).
 
 Audio stays [N, T, 1] (the reference permutes to NCT for cuDNN; here every tensor is
 channels-last, which is what the kernels want, so preprocess/postprocess are no-ops)."""
@@ -8,10 +8,31 @@ import torch.nn as nn
 
 from .encdec import Encoder, Decoder
 from .bottleneck import Bottleneck
+from ..utils.audio_utils import (DefaultSTFTValues, audio_postprocess, convergence, multispectral_loss, stft_stats)
 
 
 def calculate_strides(strides, downs):
     return [stride ** down for stride, down in zip(strides, downs)]
+
+
+def _loss_fn(loss_fn, x_target, x_pred, hps):
+    """Reconstruction loss of vqvae.py:21-40, scaled by the dataset's bandwidth: 'l1', 'l2', 'linf' (mean of the
+    hps.linf_k largest squared errors per clip) or 'lmix' (their hps.lmix_* weighted sum, zero weights skipped)."""
+    err = x_pred - x_target
+    if loss_fn == 'l1':
+        return err.abs().mean() / hps.bandwidth['l1']
+    if loss_fn == 'l2':
+        return err.square().mean() / hps.bandwidth['l2']
+    if loss_fn == 'linf':
+        worst = t.topk(err.square().reshape(x_target.shape[0], -1), hps.linf_k, dim=1).values
+        return worst.mean() / hps.bandwidth['l2']
+    if loss_fn == 'lmix':
+        total = 0.0
+        for name, weight in (('l1', hps.lmix_l1), ('l2', hps.lmix_l2), ('linf', hps.lmix_linf)):
+            if weight:
+                total = total + weight * _loss_fn(name, x_target, x_pred, hps)
+        return total
+    raise ValueError(f"Unknown loss_fn {loss_fn}")
 
 
 class VQVAE(nn.Module):
@@ -81,4 +102,64 @@ class VQVAE(nn.Module):
         return self.decode(zs)
 
     def forward(self, x, hps, loss_fn='l1'):
-        raise NotImplementedError("VQ-VAE training (losses, codebook EMA) is out of scope")
+        """Evaluation of a reconstruction (vqvae.py:150-228 in eval mode): x [N, T, 1] -> (level-0 reconstruction,
+        loss, metrics).  Every level encodes, quantises and decodes its own codes; the metrics are the reference's
+        eval-mode keys, each a detached 0-dim tensor.  hps needs the reference's loss settings and `bandwidth`,
+        dict(l1, l2, spec) of the dataset (train.py computes it with calculate_bandwidth)."""
+        if self.training:
+            raise NotImplementedError("VQ-VAE training (codebook EMA, gradients) is out of scope: call .eval() first")
+        try:
+            bandwidth = hps.bandwidth
+        except (AttributeError, KeyError):
+            bandwidth = None
+        if not isinstance(bandwidth, dict) or not {'l1', 'l2', 'spec'} <= set(bandwidth):
+            raise ValueError("hps.bandwidth must be dict(l1, l2, spec), the dataset statistics the losses are scaled by")
+        with t.no_grad():
+            return self._forward(x, hps, loss_fn)
+
+    def _forward(self, x, hps, loss_fn):
+        metrics = {}
+        x_in = self.preprocess(x)
+        xs = [self.encoders[level](x_in)[-1] for level in range(self.levels)]
+        zs, xs_quantised, commit_losses, _ = self.bottleneck(xs)
+        x_outs = []
+        for level in range(self.levels):
+            x_out = self.decoders[level](xs_quantised[level:level + 1], all_levels=False)
+            assert x_out.shape == x_in.shape, (tuple(x_out.shape), tuple(x_in.shape))
+            x_outs.append(x_out)
+
+        recons_loss = t.zeros((), device=x.device)
+        spec_loss = t.zeros((), device=x.device)
+        multispec_loss = t.zeros((), device=x.device)
+        x_target = audio_postprocess(x.float(), hps)
+        for level in reversed(range(self.levels)):
+            x_out = audio_postprocess(self.postprocess(x_outs[level]), hps)
+            this_recons_loss = _loss_fn(loss_fn, x_target, x_out, hps)
+            # the default config's norms; at level 0 they also give the spectral convergence metric below
+            residual_norm, gt_norm = stft_stats(x_target, x_out, DefaultSTFTValues(hps))
+            if hps.use_nonrelative_specloss:
+                this_spec_loss = t.mean(residual_norm / hps.bandwidth['spec'])
+            else:
+                this_spec_loss = t.mean(convergence(residual_norm, gt_norm))
+            this_multispec_loss = t.mean(multispectral_loss(x_target, x_out, hps) / hps.bandwidth['spec'])
+            metrics[f'recons_loss_l{level + 1}'] = this_recons_loss
+            metrics[f'spectral_loss_l{level + 1}'] = this_spec_loss
+            metrics[f'multispectral_loss_l{level + 1}'] = this_multispec_loss
+            recons_loss += this_recons_loss
+            spec_loss += this_spec_loss
+            multispec_loss += this_multispec_loss
+
+        commit_loss = sum(commit_losses)
+        loss = recons_loss + self.spectral * spec_loss + self.multispectral * multispec_loss + self.commit * commit_loss
+
+        # x_out, residual_norm and gt_norm are level 0's, left over from the reversed loop as in the reference
+        sc = t.mean(convergence(residual_norm, gt_norm))
+        l2_loss = _loss_fn("l2", x_target, x_out, hps)
+        l1_loss = _loss_fn("l1", x_target, x_out, hps)
+        linf_loss = _loss_fn("linf", x_target, x_out, hps)
+        metrics.update(dict(recons_loss=recons_loss, spectral_loss=spec_loss, multispectral_loss=multispec_loss,
+                            spectral_convergence=sc, l2_loss=l2_loss, l1_loss=l1_loss, linf_loss=linf_loss,
+                            commit_loss=commit_loss))
+        for key, val in metrics.items():
+            metrics[key] = val.detach()
+        return x_out, loss, metrics
