@@ -293,6 +293,33 @@ size_t  jk_stft_workspace_bytes(int n, int64_t T, int n_fft, int hop);
 int jk_sample_categorical(const float* logits, int64_t logits_stride, int n, int bins, float temp,
                           uint64_t seed, int position, int64_t* tokens, int64_t tok_stride,
                           jk_stream_t stream);
+/* The same draw, scored in the same launch.  logits: what jk_sample_categorical would take (the engine's row, or the
+ * filter_logits output with temp 1); the token drawn is bit-identical to jk_sample_categorical's for the same
+ * arguments.  logits == NULL: nothing is drawn, tokens[r, position] is given.  Either way
+ *   logp[r * logp_stride + position] = log_softmax(raw[r, :])[token]     (fp32)
+ * the log-likelihood at temperature 1 of the raw, unfiltered logits (raw: fp32 rows raw_stride floats apart); nan for a
+ * given token outside [0, bins). */
+int jk_sample_categorical_scored(const float* logits, int64_t logits_stride, const float* raw, int64_t raw_stride,
+                                 int n, int bins, float temp, uint64_t seed, int position, int64_t* tokens,
+                                 int64_t tok_stride, float* logp, int64_t logp_stride, jk_stream_t stream);
+
+/* Log-probabilities of given tokens from the activations, with no logits tensor (csrc/score.cu):
+ *   logp[m] = z[m, targets[m]] - lse[m],  lse[m] = log sum_b exp(z[m, b]),  z = h . x_out^T
+ * h: fp32 [m, width] (x_cond already added when the prior adds it behind the stack), width a multiple of 64; targets:
+ * int64 [m]; logp, and lse unless NULL: fp32 [m].  The product is the fp16 x 3 split (hi.w_hi + hi.w_lo + lo.w_hi,
+ * fp32 accumulation promoted every 64 channels) on the tensor cores, x_out scaled by 2^8 before its split.
+ * jk_pack_xout_split turns x_out fp32 [bins, width] (nn.Linear layout) into the layout the kernel streams,
+ * jk_xout_split_bytes bytes of 16-byte aligned device memory; do it once per weight load.  It returns an error when a
+ * weight lies outside what the scaled split holds (|w| > 255.9, inf, nan).
+ * jk_xout_logprob needs jk_xout_logprob_workspace_bytes of 256-byte aligned device memory and a 16-byte aligned h.  It
+ * synchronises the stream to report its range check: an activation with |h| > 65504 or not finite, or a target outside
+ * [0, bins), is an error (the outputs of the call are then nan, never a wrong number).  A row's result does not depend
+ * on the other rows: it is bitwise the same alone and in any batch. */
+int jk_xout_split_bytes(int bins, int width, size_t* bytes);
+int jk_pack_xout_split(const float* w, void* split, int bins, int width, jk_stream_t stream);
+int jk_xout_logprob_workspace_bytes(int m, int width, int bins, size_t* bytes);
+int jk_xout_logprob(const float* h, int m, int width, const void* w_split, int bins, const int64_t* targets,
+                    float* logp, float* lse, void* workspace, size_t workspace_bytes, jk_stream_t stream);
 
 /* top-k / nucleus filtering in front of the sampler (transformer/ops.py:113-142 `filter_logits`, applied to
  * logits / temp as autoregressive.py:232-234 does): out[r, v] = logits[r, v] / temp if v stays, else -inf.

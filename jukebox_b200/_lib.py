@@ -100,6 +100,11 @@ SIGNATURES = {
     "jk_prior_debug_buffer": (_I, [_P, _I, C.POINTER(_P), C.POINTER(C.c_size_t)]),
     "jk_conv1d_prefill_f16": (_I, [_P, _P, _P, _P, _I, _I, _I, _P]),
     "jk_sample_categorical": (_I, [_P, _L, _I, _I, _F, C.c_uint64, _I, _P, _L, _P]),
+    "jk_sample_categorical_scored": (_I, [_P, _L, _P, _L, _I, _I, _F, C.c_uint64, _I, _P, _L, _P, _L, _P]),
+    "jk_xout_split_bytes": (_I, [_I, _I, C.POINTER(C.c_size_t)]),
+    "jk_pack_xout_split": (_I, [_P, _P, _I, _I, _P]),
+    "jk_xout_logprob_workspace_bytes": (_I, [_I, _I, _I, C.POINTER(C.c_size_t)]),
+    "jk_xout_logprob": (_I, [_P, _I, _I, _P, _I, _P, _P, _P, _P, C.c_size_t, _P]),
     "jk_filter_logits": (_I, [_P, _L, _I, _I, _F, _I, _F, _P, _L, _P]),
     "jk_vq_argmin": (_I, [_P, _P, _P, _P, _L, _I, _I, _P]),
     "jk_vq_gather": (_I, [_P, _P, _P, _L, _I, _I, _P]),

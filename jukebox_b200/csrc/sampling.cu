@@ -27,12 +27,12 @@ __device__ __forceinline__ uint32_t philox_u32(uint64_t seed, uint32_t c0, uint3
     return c[0];
 }
 
-// max_per: bins each thread owns (compile-time bound keeps e[] in registers)
+// The draw of one row (one CTA): tokens[row * tok_stride + position] and, when s_tok is given, *s_tok (visible to the
+// whole CTA after a __syncthreads).  max_per: bins each thread owns (compile-time bound keeps e[] in registers)
 template <int MAX_PER>
-__global__ void __launch_bounds__(kThreads)
-sample_categorical_kernel(const float* __restrict__ logits, long long lstride, int bins, float temp,
-                          unsigned long long seed, int position, long long* __restrict__ tokens,
-                          long long tok_stride) {
+__device__ __forceinline__ void draw_row(const float* __restrict__ logits, long long lstride, int bins, float temp,
+                                         unsigned long long seed, int position, long long* __restrict__ tokens,
+                                         long long tok_stride, int* s_tok) {
     __shared__ float s_red[kThreads / 32];
     __shared__ float s_scan[kThreads / 32];
     __shared__ float s_bcast[2];
@@ -104,6 +104,7 @@ sample_categorical_kernel(const float* __restrict__ logits, long long lstride, i
         }
         if (pick < 0) pick = fallback;
         tokens[(long long)row * tok_stride + position] = pick;
+        if (s_tok) *s_tok = pick;
         s_bcast[1] = 0.f;
     }
     __syncthreads();
@@ -118,7 +119,56 @@ sample_categorical_kernel(const float* __restrict__ logits, long long lstride, i
             if (e[j] > 0.f) lastb = b0 + j;
         if (lastb >= 0) atomicMax(&s_last, lastb);
         __syncthreads();
-        if (last_resort) tokens[(long long)row * tok_stride + position] = s_last < 0 ? 0 : s_last;
+        if (last_resort) {
+            tokens[(long long)row * tok_stride + position] = s_last < 0 ? 0 : s_last;
+            if (s_tok) *s_tok = s_last < 0 ? 0 : s_last;
+        }
+    }
+}
+
+template <int MAX_PER>
+__global__ void __launch_bounds__(kThreads)
+sample_categorical_kernel(const float* __restrict__ logits, long long lstride, int bins, float temp,
+                          unsigned long long seed, int position, long long* __restrict__ tokens,
+                          long long tok_stride) {
+    draw_row<MAX_PER>(logits, lstride, bins, temp, seed, position, tokens, tok_stride, nullptr);
+}
+
+// The same draw (logits != NULL) or the given tokens[row, position] (logits == NULL), then
+// logp[row, position] = log_softmax(raw[row, :])[token]: the likelihood at temperature 1 of the unfiltered logits
+template <int MAX_PER>
+__global__ void __launch_bounds__(kThreads)
+sample_categorical_scored_kernel(const float* __restrict__ logits, long long lstride, const float* __restrict__ raw,
+                                 long long rstride, int bins, float temp, unsigned long long seed, int position,
+                                 long long* __restrict__ tokens, long long tok_stride, float* __restrict__ logp,
+                                 long long logp_stride) {
+    __shared__ int s_tok;
+    __shared__ float s_red[kThreads / 32];
+    const int row = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (logits) draw_row<MAX_PER>(logits, lstride, bins, temp, seed, position, tokens, tok_stride, &s_tok);
+    else if (tid == 0) s_tok = (int)tokens[(long long)row * tok_stride + position];
+    const float* r = raw + (long long)row * rstride;
+    float mx = -INFINITY;
+    for (int b = tid; b < bins; b += kThreads) mx = fmaxf(mx, __ldcg(r + b));
+    mx = jk::warp_max(mx);
+    if (lane == 0) s_red[warp] = mx;
+    __syncthreads();                                   // also publishes s_tok
+    mx = s_red[0];
+#pragma unroll
+    for (int w = 1; w < kThreads / 32; ++w) mx = fmaxf(mx, s_red[w]);
+    float se = 0.f;
+    for (int b = tid; b < bins; b += kThreads) se += expf(__ldcg(r + b) - mx);
+    se = jk::warp_sum(se);
+    __syncthreads();                                   // every thread has read the maxima
+    if (lane == 0) s_red[warp] = se;
+    __syncthreads();
+    if (tid == 0) {
+        float total = 0.f;
+#pragma unroll
+        for (int w = 0; w < kThreads / 32; ++w) total += s_red[w];
+        const int tok = s_tok;               // a given token outside [0, bins) has no likelihood: nan
+        logp[(long long)row * logp_stride + position] =
+            (tok >= 0 && tok < bins) ? __ldcg(r + tok) - mx - logf(total) : __int_as_float(0x7fffffff);
     }
 }
 
@@ -222,6 +272,30 @@ extern "C" int jk_sample_categorical(const float* logits, int64_t logits_stride,
     sample_categorical_kernel<MP><<<n, kThreads, 0, stream>>>(logits, (long long)logits_stride, bins, temp, \
                                                               (unsigned long long)seed, position,  \
                                                               (long long*)tokens, (long long)tok_stride)
+    if (per <= 4) JK_LAUNCH(4);
+    else if (per <= 8) JK_LAUNCH(8);
+    else if (per <= 16) JK_LAUNCH(16);
+    else JK_LAUNCH(32);
+#undef JK_LAUNCH
+    JK_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int jk_sample_categorical_scored(const float* logits, int64_t logits_stride, const float* raw,
+                                            int64_t raw_stride, int n, int bins, float temp, uint64_t seed, int position,
+                                            int64_t* tokens, int64_t tok_stride, float* logp, int64_t logp_stride,
+                                            jk_stream_t stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    JK_REQUIRE(raw && tokens && logp, "null argument");
+    JK_REQUIRE(bins >= 1 && bins <= 32 * kThreads, "bins must be in [1, %d]", 32 * kThreads);
+    JK_REQUIRE(temp > 0.f, "temp must be positive");
+    JK_REQUIRE(position >= 0, "negative position");
+    if (n == 0) return 0;
+    const int per = (bins + kThreads - 1) / kThreads;
+#define JK_LAUNCH(MP)                                                                                                \
+    sample_categorical_scored_kernel<MP><<<n, kThreads, 0, stream>>>(                                                \
+        logits, (long long)logits_stride, raw, (long long)raw_stride, bins, temp, (unsigned long long)seed, position, \
+        (long long*)tokens, (long long)tok_stride, logp, (long long)logp_stride)
     if (per <= 4) JK_LAUNCH(4);
     else if (per <= 8) JK_LAUNCH(8);
     else if (per <= 16) JK_LAUNCH(16);

@@ -1,0 +1,358 @@
+// Log-probabilities of given tokens straight from the activations:
+//
+//   logp[m] = z[m, target[m]] - log sum_b exp(z[m, b]),   z = h . x_out^T  (prior/autoregressive.py: x_out, no bias)
+//
+// without the [M, bins] logits ever reaching HBM.  The product is the split-precision one of conv_wide_kernel
+// (vqvae_t5.cu): hi.w_hi + hi.w_lo + lo.w_hi of fp16 halves (22 significant bits per operand), x_out scaled by 2^8
+// before its split so that the weight remainders stay normal, warpgroup MMAs with fp32 accumulation, and every 64-wide
+// K block's partial promoted into an fp32 register sum with ordinary adds (the tensor core's own accumulation alone
+// drifts to ~2e-5 of the output scale over long K).
+//
+// Work items are (128 rows x 128 bins) tiles, numbered row-tile major so that the CTAs working on the bin tiles of one
+// row tile at the same time share its activation rows in L2.  One persistent CTA per SM, four roles over mbarriers:
+//   warp 12        TMA producer: per K block the fp32 activations [128 x 64] and the hi / lo planes of the weight
+//                  block [128 x 64] (128-byte swizzle) into a 3-stage ring;
+//   warps 8-11     converters: fp32 block -> hi / lo fp16 planes in place; any value the fp16 split cannot hold
+//                  (|h| > 65504, inf, nan) raises the status word instead of saturating;
+//   warps 0-7      consumers, rows 0-63 / 64-127: 12 wgmma m64n128k16 per K block into a zeroed partial, added to the
+//                  tile's fp32 sum.  The epilogue reduces each row of the tile to (max, sum exp(z - max)) over the bins
+//                  it covers - one pair per (row, bin tile) in the workspace - and stores z[m, target] from the one
+//                  tile that holds the target.
+// A second kernel combines the pairs of a row in bin-tile order: the result does not depend on the other rows, the
+// grid or the schedule, so a row gives the same bits alone and in any batch.
+#include "split_tma.cuh"
+#include "../../include/jkb200.h"
+#include <algorithm>
+
+using namespace jk;
+
+namespace {
+
+constexpr int kBM = 128, kBN = 128, kBK = 64, kS = 3, kScoreThreads = 512;
+constexpr float kWScale = 256.f, kWInv = 1.f / 256.f, kF16Max = 65504.f;
+constexpr int kA = kBM * kBK * 4;                 // fp32 activation block; after conversion hi plane | lo plane
+constexpr int kAPlane = kBM * 128;
+constexpr int kB = kBN * 128;                     // one weight plane: 128 bins x 64 fp16
+constexpr int kStage = kA + 2 * kB;
+constexpr int kOffBar = kS * kStage;
+constexpr int kSmem = kOffBar + 128 + 1024;       // barriers, and slack to align the ring to 1024 bytes
+constexpr int kWsHead = 256;                      // workspace: status word, then the pairs, the target logits, a pad
+
+struct ScoreP {
+    const long long* targets;
+    float2* part;                                 // [M][n_bt] (max, sum exp)
+    float* tlogit;                                // [M]
+    unsigned* status;
+    int M, bins, n_kb, n_bt;
+};
+
+// fp32 block [128][64] at st -> hi plane at st, lo plane at st + 16 KB (128 converter threads); false if a value lies
+// outside the fp16 range
+__device__ __forceinline__ bool convert_block(uint8_t* st, int ct) {
+    constexpr int CH = 16, PER = kBM * CH / 128;
+    const float4* f = reinterpret_cast<const float4*>(st);
+    float4 v[PER];
+#pragma unroll
+    for (int j = 0; j < PER; ++j) v[j] = f[ct + j * 128];
+    uint2 h[PER], l[PER];
+    bool ok = true;
+#pragma unroll
+    for (int j = 0; j < PER; ++j) {
+        ok &= fabsf(v[j].x) <= kF16Max && fabsf(v[j].y) <= kF16Max && fabsf(v[j].z) <= kF16Max && fabsf(v[j].w) <= kF16Max;
+        t5_split2(v[j].x, v[j].y, h[j].x, l[j].x);
+        t5_split2(v[j].z, v[j].w, h[j].y, l[j].y);
+    }
+    named_sync(1);
+#pragma unroll
+    for (int j = 0; j < PER; ++j) {
+        const int item = ct + j * 128, r = item / CH, c4 = item % CH;
+        const uint32_t o = sw_off(r, c4 >> 1) + (c4 & 1) * 8;
+        *reinterpret_cast<uint2*>(st + o) = h[j];
+        *reinterpret_cast<uint2*>(st + kAPlane + o) = l[j];
+    }
+    return ok;
+}
+
+__global__ void __launch_bounds__(kScoreThreads, 1)
+xout_logprob_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_w, ScoreP P,
+                    int total_items) {
+    extern __shared__ __align__(1024) uint8_t sm_raw[];
+    uint8_t* sm = sm_raw + ((1024u - (smem_u32(sm_raw) & 1023u)) & 1023u);   // TMA's 128-byte swizzle needs 1024-byte stages
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sm + kOffBar);
+    uint64_t *full = bars, *conv = bars + kS, *empty = bars + 2 * kS;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    if (tid == 0) {
+        for (int i = 0; i < kS; ++i) { mbar_init(&full[i], 1); mbar_init(&conv[i], 128); mbar_init(&empty[i], 2); }
+        mbar_fence_init();
+        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_h)) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_w)) : "memory");
+    }
+    __syncthreads();
+    const int first = blockIdx.x, stride = gridDim.x, bins_pad = P.n_bt * kBN;
+
+    // register reallocation as in conv_wide_kernel: 2 x 128 x 184 + 128 x 104 + 128 x 40 = 65536
+    if (warp >= 12) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (warp == 12 && lane == 0) {
+            uint32_t kt = 0;
+            for (int item = first; item < total_items; item += stride) {
+                const int mt = item / P.n_bt, bt = item - mt * P.n_bt;
+                for (int kb = 0; kb < P.n_kb; ++kb, ++kt) {
+                    const int s = kt % kS;
+                    mbar_wait(&empty[s], ((kt / kS) & 1) ^ 1);
+                    mbar_expect_tx(&full[s], (uint32_t)kStage);
+                    uint8_t* st = sm + s * kStage;
+                    tma_load_2d(st, &map_h, kb * kBK, mt * kBM, &full[s]);          // rows >= M arrive as zeros
+                    tma_load_2d(st + kA, &map_w, kb * kBK, bt * kBN, &full[s]);
+                    tma_load_2d(st + kA + kB, &map_w, kb * kBK, bins_pad + bt * kBN, &full[s]);
+                }
+            }
+        }
+    } else if (warp >= 8) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 104;");
+        const int ct = tid & 127;
+        bool ok = true;
+        uint32_t kt = 0;
+        for (int item = first; item < total_items; item += stride) {
+            for (int kb = 0; kb < P.n_kb; ++kb, ++kt) {
+                const int s = kt % kS;
+                mbar_wait(&full[s], (kt / kS) & 1);
+                ok &= convert_block(sm + s * kStage, ct);
+                fence_async_smem();                   // the planes are read by the tensor core (async proxy)
+                mbar_arrive(&conv[s]);
+            }
+        }
+        if (!ok) atomicOr(P.status, 1u);
+    } else {
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 184;");
+        const int wg = warp >> 2, wt = tid & 127, rq = wg * 64 + (wt >> 5) * 16 + (lane >> 2);
+        const uint32_t ring = smem_u32(sm);
+        uint32_t kt = 0;
+        for (int item = first; item < total_items; item += stride) {
+            const int mt = item / P.n_bt, bt = item - mt * P.n_bt;
+            float acc[kBN / 2];
+#pragma unroll
+            for (int i = 0; i < kBN / 2; ++i) acc[i] = 0.f;
+            for (int kb = 0; kb < P.n_kb; ++kb, ++kt) {
+                const int s = kt % kS;
+                const uint32_t ph = (kt / kS) & 1;
+                mbar_wait(&full[s], ph);              // weight planes (TMA)
+                mbar_wait(&conv[s], ph);              // activation planes (converters)
+                const uint32_t st = ring + s * kStage, ah = st + wg * (64 * 128), al = ah + kAPlane;
+                const uint32_t bh = st + kA, bl = bh + kB;
+                float part[kBN / 2];
+#pragma unroll
+                for (int i = 0; i < kBN / 2; ++i) part[i] = 0.f;
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < kBK / 16; ++k) {
+                    wgmma_ss<kBN>(part, wgmma_desc_sw128(al + k * 32), wgmma_desc_sw128(bh + k * 32));
+                    wgmma_ss<kBN>(part, wgmma_desc_sw128(ah + k * 32), wgmma_desc_sw128(bl + k * 32));
+                    wgmma_ss<kBN>(part, wgmma_desc_sw128(ah + k * 32), wgmma_desc_sw128(bh + k * 32));
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                if (wt == 0) mbar_arrive(&empty[s]);  // the block has retired: free its stage
+#pragma unroll
+                for (int i = 0; i < kBN / 2; ++i) acc[i] += part[i];
+            }
+            // ---- per row: (max, sum exp) over this tile's bins, and the target's logit where it falls here.  The
+            // four lanes of a quad hold the tile's 128 columns of two rows (d[4 i + 2 h + e]: row + 8 h, column
+            // 8 i + 2 (lane % 4) + e); they combine in a fixed shuffle order ----
+            const int c0 = bt * kBN + 2 * (lane & 3);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = mt * kBM + rq + 8 * h;
+                float mx = -INFINITY;
+#pragma unroll
+                for (int i = 0; i < kBN / 8; ++i)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e)
+                        if (c0 + 8 * i + e < P.bins) mx = fmaxf(mx, acc[4 * i + 2 * h + e] * kWInv);
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                const long long tg = r < P.M ? __ldg(P.targets + r) : -1;
+                float se = 0.f;
+#pragma unroll
+                for (int i = 0; i < kBN / 8; ++i)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int col = c0 + 8 * i + e;
+                        if (col < P.bins) {
+                            const float z = acc[4 * i + 2 * h + e] * kWInv;
+                            se += expf(z - mx);
+                            if (col == tg) P.tlogit[r] = z;
+                        }
+                    }
+                se += __shfl_xor_sync(0xffffffffu, se, 1);
+                se += __shfl_xor_sync(0xffffffffu, se, 2);
+                if ((lane & 3) == 0 && r < P.M) P.part[(size_t)r * P.n_bt + bt] = make_float2(mx, se);
+            }
+        }
+    }
+}
+
+// one thread per row: the row's pairs in bin-tile order -> lse, logp.  Status bit 0: an activation outside the fp16
+// split's range (every row is void); bit 1: a target outside [0, bins)
+__global__ void xout_combine_kernel(ScoreP P, float* __restrict__ logp, float* __restrict__ lse) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= P.M) return;
+    const float2* p = P.part + (size_t)r * P.n_bt;
+    float mx = -INFINITY;
+    for (int j = 0; j < P.n_bt; ++j) mx = fmaxf(mx, p[j].x);
+    float se = 0.f;
+    for (int j = 0; j < P.n_bt; ++j) se += p[j].y * expf(p[j].x - mx);
+    const float l = mx + logf(se);
+    const long long tg = P.targets[r];
+    const bool tg_ok = tg >= 0 && tg < P.bins;
+    if (!tg_ok) atomicOr(P.status, 2u);
+    const bool ok = tg_ok && (*reinterpret_cast<volatile unsigned*>(P.status) & 1u) == 0;
+    logp[r] = ok ? P.tlogit[r] - l : __int_as_float(0x7fffffff);
+    if (lse) lse[r] = ok ? l : __int_as_float(0x7fffffff);
+}
+
+// x_out [bins, W] fp32 -> [hi | lo][bins_pad][W] fp16 of 2^8 w (padding rows stay as the caller zeroed them)
+__global__ void pack_xout_split_kernel(const float* __restrict__ w, unsigned short* __restrict__ split, int bins, int bins_pad,
+                                       int W, unsigned* status) {
+    const long long total = (long long)bins * W;
+    bool ok = true;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        unsigned short h, l;
+        const float v = kWScale * __ldg(w + i);
+        ok &= fabsf(v) <= kF16Max;
+        asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(h) : "f"(v));
+        const float rem = v - __half2float(__ushort_as_half(h));
+        asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(l) : "f"(rem));
+        split[i] = h;
+        split[(size_t)bins_pad * W + i] = l;
+    }
+    if (!ok) atomicOr(status, 1u);
+}
+
+int n_bin_tiles(int bins) { return (bins + kBN - 1) / kBN; }
+size_t split_plane_bytes(int bins, int W) { return (size_t)n_bin_tiles(bins) * kBN * W * 2; }
+size_t pad_bytes(int W) { return (size_t)kBM * W * 4; }
+size_t ws_bytes(int M, int W, int bins) {
+    const size_t pairs = ((size_t)M * n_bin_tiles(bins) * 8 + 255) / 256 * 256, tl = ((size_t)M * 4 + 255) / 256 * 256;
+    return kWsHead + pairs + tl + (M < kBM ? pad_bytes(W) : 0);
+}
+
+int read_status(const unsigned* status, unsigned* out, cudaStream_t stream) {
+    JK_CHECK_CUDA(cudaMemcpyAsync(out, status, sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
+    JK_CHECK_CUDA(cudaStreamSynchronize(stream));
+    return 0;
+}
+
+}  // namespace
+
+extern "C" int jk_xout_split_bytes(int bins, int width, size_t* bytes) {
+    JK_REQUIRE(bytes, "null argument");
+    JK_REQUIRE(bins >= 1 && width >= 64 && width % 64 == 0, "need bins >= 1 and width a positive multiple of 64 (got %d, %d)",
+               bins, width);
+    *bytes = 2 * split_plane_bytes(bins, width) + 16;    // + the status word of the range check
+    return 0;
+}
+
+extern "C" int jk_pack_xout_split(const float* w, void* split, int bins, int width, jk_stream_t stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    size_t bytes = 0;
+    if (int rc = jk_xout_split_bytes(bins, width, &bytes)) return rc;
+    JK_REQUIRE(w && split, "null argument");
+    JK_REQUIRE(((uintptr_t)split & 15) == 0, "split must be 16-byte aligned");
+    unsigned* status = reinterpret_cast<unsigned*>(static_cast<char*>(split) + 2 * split_plane_bytes(bins, width));
+    JK_CHECK_CUDA(cudaMemsetAsync(split, 0, bytes, stream));
+    const long long total = (long long)bins * width;
+    const unsigned blocks = (unsigned)std::min<long long>((total + 255) / 256, 65535);
+    pack_xout_split_kernel<<<blocks, 256, 0, stream>>>(w, static_cast<unsigned short*>(split), bins,
+                                                       n_bin_tiles(bins) * kBN, width, status);
+    JK_CHECK_CUDA(cudaGetLastError());
+    unsigned st = 0;
+    if (int rc = read_status(status, &st, stream)) return rc;
+    JK_REQUIRE(st == 0, "x_out weight outside the 2^8-scaled fp16 split (|w| > %g or not finite)", kF16Max / kWScale);
+    return 0;
+}
+
+extern "C" int jk_xout_logprob_workspace_bytes(int m, int width, int bins, size_t* bytes) {
+    JK_REQUIRE(bytes, "null argument");
+    JK_REQUIRE(m >= 0 && bins >= 1 && width >= 64 && width % 64 == 0,
+               "need m >= 0, bins >= 1 and width a positive multiple of 64 (got %d, %d, %d)", m, bins, width);
+    *bytes = ws_bytes(m, width, bins);
+    return 0;
+}
+
+extern "C" int jk_xout_logprob(const float* h, int m, int width, const void* w_split, int bins, const int64_t* targets,
+                               float* logp, float* lse, void* workspace, size_t workspace_bytes, jk_stream_t stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    size_t need = 0;
+    if (int rc = jk_xout_logprob_workspace_bytes(m, width, bins, &need)) return rc;
+    JK_REQUIRE(h && w_split && targets && logp && workspace, "null argument");
+    JK_REQUIRE(workspace_bytes >= need, "workspace of %zu bytes, need %zu", workspace_bytes, need);
+    JK_REQUIRE(((uintptr_t)h & 15) == 0 && ((uintptr_t)w_split & 15) == 0 && ((uintptr_t)workspace & 255) == 0,
+               "h and w_split must be 16-byte aligned, workspace 256-byte aligned");
+    if (m == 0) return 0;
+    const int n_bt = n_bin_tiles(bins), bins_pad = n_bt * kBN;
+    const long long total = (long long)((m + kBM - 1) / kBM) * n_bt;
+    JK_REQUIRE(total < (1ll << 31), "too many rows");
+    char* ws = static_cast<char*>(workspace);
+    ScoreP P;
+    P.status = reinterpret_cast<unsigned*>(ws);
+    P.part = reinterpret_cast<float2*>(ws + kWsHead);
+    P.tlogit = reinterpret_cast<float*>(ws + kWsHead + ((size_t)m * n_bt * 8 + 255) / 256 * 256);
+    P.targets = reinterpret_cast<const long long*>(targets);
+    P.M = m; P.bins = bins; P.n_kb = width / kBK; P.n_bt = n_bt;
+    JK_CHECK_CUDA(cudaMemsetAsync(P.status, 0, sizeof(unsigned), stream));
+    // fewer rows than one tile: the tile is staged from a zero-padded copy, so the tensor map never has a box larger
+    // than the tensor
+    const float* hsrc = h;
+    int rows = m;
+    if (m < kBM) {
+        float* pad = reinterpret_cast<float*>(ws + need - pad_bytes(width));
+        JK_CHECK_CUDA(cudaMemsetAsync(pad, 0, pad_bytes(width), stream));
+        JK_CHECK_CUDA(cudaMemcpyAsync(pad, h, (size_t)m * width * 4, cudaMemcpyDeviceToDevice, stream));
+        hsrc = pad;
+        rows = kBM;
+    }
+    EncodeTiledFnT5 enc = t5_encode();
+    JK_REQUIRE(enc, "cuTensorMapEncodeTiled is not available from the driver");
+    CUtensorMap map_h, map_w;
+    {
+        cuuint64_t dims[2] = {(cuuint64_t)width, (cuuint64_t)rows};
+        cuuint64_t strides[1] = {(cuuint64_t)width * 4};
+        cuuint32_t box[2] = {kBK, kBM};
+        cuuint32_t estr[2] = {1, 1};
+        CUresult r = enc(&map_h, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(hsrc), dims, strides, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        JK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for [%d, %d] fp32 activations", (int)r, m, width);
+    }
+    {
+        cuuint64_t dims[2] = {(cuuint64_t)width, (cuuint64_t)2 * bins_pad};
+        cuuint64_t strides[1] = {(cuuint64_t)width * 2};
+        cuuint32_t box[2] = {kBK, kBN};
+        cuuint32_t estr[2] = {1, 1};
+        CUresult r = enc(&map_w, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(w_split), dims, strides, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        JK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for the [2 x %d, %d] fp16 split x_out", (int)r,
+                   bins_pad, width);
+    }
+    static bool attr_set[64] = {};
+    static int sms[64] = {};
+    int dev = 0;
+    JK_CHECK_CUDA(cudaGetDevice(&dev));
+    if (!attr_set[dev & 63]) {
+        JK_CHECK_CUDA(cudaFuncSetAttribute(xout_logprob_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
+        JK_CHECK_CUDA(cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
+        attr_set[dev & 63] = true;
+    }
+    const unsigned grid = (unsigned)std::min<long long>(total, sms[dev & 63]);
+    xout_logprob_kernel<<<grid, kScoreThreads, kSmem, stream>>>(map_h, map_w, P, (int)total);
+    JK_CHECK_CUDA(cudaGetLastError());
+    xout_combine_kernel<<<(m + 255) / 256, 256, 0, stream>>>(P, logp, lse);
+    JK_CHECK_CUDA(cudaGetLastError());
+    unsigned st = 0;
+    if (int rc = read_status(P.status, &st, stream)) return rc;
+    JK_REQUIRE((st & 1u) == 0, "an activation lies outside the fp16 split's range (|h| > 65504 or not finite)");
+    JK_REQUIRE((st & 2u) == 0, "a target lies outside [0, %d)", bins);
+    return 0;
+}

@@ -20,8 +20,7 @@
 //                              shared-memory stage so that the residual loads and the stores are coalesced.
 // W1 / W2 are scaled by 2^8 before the split (undone in the epilogues) so that their fp16 remainders stay out of the
 // subnormal range; both are split and laid out (N-major rows, K contiguous, same swizzle) once per CTA.
-#include "common.cuh"
-#include <cuda.h>
+#include "split_tma.cuh"
 #include <algorithm>
 
 using namespace jk;
@@ -67,18 +66,6 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
         "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
         : "memory");
 }
-// two values -> packed hi / lo fp16 pairs (a in the low half); values beyond the fp16 range saturate
-__device__ __forceinline__ void t5_split2(float a, float b, uint32_t& hi, uint32_t& lo) {
-    float ha, hb;
-    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(b), "f"(a));
-    asm("{\n\t.reg .f16 l, h;\n\tmov.b32 {l, h}, %2;\n\tcvt.f32.f16 %0, l;\n\tcvt.f32.f16 %1, h;\n\t}" : "=f"(ha), "=f"(hb) : "r"(hi));
-    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(b - hb), "f"(a - ha));
-}
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// byte offset of 16-byte chunk j of row r inside a K-major 128-byte-swizzled plane
-__device__ __forceinline__ uint32_t sw_off(int r, int j) { return (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((j ^ (r & 7)) << 4)); }
-__device__ __forceinline__ void named_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
-
 // scale * (acc / 2^8 + bias) of one consumer warpgroup's 64 rows -> stage[row][C], 16-byte chunks XOR-swizzled with row & 7
 template <int C>
 __device__ __forceinline__ void stage_rows(float* stage, const float (&acc)[C / 2], const float* bias, float scale, int row0, int lane) {
@@ -489,14 +476,6 @@ struct T5W {
     static constexpr int smem = offBar + 128 + 1024;         // barriers, and slack to align the ring to 1024 bytes
 };
 
-__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-            smem_u32(smem_dst)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-        : "memory");
-}
-
 // fp32 block [128][64] at st -> (relu) -> hi plane at st, lo plane at st + 16 KB, by the 128 converter threads: every
 // value is read into registers before the group barrier, so the planes can overwrite the block they come from
 __device__ __forceinline__ void convert_block_inplace(uint8_t* st, int ct, bool relu) {
@@ -652,21 +631,6 @@ __global__ void pack_split_kernel(const float* __restrict__ packed, unsigned sho
         split[o] = h;
         split[(size_t)K * c_out + o] = l;
     }
-}
-
-typedef CUresult (*EncodeTiledFnT5)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFnT5 t5_encode() {
-    static EncodeTiledFnT5 fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFnT5>(p);
-    }
-    return fn;
 }
 
 template <int C>

@@ -13,7 +13,7 @@ import torch as t
 import torch.nn as nn
 import torch.nn.functional as F
 
-from ..transformer.ops import filter_logits_scaled, sample_categorical
+from ..transformer.ops import filter_logits_scaled, sample_categorical, sample_categorical_scored
 from ..transformer.transformer import Transformer
 from ..utils.logger import get_range
 
@@ -123,30 +123,62 @@ class ConditionalAutoregressive2D(nn.Module):
             assert x_cond is None      # zeros in the reference; NULL for the kernel
         return x_cond, y_cond
 
-    def _run(self, n_samples, prime, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds, sample_tokens):
+    def _run(self, n_samples, prime, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds, sample_tokens,
+             get_logprobs=False):
         """shared body of sample / primed_sample.  prime: LongTensor [N, P] of given tokens (P may be 0)."""
         cls = SamplingWindow if fp16 else SamplingWindowF32
         win = cls(self, n_samples, prime, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds,
-                  sample_tokens)
+                  sample_tokens, get_logprobs=get_logprobs)
         win.advance(win.sample_tokens)
         return win.finish()
 
     # ---- reference API -----------------------------------------------------------------------
+    # get_logprobs=True (not in the reference) also returns logprobs, fp32 [N, sample_tokens]: at a drawn position the
+    # log-likelihood of the drawn token under the model (log-softmax at temperature 1 of the unfiltered logits), at a
+    # given position the teacher-forced log-likelihood of the given token within this window.  The result is then
+    # (x, logprobs), or (x, preds, logprobs) with get_preds.  The tokens are those of the same call without it.
     def sample(self, n_samples, x_cond=None, y_cond=None, encoder_kv=None, fp16=False, temp=1.0, top_k=0,
-               top_p=0.0, get_preds=False, sample_tokens=None):
+               top_p=0.0, get_preds=False, sample_tokens=None, get_logprobs=False):
         prime = t.zeros(n_samples, 0, dtype=t.long, device=self.x_emb.weight.device)
         return self._run(n_samples, prime, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds,
-                         sample_tokens)
+                         sample_tokens, get_logprobs)
 
     def primed_sample(self, n_samples, x, x_cond=None, y_cond=None, encoder_kv=None, fp16=False, temp=1.0,
-                      top_k=0, top_p=0.0, get_preds=False, chunk_size=None, sample_tokens=None):
+                      top_k=0, top_p=0.0, get_preds=False, chunk_size=None, sample_tokens=None, get_logprobs=False):
         """`chunk_size` is accepted for compatibility: the prefill runs token by token through the
         same persistent kernel, which is what chunked prefill computes (reference check_chunks)."""
         with t.no_grad():
             x = self.preprocess(x)
         assert x.shape[0] == n_samples
         return self._run(n_samples, x, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds,
-                         sample_tokens)
+                         sample_tokens, get_logprobs)
+
+    def logprob(self, x, x_cond=None, y_cond=None, encoder_kv=None, fp16=True):
+        """log-likelihood in nats of every token of whole sequences x [N, input_dims] given the ones before it, fp32
+        [N, input_dims]: the activations of `forward` (fp16: the decode engine's prefill, or its steps beyond the prefill
+        capacity, in batches the engine takes; fp32: the fp32 path), + cond, then x_out and the log-softmax at the target
+        in one fused kernel (jk_xout_logprob) - no logits tensor."""
+        from ..score import xout_logprob
+        from .._lib import JK_MAX_BATCH
+        assert not self.only_encode
+        with t.no_grad():
+            x = self.preprocess(x)
+            N, D = x.shape
+            assert D == self.input_dims, f"logprob scores whole sequences of {self.input_dims} tokens, got {D}"
+            assert (0 <= x).all() and (x < self.bins).all()
+            x_cond, y_cond = self._check_conds(N, x_cond, y_cond)
+            x = x.contiguous()
+            if fp16:
+                part = lambda v, i: None if v is None else v[i:i + JK_MAX_BATCH]
+                acts = t.cat([self._acts_fp16(x[i:i + JK_MAX_BATCH], part(x_cond, i), part(y_cond, i),
+                                              part(encoder_kv, i)) for i in range(0, N, JK_MAX_BATCH)])
+            else:
+                from ..transformer import f32
+                h = f32.embed(self, x, y_cond, x_cond, N, D, 0)
+                acts = self.transformer(h, encoder_kv=encoder_kv, fp16=False)
+            if self.add_cond_after_transformer and x_cond is not None:
+                acts = acts + x_cond
+            return xout_logprob(acts.reshape(N * D, self.width), self.x_out.weight, x.view(-1)).view(N, D)
 
     def forward(self, x, x_cond=None, y_cond=None, encoder_kv=None, fp16=False, loss_full=False, encode=False,
                 get_preds=False, get_acts=False, get_sep_loss=False):
@@ -232,7 +264,7 @@ class SamplingWindow:
     per position, nothing synchronises with the host.  finish(): cache bookkeeping + postprocess."""
 
     def __init__(self, ca, n_samples, prime, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds,
-                 sample_tokens):
+                 sample_tokens, get_logprobs=False):
         assert ca.training is False
         assert not ca.only_encode
         assert fp16, "SamplingWindowF32 is the fp32 loop"
@@ -261,6 +293,8 @@ class SamplingWindow:
         else:
             self.preds = None
             self.lbuf, self.tstride = t.empty(N, ca.bins, dtype=t.float32, device=dev), 0
+        self.get_logprobs = get_logprobs
+        self.logprobs = t.zeros(N, self.sample_tokens, dtype=t.float32, device=dev) if get_logprobs else None
         self.temp, self.top_k, self.top_p, self.fp16 = temp, top_k, top_p, fp16
         # the key of this call's Philox stream comes from torch's default generator, so t.manual_seed /
         # seed_per_rank make sampling reproducible exactly as they do for the reference's Categorical
@@ -280,14 +314,20 @@ class SamplingWindow:
             if 1 < P <= eng.prefill_capacity:
                 # the given tokens go through all layers at once (the reference's chunked primed_sample,
                 # autoregressive.py:300-338); chunk_size is moot - one chunk.  With get_preds their logits come from
-                # the same pass: x_out over (activations + cond) in fp32 (autoregressive.py:318-325)
-                if get_preds:
+                # the same pass: x_out over (activations + cond) in fp32 (autoregressive.py:318-325).  With get_logprobs
+                # their log-likelihoods come from the same activations through the fused x_out + log-softmax kernel
+                if get_preds or get_logprobs:
                     from ..transformer import f32
                     h = t.empty(N, P, ca.width, dtype=t.float32, device=dev)
                     eng.prefill(N, P, tokens=self.tokens, y_cond=self.y_cond, x_cond=self.x_cond, h_out=h)
                     if ca.add_cond_after_transformer and self.x_cond is not None:
                         h = h + (self.x_cond[:, :P] if self.x_cond.shape[1] > 1 else self.x_cond)
-                    self.preds[:, :P] = f32.linear_nk(h.view(N * P, ca.width), ca.x_out.weight).view(N, P, ca.bins)
+                    if get_preds:
+                        self.preds[:, :P] = f32.linear_nk(h.view(N * P, ca.width), ca.x_out.weight).view(N, P, ca.bins)
+                    if get_logprobs:
+                        from ..score import xout_logprob
+                        self.logprobs[:, :P] = xout_logprob(h.view(N * P, ca.width), ca.x_out.weight,
+                                                            self.tokens[:, :P].reshape(-1)).view(N, P)
                 else:
                     eng.prefill(N, P, tokens=self.tokens, y_cond=self.y_cond, x_cond=self.x_cond)
                 self.pos = P
@@ -298,16 +338,11 @@ class SamplingWindow:
         eng, N, P, tokens = self.eng, self.N, self.P, self.tokens
         with t.no_grad():
             for sample_t in get_range(range(self.pos, upto)):
-                need = self.get_preds or sample_t >= P
+                need = self.get_preds or self.get_logprobs or sample_t >= P
                 eng.step(N, tokens=tokens, y_cond=self.y_cond, x_cond=self.x_cond,
                          logits=self.lbuf if need else None, logits_tstride=self.tstride, logit_bias=self.logit_bias)
-                if sample_t >= P:
-                    x = self.preds[:, sample_t] if self.get_preds else self.lbuf
-                    if self.top_k or self.top_p:   # x / temp -> top-k / nucleus filter (ops.py:113-142): one launch
-                        self.fbuf = filter_logits_scaled(x, self.temp, self.top_k, self.top_p, self.fbuf)
-                        sample_categorical(self.fbuf, 1.0, self.seed, sample_t, tokens)
-                    else:
-                        sample_categorical(x, self.temp, self.seed, sample_t, tokens)
+                x = self.preds[:, sample_t] if self.get_preds else self.lbuf
+                _draw(self, x, sample_t, sample_t >= P)
         self.pos = max(self.pos, upto)
 
     def finish(self):
@@ -319,7 +354,28 @@ class SamplingWindow:
             tr.check_cache(self.N, self.sample_tokens, self.fp16)
             tr.del_cache()
             x = self.ca.postprocess(self.tokens, self.sample_tokens)
-        return (x, self.preds) if self.get_preds else x
+        return _result(self, x)
+
+
+def _draw(win, x, sample_t, drawn):
+    """position sample_t of a window from its logits x [N, bins]: the draw (x / temp -> top-k / nucleus filter, ops.py:
+    113-142, one launch -> Categorical), and with get_logprobs the log-likelihood of the drawn or given token under x,
+    from the same sampling launch"""
+    if not drawn and not win.get_logprobs:
+        return
+    samp, temp = x, win.temp
+    if drawn and (win.top_k or win.top_p):
+        win.fbuf = filter_logits_scaled(x, win.temp, win.top_k, win.top_p, win.fbuf)
+        samp, temp = win.fbuf, 1.0
+    if win.get_logprobs:
+        sample_categorical_scored(samp if drawn else None, x, temp, win.seed, sample_t, win.tokens, win.logprobs)
+    else:
+        sample_categorical(samp, temp, win.seed, sample_t, win.tokens)
+
+
+def _result(win, x):
+    out = (x,) + ((win.preds,) if win.get_preds else ()) + ((win.logprobs,) if win.get_logprobs else ())
+    return out[0] if len(out) == 1 else out
 
 
 class SamplingWindowF32:
@@ -328,7 +384,7 @@ class SamplingWindowF32:
     calls per token instead of one persistent kernel: exactness path, not the hot path (train.py:139 sample logging)."""
 
     def __init__(self, ca, n_samples, prime, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds,
-                 sample_tokens):
+                 sample_tokens, get_logprobs=False):
         assert ca.training is False and not ca.only_encode and not fp16
         self.ca = ca
         self.sample_tokens = ca.input_dims if sample_tokens is None else int(sample_tokens)
@@ -347,6 +403,8 @@ class SamplingWindowF32:
             self.tokens[:, :P] = prime
         self.get_preds = get_preds
         self.preds = t.empty(N, self.sample_tokens, ca.bins, dtype=t.float32, device=dev) if get_preds else None
+        self.get_logprobs = get_logprobs
+        self.logprobs = t.zeros(N, self.sample_tokens, dtype=t.float32, device=dev) if get_logprobs else None
         self.temp, self.top_k, self.top_p = temp, top_k, top_p
         self.seed = int(t.empty((), dtype=t.int64).random_().item())
         self.pos = 0
@@ -363,16 +421,11 @@ class SamplingWindowF32:
                 h = self.tr(h, encoder_kv=self.encoder_kv, sample=True, fp16=False)
                 if ca.add_cond_after_transformer and self.x_cond is not None:
                     h = h + (self.x_cond[:, sample_t:sample_t + 1] if self.x_cond.shape[1] > 1 else self.x_cond)
-                if self.get_preds or sample_t >= P:
+                if self.get_preds or self.get_logprobs or sample_t >= P:
                     x = f32.linear_nk(h.view(N, ca.width), ca.x_out.weight)
                     if self.get_preds:
                         self.preds[:, sample_t] = x
-                if sample_t >= P:
-                    if self.top_k or self.top_p:
-                        self.fbuf = filter_logits_scaled(x, self.temp, self.top_k, self.top_p, self.fbuf)
-                        sample_categorical(self.fbuf, 1.0, self.seed, sample_t, tokens)
-                    else:
-                        sample_categorical(x, self.temp, self.seed, sample_t, tokens)
+                    _draw(self, x, sample_t, sample_t >= P)
         self.pos = max(self.pos, upto)
 
     def finish(self):
@@ -381,4 +434,4 @@ class SamplingWindowF32:
             self.tr.check_cache(self.N, self.sample_tokens, False)
             self.tr.del_cache()
             x = self.ca.postprocess(self.tokens, self.sample_tokens)
-        return (x, self.preds) if self.get_preds else x
+        return _result(self, x)

@@ -227,9 +227,11 @@ class SimplePrior(nn.Module):
 
     # ---- sampling -----------------------------------------------------------------------------------------------
     def sample(self, n_samples, z=None, z_conds=None, y=None, fp16=False, temp=1.0, top_k=0, top_p=0.0,
-               chunk_size=None, sample_tokens=None):
+               chunk_size=None, sample_tokens=None, get_logprobs=False):
         """one window: z = codes of this level already in the window (None / empty: ancestral), z_conds = codes of the
-        level above, y = label rows.  Returns the codes [N, sample_tokens or n_ctx]."""
+        level above, y = label rows.  Returns the codes [N, sample_tokens or n_ctx].  With get_logprobs it returns
+        (codes, logprobs): fp32 [N, sample_tokens or n_ctx], the log-likelihood in nats of each returned code under the
+        model (ConditionalAutoregressive2D.sample), so that the samples of a window can be ranked."""
         for name, v in (("z", z), ("y", y), *((f"z_conds[{i}]", c) for i, c in enumerate(z_conds or []))):
             assert v is None or v.shape[0] == n_samples, f"{name}: expected batch {n_samples}, got {tuple(v.shape)}"
         fresh = z is None or z.shape[1] == 0
@@ -237,6 +239,8 @@ class SimplePrior(nn.Module):
             print(f"{'Ancestral' if fresh else 'Primed'} sampling {n_samples} samples with temp={temp}, "
                   f"top_k={top_k}, top_p={top_p}")
         how = dict(fp16=fp16, temp=temp, top_k=top_k, top_p=top_p)
+        if get_logprobs:
+            how["get_logprobs"] = True
         with t.no_grad():
             x_cond, y_cond, lyric = self.get_cond(z_conds, y)
             if self.single_enc_dec:
@@ -244,7 +248,7 @@ class SimplePrior(nn.Module):
             else:
                 out = self._sample_separate(n_samples, None if fresh else z, lyric, x_cond, y_cond, chunk_size, sample_tokens, how)
         if sample_tokens is None:
-            assert_shape(out, (n_samples, *self.z_shape))
+            assert_shape(out[0] if get_logprobs else out, (n_samples, *self.z_shape))
         return out
 
     def _sample_joint(self, N, z, lyric, x_cond, y_cond, chunk_size, sample_tokens, how):
@@ -253,6 +257,9 @@ class SimplePrior(nn.Module):
         seq, cond = self.spaces.merge(given, [None, x_cond])
         total = None if sample_tokens is None else sample_tokens + self.n_tokens
         seq = self.prior.primed_sample(N, seq, cond, y_cond, chunk_size=chunk_size, sample_tokens=total, **how)
+        if how.get("get_logprobs"):
+            seq, lp = seq
+            return self.spaces.last(seq), lp[:, sum(self.spaces.dims[:-1]):]     # the lyric head stripped as from the codes
         return self.spaces.last(seq)
 
     def _sample_separate(self, N, z, lyric, x_cond, y_cond, chunk_size, sample_tokens, how):
@@ -314,6 +321,33 @@ class SimplePrior(nn.Module):
         if get_preds:
             metrics["preds"] = preds.clone()
         return loss, metrics
+
+    def score(self, z, z_conds=[], y=None, fp16=True):
+        """Per-item bits per token of one full window of codes, conditioned exactly as z_forward conditions it: returns
+        (gen [N], prime [N] or None).  gen is the mean over the window's codes, prime over its lyric tokens (priors with
+        lyrics: the lyric head of a single_enc_dec sequence, split where get_sep_loss splits it, or the lyric encoder's
+        next-token head prime_x_out).  Their item means are z_forward's gen_loss / prime_loss.  fp16 picks the
+        activations as z_forward does (decode engine or fp32 path); x_out and the log-softmax at the target then run in
+        one fused kernel, with no logits tensor, so that many candidates of a window can be ranked cheaply."""
+        from ..score import xout_logprob
+        ln2 = float(np.log(2.))
+        with t.no_grad():
+            x_cond, y_cond, lyric = self.get_cond(z_conds, y)
+            if self.copy_input:
+                lyric = z[:, :self.n_tokens]
+            if self.single_enc_dec:
+                seq, x_cond = self.prior_preprocess([lyric, z], [None, x_cond])
+                bits = -self.prior.logprob(seq, x_cond, y_cond, fp16=fp16) / ln2
+                pl = self.prior.prime_len
+                return bits[:, pl:].mean(1), bits[:, :pl].mean(1)
+            enc = self.get_encoder_kv(lyric, fp16=fp16)
+            gen = -self.prior.logprob(z, x_cond, y_cond, enc, fp16=fp16).mean(1) / ln2
+            prime = None
+            if enc is not None:
+                N, L, W = enc.shape
+                lp = xout_logprob(enc.float().reshape(N * L, W), self.prime_x_out.weight, lyric.reshape(-1))
+                prime = -lp.view(N, L).mean(1) / ln2
+            return gen, prime
 
     def forward(self, x, y=None, fp16=False, decode=False, get_preds=False):
         """audio -> codes of every level -> z_forward at this level (reference prior.py:351-359)"""

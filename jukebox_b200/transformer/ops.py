@@ -108,3 +108,24 @@ def sample_categorical(logits, temp, seed, position, tokens):
     check(lib().jk_sample_categorical(C.c_void_p(logits.data_ptr()), logits.stride(0), logits.shape[0],
                                       logits.shape[1], float(temp), C.c_uint64(seed & (2 ** 64 - 1)), int(position),
                                       C.c_void_p(tokens.data_ptr()), tokens.stride(0), stream_ptr()))
+
+
+def sample_categorical_scored(logits, raw, temp, seed, position, tokens, logp):
+    """sample_categorical(logits, temp, seed, position, tokens) - the same token - and, in the same launch,
+    logp[:, position] = log_softmax(raw)[token] (jk_sample_categorical_scored).  raw: the unfiltered logits the draw
+    came from (temperature 1).  logits=None draws nothing and scores the given tokens[:, position].
+    logits / raw: fp32 CUDA [N, bins] with unit inner stride; tokens int64 [N, L], logp fp32 [N, L]."""
+    from .._lib import lib, check, stream_ptr
+    import ctypes as C
+    for x in (raw, logits):
+        assert x is None or (x.dtype == t.float32 and x.dim() == 2 and x.stride(1) == 1 and x.is_cuda)
+    assert tokens.dtype == t.int64 and tokens.dim() == 2 and tokens.stride(1) == 1
+    assert logp.dtype == t.float32 and logp.dim() == 2 and logp.stride(1) == 1
+    if not tokens.is_cuda or not logp.is_cuda:
+        raise RuntimeError("sample_categorical_scored needs CUDA tensors (no CPU path)")
+    lp = C.c_void_p(0 if logits is None else logits.data_ptr())
+    check(lib().jk_sample_categorical_scored(lp, 0 if logits is None else logits.stride(0), C.c_void_p(raw.data_ptr()),
+                                             raw.stride(0), raw.shape[0], raw.shape[1], float(temp),
+                                             C.c_uint64(seed & (2 ** 64 - 1)), int(position),
+                                             C.c_void_p(tokens.data_ptr()), tokens.stride(0),
+                                             C.c_void_p(logp.data_ptr()), logp.stride(0), stream_ptr()))
