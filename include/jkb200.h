@@ -157,6 +157,23 @@ typedef struct jk_attn_record {
     void* w;
 } jk_attn_record;
 
+/* Activations of one layer returned by a prefill call (the representations of JukeMIR: a prior's intermediate layer,
+ * averaged over time).  After layer `layer`'s MLP residual add, the fp16 residual stream of positions [t0, t1) of every
+ * sample is taken in fp32, plus the call's own x_cond (x_cond_len 1 or n_ctx) when add_x_cond is set:
+ *   pool = 0: out fp32 [n_samples, t1 - t0, width];
+ *   pool = 1: out fp32 [n_samples, width], the mean over those positions.
+ * The mean sums in fp64 in an order that depends on neither the batch nor the device, so a sample's row has the same
+ * bits alone and in any batch; jk_pool_rows_f32 is the same kernel over fp32 rows.  out must be 16-byte aligned.  A layer
+ * out of range (or >= n_layers when truncating), listed twice, an empty or out-of-range [t0, t1), a NULL out or
+ * add_x_cond without x_cond is an error, and nothing is written. */
+typedef struct jk_act_capture {
+    int32_t layer;
+    int32_t t0, t1;
+    int32_t pool;
+    int32_t add_x_cond;
+    float* out;
+} jk_act_capture;
+
 /* Chunked prefill of the given (prime) tokens: positions 0 .. n_positions-1 of every sample through all
  * layers in one call - the chunked half of ConditionalAutoregressive2D.primed_sample
  * (prior/autoregressive.py:251-359), whose own check_chunks asserts it equals stepping token by token.
@@ -176,7 +193,20 @@ typedef struct jk_prefill_args {
     float* h_out;
     const jk_attn_record* record;   /* n_record distinct layers whose weights this call records, or NULL */
     int32_t n_record;
+    /* 0: every layer.  1 <= n_layers < depth: layers 0 .. n_layers-1 only (h_out is then the last of them).  Such a
+     * truncated call leaves the later layers' K/V caches unfilled, so the engine cannot go on: jk_prior_position
+     * reports -1 and jk_prior_step / jk_prior_prefill return an error until jk_prior_reset.  n_layers == depth is a
+     * full call. */
+    int32_t n_layers;
+    const jk_act_capture* capture;           /* n_capture distinct layers whose activations this call returns, or NULL */
+    int32_t n_capture;
 } jk_prefill_args;
+
+/* out[b, :] = mean over t in [t0, t1) of (x[b, t, :] (+ x_cond[b, x_cond_len > 1 ? t : 0, :])), x fp32 [n, P, width],
+ * x_cond fp32 [n, x_cond_len, width] or NULL (x_cond_len 1 or >= t1), out fp32 [n, width], 16-byte aligned: the pooling
+ * of jk_act_capture for rows computed elsewhere (the fp32 path), the same kernel and summation order. */
+int jk_pool_rows_f32(const float* x, int n, int P, int width, int t0, int t1, const float* x_cond, int64_t x_cond_len,
+                     float* out, jk_stream_t stream);
 /* positions one prefill call can take; 0 when the configuration has no tensor-core prefill (a GEMM K that
  * is not a multiple of 64, or encoder-decoder layers): step the given tokens instead */
 int jk_prior_prefill_capacity(const jk_prior* p, int* max_positions);
@@ -188,7 +218,8 @@ int jk_prior_prefill(jk_prior* p, const jk_prefill_args* args, jk_stream_t strea
 
 /* one token position; increments the device-side position counter */
 int jk_prior_step(jk_prior* p, const jk_step_args* a, jk_stream_t stream);
-/* current position (host copy of the device counter as tracked by the calls made so far) */
+/* current position (host copy of the device counter as tracked by the calls made so far); -1 after a truncated prefill
+ * (jk_prefill_args.n_layers), until jk_prior_reset */
 int jk_prior_position(const jk_prior* p, int* t);
 /* profiling buffers of the decode kernel (device ptr and size in halfs; any other `which` is an error):
  * which: 5 = globaltimer stamps (uint64 per phase), 6 = clock64 stamps (int64 [phase][8]), 7 = globaltimer entry / exit

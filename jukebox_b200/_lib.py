@@ -61,11 +61,17 @@ class AttnRecord(C.Structure):
     _fields_ = [("layer", C.c_int32), ("ld", C.c_int32), ("w", C.c_void_p)]
 
 
+class ActCapture(C.Structure):
+    _fields_ = [("layer", C.c_int32), ("t0", C.c_int32), ("t1", C.c_int32), ("pool", C.c_int32),
+                ("add_x_cond", C.c_int32), ("out", C.c_void_p)]
+
+
 class PrefillArgs(C.Structure):
     _fields_ = [("n_samples", C.c_int32), ("n_positions", C.c_int32), ("tokens", C.c_void_p),
                 ("tok_stride", C.c_int64), ("y_cond", C.c_void_p), ("x_cond", C.c_void_p),
                 ("x_cond_len", C.c_int64), ("h_out", C.c_void_p), ("record", C.POINTER(AttnRecord)),
-                ("n_record", C.c_int32)]
+                ("n_record", C.c_int32), ("n_layers", C.c_int32), ("capture", C.POINTER(ActCapture)),
+                ("n_capture", C.c_int32)]
 
 
 class ConvArgs(C.Structure):
@@ -95,6 +101,7 @@ SIGNATURES = {
     "jk_prior_prefill_capacity": (_I, [_P, C.POINTER(C.c_int)]),
     "jk_prior_config_prefill_capacity": (_I, [C.POINTER(PriorConfig), C.POINTER(C.c_int)]),
     "jk_prior_prefill": (_I, [_P, C.POINTER(PrefillArgs), _P]),
+    "jk_pool_rows_f32": (_I, [_P, _I, _I, _I, _I, _I, _P, _L, _P, _P]),
     "jk_prior_position": (_I, [_P, C.POINTER(C.c_int)]),
     "jk_prior_has_logits_gemm": (_I, [_P, C.POINTER(C.c_int)]),
     "jk_prior_debug_buffer": (_I, [_P, _I, C.POINTER(_P), C.POINTER(C.c_size_t)]),

@@ -2192,6 +2192,8 @@ extern "C" int jk_prior_step(jk_prior* p, const jk_step_args* a, jk_stream_t str
     JK_REQUIRE(p && a, "null argument");
     JK_REQUIRE(a->n_samples >= 1 && a->n_samples <= p->cfg.max_batch, "n_samples %d out of range (max_batch %d)",
                a->n_samples, p->cfg.max_batch);
+    JK_REQUIRE(p->t_host >= 0, "the last prefill stopped early (n_layers) and left later layers' caches unfilled: "
+                               "call jk_prior_reset first");
     JK_REQUIRE(p->t_host < p->cfg.n_ctx, "position %d is past the context (n_ctx %d): reset the engine", p->t_host, p->cfg.n_ctx);
     JK_REQUIRE(a->x_in || a->tokens || p->t_host == 0, "tokens required for t > 0");
     JK_REQUIRE(a->x_in || (p->host.pos_emb && p->host.x_emb), "embeddings not set (jk_prior_set_embeddings)");

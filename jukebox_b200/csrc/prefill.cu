@@ -616,7 +616,87 @@ __global__ void rows_to_float_kernel(const __half* __restrict__ x, float* __rest
 
 __global__ void set_position_kernel(int* t, int v) { *t = v; }
 
+// ---- activations of one layer (jk_act_capture, jk_pool_rows_f32): fp32 rows of [t0, t1), or their mean -------------
+// One CTA = one sample x a strip of 64 columns; 256 threads = 32 position slots x 8 threads of 8 columns.  Slot s walks
+// positions t0 + s, t0 + s + 32, ... and sums in fp64; the 32 slot sums of a column are then added in slot order.  That
+// order depends on neither the batch nor the device, so a sample's mean has the same bits alone and in any batch.
+constexpr int kActCols = 64, kActSlots = 32;
+
+__device__ __forceinline__ void load8(const __half* p, float (&v)[8], int) {     // the prefill's rows: width % 8 == 0
+    const uint4 u = *reinterpret_cast<const uint4*>(p);
+    const __half* h = reinterpret_cast<const __half*>(&u);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) v[e] = __half2float(h[e]);
+}
+__device__ __forceinline__ void load8(const float* p, float (&v)[8], int m) {   // any width: m valid columns
+#pragma unroll
+    for (int e = 0; e < 8; ++e) v[e] = e < m ? p[e] : 0.f;
+}
+
+template <typename T, bool POOL>
+__global__ void __launch_bounds__(256) act_rows_kernel(const T* __restrict__ x, int P, int W, int t0, int t1,
+                                                       const float* __restrict__ xc, long long xcl, float* __restrict__ out) {
+    __shared__ double red[kActSlots][kActCols];
+    const int b = blockIdx.y, tid = threadIdx.x, s = tid >> 3, c8 = (tid & 7) * 8;
+    const int c = blockIdx.x * kActCols + c8;
+    const int m = min(8, W - c);                          // columns of this thread (<= 0: none)
+    double acc[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[e] = 0.0;
+    if (m > 0) {
+#pragma unroll 4
+        for (int t = t0 + s; t < t1; t += kActSlots) {
+            float v[8];
+            load8(x + ((size_t)b * P + t) * W + c, v, m);
+            if (xc) {
+                const float* r = xc + ((size_t)b * xcl + (xcl > 1 ? t : 0)) * W + c;
+#pragma unroll
+                for (int e = 0; e < 8; ++e) if (e < m) v[e] += r[e];
+            }
+            if (POOL) {
+#pragma unroll
+                for (int e = 0; e < 8; ++e) acc[e] += (double)v[e];
+            } else {                                      // width % 8 == 0 here (the prefill's rows)
+                float4* o = reinterpret_cast<float4*>(out + ((size_t)b * (t1 - t0) + (t - t0)) * W + c);
+                o[0] = make_float4(v[0], v[1], v[2], v[3]);
+                o[1] = make_float4(v[4], v[5], v[6], v[7]);
+            }
+        }
+    }
+    if (!POOL) return;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) red[s][c8 + e] = acc[e];
+    __syncthreads();
+    const int col = blockIdx.x * kActCols + tid;
+    if (tid < kActCols && col < W) {
+        double sum = 0.0;
+        for (int k = 0; k < kActSlots; ++k) sum += red[k][tid];
+        out[(size_t)b * W + col] = (float)(sum / (double)(t1 - t0));
+    }
+}
+
+template <typename T>
+int launch_act_rows(const T* x, int n, int P, int W, int t0, int t1, const float* xc, long long xcl, int pool, float* out,
+                    cudaStream_t stream) {
+    const dim3 grid((unsigned)((W + kActCols - 1) / kActCols), (unsigned)n);
+    if (pool) act_rows_kernel<T, true><<<grid, 256, 0, stream>>>(x, P, W, t0, t1, xc, xcl, out);
+    else act_rows_kernel<T, false><<<grid, 256, 0, stream>>>(x, P, W, t0, t1, xc, xcl, out);
+    JK_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
 }  // namespace
+
+extern "C" int jk_pool_rows_f32(const float* x, int n, int P, int width, int t0, int t1, const float* x_cond,
+                                int64_t x_cond_len, float* out, jk_stream_t stream) {
+    JK_REQUIRE(x && out, "null argument");
+    JK_REQUIRE(n >= 1 && P >= 1 && width >= 1, "empty rows (n %d, P %d, width %d)", n, P, width);
+    JK_REQUIRE(t0 >= 0 && t0 < t1 && t1 <= P, "positions [%d, %d) empty or outside [0, %d)", t0, t1, P);
+    JK_REQUIRE(!x_cond || x_cond_len == 1 || x_cond_len >= t1, "x_cond_len %lld: 1, or at least t1 = %d rows",
+               (long long)x_cond_len, t1);
+    JK_REQUIRE(((uintptr_t)out & 15) == 0, "out must be 16-byte aligned");
+    return launch_act_rows<float>(x, n, P, width, t0, t1, x_cond, x_cond ? x_cond_len : 1, 1, out, (cudaStream_t)stream);
+}
 
 extern "C" int jk_prior_prefill_capacity(const jk_prior* p, int* max_positions) {
     JK_REQUIRE(p && max_positions, "null argument");
@@ -631,6 +711,8 @@ extern "C" int jk_prior_prefill(jk_prior* p, const jk_prefill_args* a, jk_stream
     const EngineDev& E = p->host;
     JK_REQUIRE(p->pf_len > 0, "this configuration has no chunked prefill (needs width, n_state, mlp_width >= 64 and %% 8 == 0): "
                               "step the given tokens through jk_prior_step");
+    JK_REQUIRE(p->t_host >= 0, "the last prefill stopped early (n_layers) and left later layers' caches unfilled: "
+                               "call jk_prior_reset first");
     JK_REQUIRE(p->t_host == 0, "prefill starts at position 0 (engine is at %d)", p->t_host);
     const int n = a->n_samples, P = a->n_positions;
     JK_REQUIRE(n >= 1 && n <= c.max_batch, "n_samples %d out of range (max_batch %d)", n, c.max_batch);
@@ -640,15 +722,32 @@ extern "C" int jk_prior_prefill(jk_prior* p, const jk_prefill_args* a, jk_stream
     JK_REQUIRE(a->x_cond_len == 0 || a->x_cond_len == 1 || a->x_cond_len == c.n_ctx, "x_cond_len must be 1 or n_ctx");
     const int W = c.width, S = c.n_state, Mw = c.mlp_width, H = c.heads;
     const int rows = n * P;
+    JK_REQUIRE(a->n_layers >= 0 && a->n_layers <= c.depth, "n_layers %d out of range (0 = all, else 1 .. depth %d)",
+               a->n_layers, c.depth);
+    const int depth = a->n_layers ? a->n_layers : c.depth;      // layers this call runs
     JK_REQUIRE(a->n_record >= 0 && (a->n_record == 0 || a->record), "record: %d layers but no table", a->n_record);
     const jk_attn_record* rec[JK_MAX_DEPTH] = {};     // per layer: its entry of a->record, or NULL
     for (int i = 0; i < a->n_record; ++i) {
         const jk_attn_record& r = a->record[i];
-        JK_REQUIRE(r.layer >= 0 && r.layer < c.depth, "record: layer %d out of range (depth %d)", r.layer, c.depth);
+        JK_REQUIRE(r.layer >= 0 && r.layer < depth, "record: layer %d out of range (depth %d)", r.layer, depth);
         JK_REQUIRE(!rec[r.layer], "record: layer %d listed twice", r.layer);
         JK_REQUIRE(r.ld >= 1, "record: layer %d has ld %d (>= 1 keys per row)", r.layer, r.ld);
         JK_REQUIRE(r.w, "record: layer %d has no output buffer", r.layer);
         rec[r.layer] = &r;
+    }
+    JK_REQUIRE(a->n_capture >= 0 && (a->n_capture == 0 || a->capture), "capture: %d layers but no table", a->n_capture);
+    const jk_act_capture* cap[JK_MAX_DEPTH] = {};     // per layer: its entry of a->capture, or NULL
+    for (int i = 0; i < a->n_capture; ++i) {
+        const jk_act_capture& k = a->capture[i];
+        JK_REQUIRE(k.layer >= 0 && k.layer < depth, "capture: layer %d out of range (%d layers run)", k.layer, depth);
+        JK_REQUIRE(!cap[k.layer], "capture: layer %d listed twice", k.layer);
+        JK_REQUIRE(k.t0 >= 0 && k.t0 < k.t1 && k.t1 <= P, "capture: layer %d positions [%d, %d) empty or outside [0, %d)",
+                   k.layer, k.t0, k.t1, P);
+        JK_REQUIRE(k.pool == 0 || k.pool == 1, "capture: layer %d has pool %d (0 or 1)", k.layer, k.pool);
+        JK_REQUIRE(k.out, "capture: layer %d has no output buffer", k.layer);
+        JK_REQUIRE(((uintptr_t)k.out & 15) == 0, "capture: layer %d output is not 16-byte aligned", k.layer);
+        JK_REQUIRE(!k.add_x_cond || a->x_cond, "capture: layer %d adds x_cond, but the call has none", k.layer);
+        cap[k.layer] = &k;
     }
     {
         const size_t cnt = (size_t)rows * W;
@@ -668,7 +767,7 @@ extern "C" int jk_prior_prefill(jk_prior* p, const jk_prefill_args* a, jk_stream
         attr_set[dev & 63] = true;
     }
     JK_REQUIRE(fwd_smem <= 64 * 1024, "prefill attention tile too large");
-    for (int l = 0; l < c.depth; ++l) {
+    for (int l = 0; l < depth; ++l) {
         const LayerDev& LD = E.layer[l];
         ln_rows_kernel<<<ln_grid, 256, 0, stream>>>(p->pf_x, LD.ln0_g, LD.ln0_b, p->pf_xn, rows, W);
         JK_CHECK_CUDA(cudaGetLastError());
@@ -710,11 +809,20 @@ extern "C" int jk_prior_prefill(jk_prior* p, const jk_prefill_args* a, jk_stream
         if (rc) return rc;
         rc = gemm_f16_tc(p->pf_g, p->wt[3][l], LD.b_2, p->pf_x1, p->pf_x, rows, W, Mw, 2, stream);
         if (rc) return rc;
+        if (const jk_act_capture* k = cap[l]) {         // the layer's output, before the next layer overwrites pf_x
+            rc = launch_act_rows<__half>(p->pf_x, n, P, W, k->t0, k->t1, k->add_x_cond ? a->x_cond : nullptr,
+                                         a->x_cond_len ? a->x_cond_len : 1, k->pool, k->out, stream);
+            if (rc) return rc;
+        }
     }
     if (a->h_out) {
         const size_t cnt = (size_t)rows * W;
         rows_to_float_kernel<<<(unsigned)((cnt + 255) / 256), 256, 0, stream>>>(p->pf_x, a->h_out, cnt);
         JK_CHECK_CUDA(cudaGetLastError());
+    }
+    if (depth < c.depth) {      // later layers' caches are not filled: not steppable until jk_prior_reset
+        p->t_host = -1;
+        return 0;
     }
     set_position_kernel<<<1, 1, 0, stream>>>(E.t, P);
     JK_CHECK_CUDA(cudaGetLastError());

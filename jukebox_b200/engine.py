@@ -4,11 +4,17 @@ Owns the arena (one torch uint8 CUDA tensor: packed weight streams, KV caches, a
 and keeps every tensor whose address was handed to the library alive.
 """
 import ctypes as C
+from collections import namedtuple
 
 import torch
 
 from . import _lib
 from ._lib import lib, check, ptr, stream_ptr
+
+
+# one entry of DecodeEngine.prefill(capture=...): out receives the layer's fp32 rows of positions [t0, t1) (pool False:
+# [n, t1 - t0, width]) or their mean (pool True: [n, width]), x_cond added first when add_x_cond (jk_act_capture)
+Capture = namedtuple("Capture", "out t0 t1 pool add_x_cond")
 
 
 def prior_config(*, width, depth, heads, n_state, mlp_width, n_ctx, blocks, attn_funcs, bins=0, prime_len=0,
@@ -147,13 +153,17 @@ class DecodeEngine:
         check(lib().jk_prior_prefill_capacity(self.handle, C.byref(out)))
         return out.value
 
-    def prefill(self, n, n_positions, *, tokens=None, y_cond=None, x_cond=None, h_out=None, record=None):
+    def prefill(self, n, n_positions, *, tokens=None, y_cond=None, x_cond=None, h_out=None, record=None, n_layers=0,
+                capture=None):
         """positions 0..n_positions-1 of all samples through every layer at once (wgmma GEMMs);
         afterwards the engine is at position n_positions.
 
         record: {layer: w} - fp16 CUDA tensors [n, heads, n_positions, ld] that receive the layer's normalised attention
         weights (keys by absolute position, or encoder row for an encoder-decoder layer; keys >= ld are dropped; zeros
-        outside the layer's pattern).  See jk_attn_record in include/jkb200.h."""
+        outside the layer's pattern).  See jk_attn_record in include/jkb200.h.
+        n_layers: 0 runs every layer; 1 <= n_layers < depth stops after layer n_layers - 1, and the engine (position -1)
+        must be reset before it steps or prefills again.
+        capture: {layer: Capture(out, t0, t1, pool, add_x_cond)} - the layer's activations (jk_act_capture)."""
         a = _lib.PrefillArgs()
         a.n_samples, a.n_positions = n, n_positions
         a.tokens = ptr(tokens)
@@ -172,9 +182,24 @@ class DecodeEngine:
                                        f"{'' if w.is_contiguous() else ' (strided)'}")
                 e.layer, e.ld, e.w = int(layer), w.shape[3], ptr(w)
             a.record, a.n_record = table, len(record)
+        if capture:
+            table = (_lib.ActCapture * len(capture))()
+            for e, (layer, k) in zip(table, capture.items()):
+                k = Capture(*k)
+                want = (n, self.cfg.width) if k.pool else (n, k.t1 - k.t0, self.cfg.width)
+                out = k.out
+                if (out.dtype != torch.float32 or tuple(out.shape) != want or out.device != self.device
+                        or not out.is_contiguous()):
+                    raise RuntimeError(f"capture[{layer}]: need a contiguous fp32 tensor {list(want)} on {self.device}, "
+                                       f"got {out.dtype} {tuple(out.shape)} on {out.device}"
+                                       f"{'' if out.is_contiguous() else ' (strided)'}")
+                e.layer, e.t0, e.t1 = int(layer), int(k.t0), int(k.t1)
+                e.pool, e.add_x_cond, e.out = int(bool(k.pool)), int(bool(k.add_x_cond)), ptr(out)
+            a.capture, a.n_capture = table, len(capture)
+        a.n_layers = int(n_layers)
         with torch.cuda.device(self.device):
             check(lib().jk_prior_prefill(self.handle, C.byref(a), stream_ptr()))
-        self.position = n_positions
+        self.position = -1 if 0 < n_layers < self.cfg.depth else n_positions
 
     # ---- one token -----------------------------------------------------------------------
     def step(self, n, *, x_in=None, tokens=None, y_cond=None, x_cond=None, h_out=None, logits=None,

@@ -227,6 +227,83 @@ class ConditionalAutoregressive2D(nn.Module):
             return loss, acts
         return loss, None
 
+    def items_per_prefill(self, N):
+        """items one fp16 prefill of this model takes: up to JK_MAX_BATCH, or half that when only the 16-row engine fits
+        (5b_lyrics); 0 when the configuration has no prefill"""
+        from .._lib import JK_MAX_BATCH
+        tr = self.transformer
+        tr.configure_engine(bins=0 if self.only_encode else self.bins, add_cond_after=self.add_cond_after_transformer)
+        for n in sorted({min(N, JK_MAX_BATCH), min(N, max(1, JK_MAX_BATCH // 2))}, reverse=True):
+            if tr.prefill_capacity(n) > 0:
+                return n
+        return 0
+
+    def layer_acts(self, x, x_cond=None, y_cond=None, encoder_kv=None, layers=(), fp16=True, pool=True, add_cond=True,
+                   t0=0):
+        """Representations (not in the reference; JukeMIR, Castellon et al. 2021): the output of intermediate layers of
+        the stack over the tokens x [N, D] (1 < D <= input_dims; the stack is causal, so a prefix's activations are the
+        full window's).  Returns {layer: fp32 [N, width]} with pool (the mean over positions [t0, D)), else
+        {layer: fp32 [N, D - t0, width]}.  It is what `forward` of an `only_encode` model truncated after that layer
+        returns; with add_cond, x_cond is added as `forward` adds it (add_cond_after_transformer).  x_cond is
+        [N, input_dims or 1, width]: a short window reads its first D rows.
+        fp16: the decode engine's prefill, stopped after the deepest requested layer, with the layers' rows taken (and
+        averaged) inside it (jk_act_capture); items in batches of one engine; a window beyond the prefill capacity is an
+        error.  fp32: the fp32 path up to the deepest layer, averaged by the same kernel (jk_pool_rows_f32)."""
+        from .. import _lib
+        from ..engine import Capture
+        layers = sorted(set(int(l) for l in layers))
+        assert layers and 0 <= layers[0] and layers[-1] < self.depth, f"layers {layers} outside [0, {self.depth})"
+        with t.no_grad():
+            x = self.preprocess(x)
+            N, D = x.shape
+            assert 1 < D <= self.input_dims, f"windows of 2 .. {self.input_dims} tokens, got {D}"
+            assert 0 <= t0 < D, f"t0 {t0} outside [0, {D})"
+            assert (0 <= x).all() and (x < self.bins).all()
+            x_cond, y_cond = self._check_conds(N, x_cond, y_cond)
+            x = x.contiguous()
+            addc = bool(add_cond) and self.add_cond_after_transformer and x_cond is not None
+            dev, W = x.device, self.width
+            if not fp16:
+                from ..transformer import f32
+                h = f32.embed(self, x, y_cond, x_cond, N, D, 0)
+                outs = self.transformer(h, encoder_kv=encoder_kv, fp16=False, layers=layers)
+                res = {}
+                for l, o in outs.items():
+                    if pool:
+                        res[l] = t.empty(N, W, dtype=t.float32, device=dev)
+                        xc = x_cond if addc else None
+                        _lib.check(_lib.lib().jk_pool_rows_f32(
+                            _lib.ptr(o), N, D, W, int(t0), D, _lib.ptr(xc), 0 if xc is None else xc.shape[1],
+                            _lib.ptr(res[l]), _lib.stream_ptr()))
+                    else:
+                        o = o[:, t0:]
+                        if addc:
+                            o = o + (x_cond[:, t0:D] if x_cond.shape[1] > 1 else x_cond)
+                        res[l] = o.contiguous()
+                return res
+            step = self.items_per_prefill(N)
+            cap = self.transformer.prefill_capacity(step) if step else 0
+            if not 1 < D <= cap:
+                raise RuntimeError(f"layer_acts(fp16=True): a window of {D} positions exceeds the prefill capacity "
+                                   f"{cap} of this model; use fp16=False")
+            res = {l: t.empty((N, W) if pool else (N, D - t0, W), dtype=t.float32, device=dev) for l in layers}
+            tr = self.transformer
+            part = lambda v, i: None if v is None else v[i:i + step].contiguous()
+            for i in range(0, N, step):
+                n = min(step, N - i)
+                eng = self._engine(n)
+                tr.del_cache()
+                if any(b.attn_func == 6 for b in tr._attn_mods):
+                    assert encoder_kv is not None
+                    eng.set_encoder_kv(encoder_kv[i:i + n])
+                bufs = {l: t.empty((n, W) if pool else (n, D - t0, W), dtype=t.float32, device=dev) for l in layers}
+                eng.prefill(n, D, tokens=x[i:i + n], y_cond=part(y_cond, i), x_cond=part(x_cond, i),
+                            n_layers=layers[-1] + 1, capture={l: Capture(b, t0, D, pool, addc) for l, b in bufs.items()})
+                tr.del_cache()
+                for l, b in bufs.items():
+                    res[l][i:i + n] = b
+            return res
+
     def _acts_fp16(self, x, x_cond, y_cond, encoder_kv):
         """the causal stack over given tokens on the fp16 decode engine: position by position it computes exactly the
         forward pass (reference check_sample, factored_attention.py:424-455).  The recorded layers' attention weights come

@@ -349,6 +349,23 @@ class SimplePrior(nn.Module):
                 prime = -lp.view(N, L).mean(1) / ln2
             return gen, prime
 
+    def layer_acts(self, z, z_conds=[], y=None, layers=(), fp16=True, pool=True):
+        """Representations of codes z [N, D] (D <= n_ctx) of this level, conditioned exactly as z_forward / score
+        condition them: {layer: fp32 [N, width]} (pool: the mean over the window's codes) or [N, D, width], the outputs
+        of those layers of the stack + x_cond (ConditionalAutoregressive2D.layer_acts).  A single_enc_dec prior takes
+        its lyric head into the causal pass but keeps only the music positions; a separate lyric encoder gives the
+        encoder-decoder layers their keys as in score."""
+        with t.no_grad():
+            x_cond, y_cond, lyric = self.get_cond(z_conds, y)
+            if self.copy_input:
+                lyric = z[:, :self.n_tokens]
+            if self.single_enc_dec:
+                seq, x_cond = self.prior_preprocess([lyric, z], [None, x_cond])
+                return self.prior.layer_acts(seq, x_cond, y_cond, layers=layers, fp16=fp16, pool=pool,
+                                             t0=self.prior.prime_len)
+            enc = self.get_encoder_kv(lyric, fp16=fp16)
+            return self.prior.layer_acts(z, x_cond, y_cond, enc, layers=layers, fp16=fp16, pool=pool)
+
     def forward(self, x, y=None, fp16=False, decode=False, get_preds=False):
         """audio -> codes of every level -> z_forward at this level (reference prior.py:351-359)"""
         z, *z_conds = self.encode(x, bs_chunks=x.shape[0])

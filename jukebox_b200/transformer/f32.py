@@ -56,10 +56,14 @@ class F32Path:
             self.keep.append(d)
         return d.data_ptr()
 
-    def _alloc_caches(self, n):
+    def _alloc_caches(self, n, upto=None):
+        """caches of layers [0, upto) (all when None); later layers get none and must not run"""
         tr = self.tr
         self.caches = []
         for i, blk in enumerate(tr._attn_mods):
+            if upto is not None and i >= upto:
+                self.layers[i].k_cache = self.layers[i].v_cache = 0
+                continue
             rows = tr.encoder_dims if blk.attn_func == 6 else tr.n_ctx
             k = t.zeros(n, rows, self.S, dtype=t.float32, device=self.dev)
             v = t.zeros(n, rows, self.S, dtype=t.float32, device=self.dev)
@@ -72,9 +76,13 @@ class F32Path:
         self.caches = None
         self.cache_n = 0
 
-    def run(self, x, encoder_kv, p0, record=None):
+    def run(self, x, encoder_kv, p0, record=None, first=0, count=None):
         """x: [n, P, width] fp32 CUDA (a new tensor is returned); positions [p0, p0 + P).  `record`: None or a list of
-        layer indices whose attention weights are returned as {layer: [n, heads, P, keys]}."""
+        layer indices whose attention weights are returned as {layer: [n, heads, P, keys]}.  first / count: the layers
+        run, [first, first + count) (default: all); jk_f32_forward reads no absolute layer index, so a stretch of the
+        stack is a pointer into the layer table and a smaller depth."""
+        count = self.depth - first if count is None else count
+        assert 0 <= first and 1 <= count and first + count <= self.depth
         tr = self.tr
         n, P, W = x.shape
         assert W == self.W
@@ -98,7 +106,7 @@ class F32Path:
             self.layers[i].attn_w = ws[i].data_ptr()
         a = _lib.F32Args(n=n, P=P, p0=p0, width=W, n_state=self.S, mlp_width=self.M, heads=tr.n_head, n_ctx=tr.n_ctx,
                          blocks=tr.blocks or 0, prime_len=tr.prime_len or 0, encoder_dims=tr.encoder_dims or 0,
-                         depth=self.depth, x=out.data_ptr(), encoder_kv=_lib.ptr(encoder_kv).value or 0, work=0)
+                         depth=count, x=out.data_ptr(), encoder_kv=_lib.ptr(encoder_kv).value or 0, work=0)
         if not has6:
             a.encoder_dims = 0
         need = C.c_size_t(0)
@@ -106,8 +114,27 @@ class F32Path:
         if self.work is None or self.work.numel() < need.value:
             self.work = t.empty(need.value, dtype=t.float32, device=self.dev)
         a.work = self.work.data_ptr()
-        _lib.check(_lib.lib().jk_f32_forward(C.byref(a), self.layers, _lib.stream_ptr()))
+        table = C.cast(C.addressof(self.layers) + first * C.sizeof(_lib.F32Layer), C.POINTER(_lib.F32Layer))
+        _lib.check(_lib.lib().jk_f32_forward(C.byref(a), table, _lib.stream_ptr()))
         return out, ws
+
+    def run_layers(self, x, encoder_kv, layers):
+        """forward mode over positions [0, P) of x [n, P, width], stopped after the deepest of `layers`: returns
+        {layer: [n, P, width] fp32 output of that layer}.  Each stretch between two of them is one jk_f32_forward call;
+        caches are made for the layers that run only, and dropped afterwards."""
+        layers = sorted(set(int(l) for l in layers))
+        assert layers and 0 <= layers[0] and layers[-1] < self.depth, f"layers {layers} outside [0, {self.depth})"
+        self.reset()
+        self._alloc_caches(x.shape[0], upto=layers[-1] + 1)
+        outs, h, first = {}, x, 0
+        try:
+            for l in layers:
+                h, _ = self.run(h, encoder_kv, 0, first=first, count=l + 1 - first)
+                outs[l] = h
+                first = l + 1
+        finally:
+            self.reset()
+        return outs
 
 
 def embed(ca, tokens, y_cond, x_cond, n, P, p0):

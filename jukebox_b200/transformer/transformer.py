@@ -208,8 +208,15 @@ class Transformer(nn.Module):
         for i in self._record_layers:
             self._attn_mods[i].attn.w = ws[i]
 
-    def forward(self, x, encoder_kv=None, sample=False, fp16=False, fp16_out=False):
+    def forward(self, x, encoder_kv=None, sample=False, fp16=False, fp16_out=False, layers=None):
+        """layers (not in the reference): a collection of layer indices - forward mode stops after the deepest of them
+        and returns {layer: that layer's output [n, P, width]}, computed on the fp32 path (any fp16 flag, as forward mode
+        here always is).  P may be shorter than n_ctx: the stack is causal, so a prefix's outputs are the full window's."""
         assert x.dim() == 3 and x.shape[2] == self.n_in
+        if layers is not None:
+            assert not sample, "layer outputs come from forward mode"
+            outs = self.f32_path().run_layers(x, encoder_kv, layers)
+            return {l: (o.half() if fp16_out else o) for l, o in outs.items()}
         if not sample or not fp16:
             # forward mode over activations (any fp16 flag: computed in fp32, a superset of the reference's fp16
             # precision; the fp16 prefill starts from tokens, ConditionalAutoregressive2D._acts_fp16) and fp32 sampling:
