@@ -266,8 +266,9 @@ typedef struct jk_conv_args {
     float scale;
     int32_t n;                        /* batch */
     int32_t tensor_cores;             /* 0: exact fp32 FMAs in a fixed order (the encoder: its output feeds the bit-exact argmin);
-                                         1: decoder side - c_in, c_out in {32, 64} run on mma.sync with the fp16 x 3 split
-                                         (fp32-level accuracy, free summation order); other shapes ignore the flag */
+                                         1: decoder side - c_in, c_out in {32, 64} run with the fp16 x 3 split (fp32-level
+                                         accuracy, free summation order): on wgmma + TMA for stride-1 inputs of >= 128
+                                         positions and <= 3 taps, on mma.sync otherwise; other shapes ignore the flag */
 } jk_conv_args;
 int jk_conv1d_cl(const jk_conv_args* a, jk_stream_t stream);
 
@@ -278,8 +279,8 @@ int jk_conv1d_cl(const jk_conv_args* a, jk_stream_t stream);
  * jk_pack_conv_weight_split turns a packed fp32 weight [k, c_in, c_out] (jk_pack_conv_weight, or one phase of a
  * transposed conv) into the layout the kernel streams: [hi | lo][c_out][k * c_in] fp16, jk_conv_weight_split_bytes bytes
  * of device memory (16-byte aligned).  Do it once per weight load.
- * jk_conv1d_tc_wide computes exactly what jk_conv1d_cl documents, reading the weight from w_split (a->w is read only
- * when JK_CONV_EXACT is set, which runs the exact FMA kernel instead); a->tensor_cores is ignored.  It takes in_stride 1,
+ * jk_conv1d_tc_wide computes what jk_conv1d_cl documents, reading the weight from w_split; a->w and a->tensor_cores are
+ * not read (the exact route is jk_conv1d_cl with tensor_cores = 0 and the packed weight).  It takes in_stride 1,
  * 1..3 taps, t_in >= 128 and 16-byte aligned in / out / bias / res, and returns an error naming the constraint otherwise:
  * callers keep jk_conv1d_cl for those shapes. */
 int jk_conv_weight_split_bytes(int k, int c_in, int c_out, size_t* bytes);
@@ -295,9 +296,10 @@ int jk_resblock_cl(const float* x, float* out, float* tmp, const float* w1, cons
                    jk_stream_t stream);
 
 /* The same ResConv1DBlock on the tensor cores for the DECODER side (Decoder stacks of vqvae/encdec.py:87-131 and the
- * upsampler Conditioner, prior/conditioners.py:8-48), C == Cs in {32, 64}: 3xTF32 split (hi/lo operands, fp32 accumulate in
- * mma.sync m16n8k8), i.e. fp32 accuracy up to the 2^-22 lo.lo term but NOT the FMA order of jk_resblock_cl.  The encoder,
- * whose output feeds the bit-exact codebook argmin, must keep jk_resblock_cl. */
+ * upsampler Conditioner, prior/conditioners.py:8-48), C == Cs in {32, 64}: fp16 x 3 split (hi / lo fp16 operands, weights
+ * scaled by 2^8 before their split, hi.w_hi + lo.w_hi + hi.w_lo accumulated in fp32), on wgmma + TMA for T >= 128 and
+ * 16-byte aligned x / out, on mma.sync m16n8k16 otherwise; i.e. fp32 accuracy up to the dropped lo.w_lo term but NOT the
+ * FMA order of jk_resblock_cl.  The encoder, whose output feeds the bit-exact codebook argmin, must keep jk_resblock_cl. */
 int jk_resblock_tc(const float* x, float* out, const float* w1, const float* b1, const float* w2, const float* b2,
                    int n, int64_t T, int C, int dilation, float res_scale, jk_stream_t stream);
 

@@ -35,16 +35,6 @@ def _digest():
     return h.hexdigest()
 
 
-def build_variant(out, defines):
-    """A/B builds: the library with extra -D flags, written to `out` (variants/*.so)."""
-    cmd = [_nvcc()] + NVCC_FLAGS + ["-D" + d for d in defines] + [os.path.join(CSRC, s) for s in SOURCES] + ["-o", out]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    if res.returncode != 0:
-        sys.stderr.write(res.stdout + res.stderr)
-        raise RuntimeError("nvcc failed building " + out)
-    return out
-
-
 def build(force=False, verbose=False):
     dig = _digest()
     if not force and os.path.exists(LIB) and os.path.exists(STAMP) and open(STAMP).read().strip() == dig:
@@ -63,8 +53,4 @@ def build(force=False, verbose=False):
 
 
 if __name__ == "__main__":
-    if "--variant" in sys.argv:          # python -m jukebox_b200.build --variant out.so JK_FOO=1 JK_BAR=0
-        i = sys.argv.index("--variant")
-        print(build_variant(sys.argv[i + 1], sys.argv[i + 2:]))
-        sys.exit(0)
     print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))

@@ -1,4 +1,4 @@
-// Shared helpers: error reporting for the C ABI and sm_90a PTX wrappers
+// Shared helpers: error reporting for the C ABI, launch setup, and sm_90a PTX wrappers
 // (mbarrier, TMA bulk copy, ldmatrix, mma.sync, wgmma, cache-hinted loads).
 #pragma once
 #include <cuda_runtime.h>
@@ -27,6 +27,30 @@ void jk_set_error(const char* fmt, ...);
     } while (0)
 
 namespace jk {
+
+// ---- launch setup ---------------------------------------------------------------------
+// Dynamic shared memory above 48 KB must be allowed per kernel, and the attribute belongs to the current device's copy
+// of the kernel: set it on the first launch on each device (64 slots per kernel).
+template <auto Kernel>
+int set_max_smem_once(int bytes) {
+    static bool set[64] = {};
+    int dev = 0;
+    JK_CHECK_CUDA(cudaGetDevice(&dev));
+    if (!set[dev & 63]) {
+        JK_CHECK_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        set[dev & 63] = true;
+    }
+    return 0;
+}
+// SM count of the current device, queried once per device: the grid size of the persistent kernels
+inline int sm_count(int* sms) {
+    static int cached[64] = {};
+    int dev = 0;
+    JK_CHECK_CUDA(cudaGetDevice(&dev));
+    if (!cached[dev & 63]) JK_CHECK_CUDA(cudaDeviceGetAttribute(&cached[dev & 63], cudaDevAttrMultiProcessorCount, dev));
+    *sms = cached[dev & 63];
+    return 0;
+}
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));

@@ -241,13 +241,7 @@ extern "C" int jk_f32_forward(const jk_f32_args* a, const jk_f32_layer* layers, 
     float* enc_tmp = g + (size_t)M * Mw;
     double sc = 1.0 / sqrt(sqrt((double)dh));
     const float scale2 = (float)(sc * sc);
-    static bool attr_set[64] = {};
-    int dev = 0;
-    JK_CHECK_CUDA(cudaGetDevice(&dev));
-    if (!attr_set[dev & 63]) {
-        JK_CHECK_CUDA(cudaFuncSetAttribute(attn_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-        attr_set[dev & 63] = true;
-    }
+    if (int rc = jk::set_max_smem_once<attn_f32_kernel>(96 * 1024)) return rc;
     for (int l = 0; l < a->depth; ++l) {
         const jk_f32_layer& L = layers[l];
         const int af = L.attn_func;

@@ -538,22 +538,13 @@ __global__ void __launch_bounds__(128) attn_record_mma_kernel(AttnFwd A, AttnSeq
 template <int DH, bool W16>
 int launch_attn_mma(const AttnFwd& A, const AttnSeqs& Q, int nseq, int n, __half* w, int ld, cudaStream_t stream) {
     const dim3 grid((unsigned)(nseq * Q.tiles_per_seq), A.H, n);
-    static bool attr_set[2][64] = {};
-    int dev = 0;
-    JK_CHECK_CUDA(cudaGetDevice(&dev));
     if (!w) {
         constexpr size_t smem = (size_t)(kBQ + 2 * kBK) * (DH + 8) * 2;
-        if (!attr_set[0][dev & 63]) {
-            JK_CHECK_CUDA(cudaFuncSetAttribute((attn_fwd_mma_kernel<DH, W16>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            attr_set[0][dev & 63] = true;
-        }
+        if (int rc = set_max_smem_once<attn_fwd_mma_kernel<DH, W16>>((int)smem)) return rc;
         attn_fwd_mma_kernel<DH, W16><<<grid, 128, smem, stream>>>(A, Q);
     } else {
         constexpr size_t smem = (size_t)(kBQ + kBK) * (DH + 8) * 2;
-        if (!attr_set[1][dev & 63]) {
-            JK_CHECK_CUDA(cudaFuncSetAttribute((attn_record_mma_kernel<DH, W16>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            attr_set[1][dev & 63] = true;
-        }
+        if (int rc = set_max_smem_once<attn_record_mma_kernel<DH, W16>>((int)smem)) return rc;
         attn_record_mma_kernel<DH, W16><<<grid, 128, smem, stream>>>(A, Q, w, ld);
     }
     JK_CHECK_CUDA(cudaGetLastError());
@@ -757,15 +748,9 @@ extern "C" int jk_prior_prefill(jk_prior* p, const jk_prefill_args* a, jk_stream
         JK_CHECK_CUDA(cudaGetLastError());
     }
     const unsigned ln_grid = (unsigned)((rows + 7) / 8);
-    static bool attr_set[64] = {};         // per device: the attribute belongs to the device's copy of the function
     const size_t fwd_smem = (size_t)(E.dh + std::max(P, E.enc_dims)) * 4;
-    int dev = 0;
-    JK_CHECK_CUDA(cudaGetDevice(&dev));
-    if (!attr_set[dev & 63]) {
-        JK_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-        JK_CHECK_CUDA(cudaFuncSetAttribute(attn_record_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-        attr_set[dev & 63] = true;
-    }
+    if (int rc = set_max_smem_once<attn_fwd_kernel>(64 * 1024)) return rc;
+    if (int rc = set_max_smem_once<attn_record_kernel>(64 * 1024)) return rc;
     JK_REQUIRE(fwd_smem <= 64 * 1024, "prefill attention tile too large");
     for (int l = 0; l < depth; ++l) {
         const LayerDev& LD = E.layer[l];

@@ -167,13 +167,8 @@ int jk::gemm_f16_tc(const void* x, const void* w_t, const float* bias, const voi
     if (rc) return rc;
     rc = make_map(&mw, w_t, N, K);
     if (rc) return rc;
-    static bool attr_set[64] = {};         // per device: the attribute belongs to the device's copy of the function
-    int dev = 0;
-    JK_CHECK_CUDA(cudaGetDevice(&dev));
-    if (!attr_set[dev & 63]) {
-        JK_CHECK_CUDA(cudaFuncSetAttribute(prefill_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemmSmem));
-        attr_set[dev & 63] = true;
-    }
+    rc = set_max_smem_once<prefill_gemm_kernel>(kGemmSmem);
+    if (rc) return rc;
     dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM);
     prefill_gemm_kernel<<<grid, kGemmThreads, kGemmSmem, stream>>>(mx, mw, bias, (const __half*)res, (__half*)y, M, N, K, epi);
     JK_CHECK_CUDA(cudaGetLastError());

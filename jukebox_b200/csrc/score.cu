@@ -29,7 +29,7 @@ using namespace jk;
 namespace {
 
 constexpr int kBM = 128, kBN = 128, kBK = 64, kS = 3, kScoreThreads = 512;
-constexpr float kWScale = 256.f, kWInv = 1.f / 256.f, kF16Max = 65504.f;
+constexpr float kF16Max = 65504.f;
 constexpr int kA = kBM * kBK * 4;                 // fp32 activation block; after conversion hi plane | lo plane
 constexpr int kAPlane = kBM * 128;
 constexpr int kB = kBN * 128;                     // one weight plane: 128 bins x 64 fp16
@@ -59,8 +59,8 @@ __device__ __forceinline__ bool convert_block(uint8_t* st, int ct) {
 #pragma unroll
     for (int j = 0; j < PER; ++j) {
         ok &= fabsf(v[j].x) <= kF16Max && fabsf(v[j].y) <= kF16Max && fabsf(v[j].z) <= kF16Max && fabsf(v[j].w) <= kF16Max;
-        t5_split2(v[j].x, v[j].y, h[j].x, l[j].x);
-        t5_split2(v[j].z, v[j].w, h[j].y, l[j].y);
+        split_f16x2(v[j].x, v[j].y, h[j].x, l[j].x);
+        split_f16x2(v[j].z, v[j].w, h[j].y, l[j].y);
     }
     named_sync(1);
 #pragma unroll
@@ -217,14 +217,12 @@ __global__ void pack_xout_split_kernel(const float* __restrict__ w, unsigned sho
     const long long total = (long long)bins * W;
     bool ok = true;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        unsigned short h, l;
+        __half h, l;
         const float v = kWScale * __ldg(w + i);
         ok &= fabsf(v) <= kF16Max;
-        asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(h) : "f"(v));
-        const float rem = v - __half2float(__ushort_as_half(h));
-        asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(l) : "f"(rem));
-        split[i] = h;
-        split[(size_t)bins_pad * W + i] = l;
+        split_f16(v, h, l);
+        split[i] = __half_as_ushort(h);
+        split[(size_t)bins_pad * W + i] = __half_as_ushort(l);
     }
     if (!ok) atomicOr(status, 1u);
 }
@@ -336,16 +334,10 @@ extern "C" int jk_xout_logprob(const float* h, int m, int width, const void* w_s
         JK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for the [2 x %d, %d] fp16 split x_out", (int)r,
                    bins_pad, width);
     }
-    static bool attr_set[64] = {};
-    static int sms[64] = {};
-    int dev = 0;
-    JK_CHECK_CUDA(cudaGetDevice(&dev));
-    if (!attr_set[dev & 63]) {
-        JK_CHECK_CUDA(cudaFuncSetAttribute(xout_logprob_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
-        JK_CHECK_CUDA(cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
-        attr_set[dev & 63] = true;
-    }
-    const unsigned grid = (unsigned)std::min<long long>(total, sms[dev & 63]);
+    int sms = 0;
+    if (int rc = set_max_smem_once<xout_logprob_kernel>(kSmem)) return rc;
+    if (int rc = sm_count(&sms)) return rc;
+    const unsigned grid = (unsigned)std::min<long long>(total, sms);
     xout_logprob_kernel<<<grid, kScoreThreads, kSmem, stream>>>(map_h, map_w, P, (int)total);
     JK_CHECK_CUDA(cudaGetLastError());
     xout_combine_kernel<<<(m + 255) / 256, 256, 0, stream>>>(P, logp, lse);

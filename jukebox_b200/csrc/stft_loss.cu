@@ -209,13 +209,7 @@ extern "C" int jk_stft_mag_diff(const float* a, const float* b, const float* win
     const size_t need = jk_stft_workspace_bytes(n, T, n_fft, hop);
     JK_REQUIRE(workspace_bytes >= need, "jk_stft_mag_diff: workspace of %zu bytes, %zu needed", workspace_bytes, need);
 
-    static bool attr_set[64] = {};
-    int dev = 0;
-    JK_CHECK_CUDA(cudaGetDevice(&dev));
-    if (!attr_set[dev & 63]) {
-        JK_CHECK_CUDA(cudaFuncSetAttribute(stft_mag_diff_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
-        attr_set[dev & 63] = true;
-    }
+    if (int rc = jk::set_max_smem_once<stft_mag_diff_kernel>((int)kSmemBytes)) return rc;
     int log_n = 0;
     while ((1 << log_n) < n_fft) ++log_n;
     double* partials = static_cast<double*>(workspace);

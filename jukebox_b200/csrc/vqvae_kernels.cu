@@ -4,8 +4,7 @@
 // encdec.py:6-131 and resnet.py:27-75 (Conv1d / ConvTranspose1d / ResConv1DBlock stacks).
 // The encoder feeds an argmin whose indices must be bit-exact, so these kernels keep true fp32 FMA
 // arithmetic (no TF32): see DESIGN.md "VQ-VAE numerics".
-#include "common.cuh"
-#include <stdlib.h>
+#include "split_tma.cuh"
 #include <algorithm>
 #include "../../include/jkb200.h"
 
@@ -403,7 +402,7 @@ int launch_conv_tile(const ConvP& P, int n, cudaStream_t stream, bool* took) {
     const size_t smem = ((size_t)P.n_taps * P.c_in * CO + (size_t)P.n_taps * TT * (P.c_in + 4)) * sizeof(float);
     *took = false;
     if (smem > 220 * 1024) return 0;
-    JK_CHECK_CUDA(cudaFuncSetAttribute(conv1d_cl_tile_kernel<CO>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+    if (int rc = set_max_smem_once<conv1d_cl_tile_kernel<CO>>(220 * 1024)) return rc;
     dim3 grid((unsigned)((P.t_out + TT - 1) / TT), (unsigned)n);
     conv1d_cl_tile_kernel<CO><<<grid, 256, smem, stream>>>(P);
     JK_CHECK_CUDA(cudaGetLastError());
@@ -416,13 +415,7 @@ int launch_resblock_fused(const float* x, float* out, const float* w1, const flo
                           int n, long long T, int dil, float rs, cudaStream_t stream) {
     constexpr int TX = C / 4, TY = 256 / TX, TT = TY * 8, XS = C + 4;
     constexpr size_t smem = (size_t)(4 * C * C + 4 * TT * XS) * sizeof(float);
-    static bool attr_set[64] = {};         // per device: the attribute belongs to the device's copy of the function
-    int dev = 0;
-    JK_CHECK_CUDA(cudaGetDevice(&dev));
-    if (!attr_set[dev & 63]) {
-        JK_CHECK_CUDA(cudaFuncSetAttribute(resblock_fused_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set[dev & 63] = true;
-    }
+    if (int rc = set_max_smem_once<resblock_fused_kernel<C>>((int)smem)) return rc;
     dim3 grid((unsigned)((T + TT - 1) / TT), (unsigned)n);
     resblock_fused_kernel<C><<<grid, 256, smem, stream>>>(x, out, w1, b1, w2, b2, T, dil, rs);
     JK_CHECK_CUDA(cudaGetLastError());
@@ -431,209 +424,24 @@ int launch_resblock_fused(const float* x, float* out, const float* w1, const flo
 
 // ---------------------------------------------------------------------------------------
 // ResConv1DBlock on the tensor cores, for the DECODER side (Decoder / Conditioner stacks: their outputs are audio and
-// conditioning, never an argmin input, so summation order is free; the encoder keeps the exact-FMA kernel above).
-// fp32 accuracy is kept with the 3xTF32 split: x = hi + lo (both TF32), x.w ~= lo.w_hi + hi.w_lo + hi.w_hi with fp32
-// accumulation in mma.sync.m16n8k8 - only the lo.lo term (2^-22 relative) is dropped.
-//   * persistent CTAs (grid = #SMs): W1 / W2 are split into hi / lo planes in shared memory ONCE per CTA, then the CTA
-//     walks tiles of 64 positions; per tile the three relu'd input tap tiles are staged like in the FMA kernel
-//   * 8 warps = 4 row blocks of 16 positions x 2 halves of the output channels; A fragments come from the tap tiles
-//     (row stride C + 4: the (g, t) lanes of a fragment land in 32 different banks), B fragments from the weight planes
-//     (row stride C + 8: likewise); the hidden tile goes through shared memory between the two convolutions
-// ---------------------------------------------------------------------------------------
-__device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(x));
-    const float r = x - __uint_as_float(hi);
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lo) : "f"(r));
-}
-__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-template <int C>
-struct ResTC {
-    static constexpr int TT = 64, XS = C + 4, WS = C + 8, NT = C / 16;
-    static constexpr size_t smem_floats = (size_t)2 * 3 * C * WS + (size_t)2 * C * WS + (size_t)3 * TT * XS + (size_t)TT * XS;
-};
-
-// one k8 step of a warp tile: A fragment (16 positions x 8 channels) from `arow`, NT n-tiles of 8 output channels
-template <int C>
-__device__ __forceinline__ void tc_kstep(float (&acc)[ResTC<C>::NT][4], const float* arow, const float* wh, const float* wl,
-                                         int g, int t4) {
-    constexpr int XS = ResTC<C>::XS, WS = ResTC<C>::WS, NT = ResTC<C>::NT;
-    uint32_t ah[4], al[4];
-    split_tf32(arow[g * XS + t4], ah[0], al[0]);
-    split_tf32(arow[(g + 8) * XS + t4], ah[1], al[1]);
-    split_tf32(arow[g * XS + t4 + 4], ah[2], al[2]);
-    split_tf32(arow[(g + 8) * XS + t4 + 4], ah[3], al[3]);
-#pragma unroll
-    for (int nt = 0; nt < NT; ++nt) {
-        const int o0 = t4 * WS + nt * 8 + g, o1 = (t4 + 4) * WS + nt * 8 + g;
-        const uint32_t bh0 = __float_as_uint(wh[o0]), bh1 = __float_as_uint(wh[o1]);
-        const uint32_t bl0 = __float_as_uint(wl[o0]), bl1 = __float_as_uint(wl[o1]);
-        mma_tf32(acc[nt], al, bh0, bh1);
-        mma_tf32(acc[nt], ah, bl0, bl1);
-        mma_tf32(acc[nt], ah, bh0, bh1);
-    }
-}
-
-template <int C>
-__global__ void __launch_bounds__(256, 1)
-resblock_tc_kernel(const float* __restrict__ x, float* __restrict__ out, const float* __restrict__ w1,
-                   const float* __restrict__ b1, const float* __restrict__ w2, const float* __restrict__ b2,
-                   long long T, int dil, float rs, long long tiles_per_clip, long long total_tiles) {
-    constexpr int TT = ResTC<C>::TT, XS = ResTC<C>::XS, WS = ResTC<C>::WS, NT = ResTC<C>::NT;
-    extern __shared__ __align__(16) float tsm[];
-    float* w1h = tsm;                       // [3][C][WS]
-    float* w1l = w1h + 3 * C * WS;
-    float* w2h = w1l + 3 * C * WS;          // [C][WS]
-    float* w2l = w2h + C * WS;
-    float* xs = w2l + C * WS;               // [3][TT][XS]  relu(x) at t + (tap - 1) * dil
-    float* hs = xs + 3 * TT * XS;           // [TT][XS]     relu(hidden)
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int g = lane >> 2, t4 = lane & 3;
-    const int m0 = (warp & 3) * 16, n0 = (warp >> 2) * (C / 2);
-    for (int i = tid; i < 3 * C * C; i += 256) {
-        uint32_t hi, lo;
-        split_tf32(__ldg(w1 + i), hi, lo);
-        const int o = (i / C) * WS + i % C;
-        w1h[o] = __uint_as_float(hi); w1l[o] = __uint_as_float(lo);
-    }
-    for (int i = tid; i < C * C; i += 256) {
-        uint32_t hi, lo;
-        split_tf32(__ldg(w2 + i), hi, lo);
-        const int o = (i / C) * WS + i % C;
-        w2h[o] = __uint_as_float(hi); w2l[o] = __uint_as_float(lo);
-    }
-    constexpr int TX = C / 4;
-#pragma unroll 1
-    for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const long long nb = tile / tiles_per_clip, t0 = (tile - nb * tiles_per_clip) * TT;
-        const float* xin = x + (size_t)nb * T * C;
-        float* xout = out + (size_t)nb * T * C;
-        __syncthreads();                    // previous tile's readers of xs / hs are done (and the weights are staged)
-#pragma unroll
-        for (int tap = 0; tap < 3; ++tap) {
-            const long long off = (long long)(tap - 1) * dil;
-#pragma unroll 4
-            for (int i = tid; i < TT * TX; i += 256) {
-                const int tt = i / TX, c4 = i % TX;
-                const long long tp = t0 + tt + off;
-                float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (tp >= 0 && tp < T) v = __ldg(reinterpret_cast<const float4*>(xin + (size_t)tp * C) + c4);
-                v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
-                *reinterpret_cast<float4*>(xs + ((size_t)tap * TT + tt) * XS + c4 * 4) = v;
-            }
-        }
-        __syncthreads();
-        float acc[NT][4];
-#pragma unroll
-        for (int nt = 0; nt < NT; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
-#pragma unroll 1
-        for (int tap = 0; tap < 3; ++tap) {
-#pragma unroll 2
-            for (int k8 = 0; k8 < C / 8; ++k8)
-                tc_kstep<C>(acc, xs + ((size_t)tap * TT + m0) * XS + k8 * 8, w1h + ((size_t)tap * C + k8 * 8) * WS + n0,
-                            w1l + ((size_t)tap * C + k8 * 8) * WS + n0, g, t4);
-        }
-#pragma unroll
-        for (int nt = 0; nt < NT; ++nt) {   // hidden = relu(conv1 + b1) -> shared memory
-            const int col = n0 + nt * 8 + 2 * t4;
-            const float2 bv = __ldg(reinterpret_cast<const float2*>(b1 + col));
-            *reinterpret_cast<float2*>(hs + (size_t)(m0 + g) * XS + col) = make_float2(fmaxf(acc[nt][0] + bv.x, 0.f), fmaxf(acc[nt][1] + bv.y, 0.f));
-            *reinterpret_cast<float2*>(hs + (size_t)(m0 + g + 8) * XS + col) = make_float2(fmaxf(acc[nt][2] + bv.x, 0.f), fmaxf(acc[nt][3] + bv.y, 0.f));
-            acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
-        }
-        __syncthreads();
-#pragma unroll 2
-        for (int k8 = 0; k8 < C / 8; ++k8)
-            tc_kstep<C>(acc, hs + (size_t)m0 * XS + k8 * 8, w2h + (size_t)(k8 * 8) * WS + n0, w2l + (size_t)(k8 * 8) * WS + n0, g, t4);
-#pragma unroll
-        for (int nt = 0; nt < NT; ++nt) {
-            const int col = n0 + nt * 8 + 2 * t4;
-            const float2 bv = __ldg(reinterpret_cast<const float2*>(b2 + col));
-#pragma unroll
-            for (int hlf = 0; hlf < 2; ++hlf) {
-                const long long t = t0 + m0 + g + 8 * hlf;
-                if (t < T) {
-                    const float2 r = __ldg(reinterpret_cast<const float2*>(xin + (size_t)t * C + col));
-                    float2 v;
-                    v.x = rs * (acc[nt][2 * hlf] + bv.x); v.x += r.x;
-                    v.y = rs * (acc[nt][2 * hlf + 1] + bv.y); v.y += r.y;
-                    *reinterpret_cast<float2*>(xout + (size_t)t * C + col) = v;
-                }
-            }
-        }
-    }
-}
-
-template <int C>
-int launch_resblock_tc(const float* x, float* out, const float* w1, const float* b1, const float* w2, const float* b2,
-                       int n, long long T, int dil, float rs, cudaStream_t stream) {
-    constexpr size_t smem = ResTC<C>::smem_floats * sizeof(float);
-    static bool attr_set[64] = {};
-    static int sms[64] = {};
-    int dev = 0;
-    JK_CHECK_CUDA(cudaGetDevice(&dev));
-    if (!attr_set[dev & 63]) {
-        JK_CHECK_CUDA(cudaFuncSetAttribute(resblock_tc_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        JK_CHECK_CUDA(cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
-        attr_set[dev & 63] = true;
-    }
-    const long long per_clip = (T + ResTC<C>::TT - 1) / ResTC<C>::TT, total = per_clip * n;
-    const unsigned grid = (unsigned)std::min<long long>(total, sms[dev & 63]);
-    resblock_tc_kernel<C><<<grid, 256, smem, stream>>>(x, out, w1, b1, w2, b2, T, dil, rs, per_clip, total);
-    JK_CHECK_CUDA(cudaGetLastError());
-    return 0;
-}
-
-// ---------------------------------------------------------------------------------------
-// The same block with the fp16 x 3 split on mma.sync.m16n8k16 (the default decoder-side kernel).
-// x = hi + lo with hi = fp16(x), lo = fp16(x - hi): 22 mantissa bits, the same as the TF32 split (fp16 and TF32 both carry
-// 11 significant bits), products hi.w_hi + lo.w_hi + hi.w_lo accumulated in fp32.  Against 3xTF32: an MMA covers k = 16
-// instead of 8 at the same issue cost, operands are half the shared-memory bytes and arrive as whole fragments through
-// ldmatrix (A: [position][channel] rows, B: [k][n] rows with .trans) - 10 ldmatrix + 24 MMA per k16 step at C = 64 where the
-// TF32 kernel issued 32 LDS + 24 cvt/sub + 24 MMA for the same k range.  Values beyond the fp16 range saturate
-// (cvt.satfinite); VQ-VAE activations are O(1).  Small activations lose nothing that matters: an fp16 remainder below
-// 2^-14 is kept to an ABSOLUTE 2^-25.
+// conditioning, never an argmin input, so summation order is free; the encoder keeps the exact-FMA kernel above).  This
+// kernel takes the shapes resblock_t5_kernel (vqvae_t5.cu) does not: clips under 128 positions, unaligned pointers.
+// The fp16 x 3 split of split_tma.cuh on mma.sync.m16n8k16: x = hi + lo with hi = fp16(x), lo = fp16(x - hi): 22 mantissa
+// bits, the same as a 3xTF32 split (fp16 and TF32 both carry 11 significant bits), products hi.w_hi + lo.w_hi + hi.w_lo
+// accumulated in fp32.  Against 3xTF32 on m16n8k8: an MMA covers k = 16 instead of 8 at the same issue cost, operands are
+// half the shared-memory bytes and arrive as whole fragments through ldmatrix (A: [position][channel] rows, B: [k][n] rows
+// with .trans) - 10 ldmatrix + 24 MMA per k16 step at C = 64 where a TF32 kernel issued 32 LDS + 24 cvt/sub + 24 MMA for
+// the same k range.  Values beyond the fp16 range saturate (cvt.satfinite); VQ-VAE activations are O(1).  Small
+// activations lose nothing that matters: an fp16 remainder below 2^-14 is kept to an ABSOLUTE 2^-25.
 //   * ONE WARP PER 16-POSITION TILE: a warp's output rows need only its own rows of the three tap tiles and of the hidden
 //     tile, so nothing is shared between warps except the weights - no CTA barrier in the tile loop, and the sixteen warps
 //     of a CTA (4 per scheduler) drift apart so that one's global loads overlap another's MMAs
 //   * persistent CTAs (grid = #SMs), W1 / W2 hi + lo planes staged once per CTA
 // ---------------------------------------------------------------------------------------
-__device__ __forceinline__ void split_h2(float x, __half& hi, __half& lo) {
-    unsigned short h, l;
-    asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(h) : "f"(x));
-    hi = __ushort_as_half(h);
-    const float r = x - __half2float(hi);
-    asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(l) : "f"(r));
-    lo = __ushort_as_half(l);
-}
-// two values at once: hi / lo as packed half2 (a in the low half), 6 instructions for the pair
-__device__ __forceinline__ void split_h2x2(float a, float b, uint32_t& hi, uint32_t& lo) {
-    float ha, hb;
-    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(b), "f"(a));
-    asm("{\n\t.reg .f16 l, h;\n\tmov.b32 {l, h}, %2;\n\tcvt.f32.f16 %0, l;\n\tcvt.f32.f16 %1, h;\n\t}" : "=f"(ha), "=f"(hb) : "r"(hi));
-    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(b - hb), "f"(a - ha));
-}
-__device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], const void* p) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"((uint32_t)__cvta_generic_to_shared(p)));
-}
 __device__ __forceinline__ void ldsm_x4_t(uint32_t (&r)[4], const void* p) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
                  : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"((uint32_t)__cvta_generic_to_shared(p)));
 }
-__device__ __forceinline__ void mma_h(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-// weights are split after an exact scaling by 2^8 (undone in the epilogues): a typical |w| ~ 0.05 has its fp16 remainder
-// (~2e-5) in the subnormal range, where the split would keep only ~19 bits
-constexpr float kWScale = 256.f, kWInv = 1.f / 256.f;
 
 template <int C>
 struct ResH2 {
@@ -651,19 +459,19 @@ __device__ __forceinline__ void h2_kstep(float (&acc)[C / 8][4], const __half* a
     constexpr int XS = ResH2<C>::XS;
     const int r = lane & 15, c8 = (lane >> 4) * 8;
     uint32_t fh[4], fl[4];
-    ldsm_x4(fh, ah + r * XS + c8);
-    ldsm_x4(fl, al + r * XS + c8);
+    ldmatrix_x4(fh, ah + r * XS + c8);
+    ldmatrix_x4(fl, al + r * XS + c8);
 #pragma unroll
     for (int np = 0; np < C / 16; ++np) {
         uint32_t wh[4], wl[4];
         ldsm_x4_t(wh, bh + r * XS + np * 16 + c8);
         ldsm_x4_t(wl, bl + r * XS + np * 16 + c8);
-        mma_h(acc[2 * np], fl, wh[0], wh[1]);
-        mma_h(acc[2 * np], fh, wl[0], wl[1]);
-        mma_h(acc[2 * np], fh, wh[0], wh[1]);
-        mma_h(acc[2 * np + 1], fl, wh[2], wh[3]);
-        mma_h(acc[2 * np + 1], fh, wl[2], wl[3]);
-        mma_h(acc[2 * np + 1], fh, wh[2], wh[3]);
+        mma_16816(acc[2 * np], fl, wh[0], wh[1]);
+        mma_16816(acc[2 * np], fh, wl[0], wl[1]);
+        mma_16816(acc[2 * np], fh, wh[0], wh[1]);
+        mma_16816(acc[2 * np + 1], fl, wh[2], wh[3]);
+        mma_16816(acc[2 * np + 1], fh, wl[2], wl[3]);
+        mma_16816(acc[2 * np + 1], fh, wh[2], wh[3]);
     }
 }
 
@@ -686,11 +494,11 @@ resblock_h2_kernel(const float* __restrict__ x, float* __restrict__ out, const f
     const int g = lane >> 2, t4 = lane & 3;
     for (int i = tid; i < 3 * C * C; i += WARPS * 32) {
         const int o = (i / C) * XS + i % C;
-        split_h2(kWScale * __ldg(w1 + i), w1h[o], w1l[o]);
+        split_f16(kWScale * __ldg(w1 + i), w1h[o], w1l[o]);
     }
     for (int i = tid; i < C * C; i += WARPS * 32) {
         const int o = (i / C) * XS + i % C;
-        split_h2(kWScale * __ldg(w2 + i), w2h[o], w2l[o]);
+        split_f16(kWScale * __ldg(w2 + i), w2h[o], w2l[o]);
     }
     __syncthreads();
     constexpr int TX = C / 4, PER = 16 * TX / 32, RJ = 32 / TX;   // float4 loads per lane per tap tile; rows between them
@@ -725,8 +533,8 @@ resblock_h2_kernel(const float* __restrict__ x, float* __restrict__ out, const f
 #pragma unroll
             for (int j = 0; j < PER; ++j) {
                 uint2 h, l;
-                split_h2x2(fmaxf(v[j].x, 0.f), fmaxf(v[j].y, 0.f), h.x, l.x);
-                split_h2x2(fmaxf(v[j].z, 0.f), fmaxf(v[j].w, 0.f), h.y, l.y);
+                split_f16x2(fmaxf(v[j].x, 0.f), fmaxf(v[j].y, 0.f), h.x, l.x);
+                split_f16x2(fmaxf(v[j].z, 0.f), fmaxf(v[j].w, 0.f), h.y, l.y);
                 *reinterpret_cast<uint2*>(xh + (lr + j * RJ) * XS + lc * 4) = h;
                 *reinterpret_cast<uint2*>(xl + (lr + j * RJ) * XS + lc * 4) = l;
             }
@@ -742,10 +550,10 @@ resblock_h2_kernel(const float* __restrict__ x, float* __restrict__ out, const f
             const int col = nt * 8 + 2 * t4;
             const float2 bv = __ldg(reinterpret_cast<const float2*>(b1 + col));
             uint32_t h, l;
-            split_h2x2(fmaxf(fmaf(acc[nt][0], kWInv, bv.x), 0.f), fmaxf(fmaf(acc[nt][1], kWInv, bv.y), 0.f), h, l);
+            split_f16x2(fmaxf(fmaf(acc[nt][0], kWInv, bv.x), 0.f), fmaxf(fmaf(acc[nt][1], kWInv, bv.y), 0.f), h, l);
             *reinterpret_cast<uint32_t*>(xh + g * XS + col) = h;
             *reinterpret_cast<uint32_t*>(xl + g * XS + col) = l;
-            split_h2x2(fmaxf(fmaf(acc[nt][2], kWInv, bv.x), 0.f), fmaxf(fmaf(acc[nt][3], kWInv, bv.y), 0.f), h, l);
+            split_f16x2(fmaxf(fmaf(acc[nt][2], kWInv, bv.x), 0.f), fmaxf(fmaf(acc[nt][3], kWInv, bv.y), 0.f), h, l);
             *reinterpret_cast<uint32_t*>(xh + (g + 8) * XS + col) = h;
             *reinterpret_cast<uint32_t*>(xl + (g + 8) * XS + col) = l;
             acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
@@ -777,18 +585,12 @@ template <int C>
 int launch_resblock_h2(const float* x, float* out, const float* w1, const float* b1, const float* w2, const float* b2,
                        int n, long long T, int dil, float rs, cudaStream_t stream) {
     constexpr size_t smem = ResH2<C>::smem;
-    static bool attr_set[64] = {};
-    static int sms[64] = {};
-    int dev = 0;
-    JK_CHECK_CUDA(cudaGetDevice(&dev));
-    if (!attr_set[dev & 63]) {
-        JK_CHECK_CUDA(cudaFuncSetAttribute(resblock_h2_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        JK_CHECK_CUDA(cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
-        attr_set[dev & 63] = true;
-    }
+    int sms = 0;
+    if (int rc = set_max_smem_once<resblock_h2_kernel<C>>((int)smem)) return rc;
+    if (int rc = sm_count(&sms)) return rc;
     const long long per_clip = (T + 15) / 16, total = per_clip * n;
     constexpr int WARPS = ResH2<C>::WARPS;
-    const unsigned grid = (unsigned)std::min<long long>((total + WARPS - 1) / WARPS, sms[dev & 63]);
+    const unsigned grid = (unsigned)std::min<long long>((total + WARPS - 1) / WARPS, sms);
     resblock_h2_kernel<C><<<grid, WARPS * 32, smem, stream>>>(x, out, w1, b1, w2, b2, T, dil, rs, per_clip, total);
     JK_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -821,7 +623,7 @@ __global__ void __launch_bounds__(512, 1) conv1d_h2_kernel(ConvP P, long long ti
     const int g = lane >> 2, t4 = lane & 3;
     for (int i = tid; i < ntap * CI * CO; i += WARPS * 32) {
         const int o = (i / CO) * XB + i % CO;
-        split_h2(kWScale * __ldg(P.w + i), wh[o], wl[o]);
+        split_f16(kWScale * __ldg(P.w + i), wh[o], wl[o]);
     }
     __syncthreads();
     constexpr int TX = CI / 4, PER = 16 * TX / 32, RJ = 32 / TX;
@@ -858,8 +660,8 @@ __global__ void __launch_bounds__(512, 1) conv1d_h2_kernel(ConvP P, long long ti
             for (int j = 0; j < PER; ++j) {
                 if (P.relu_in) { v[j].x = fmaxf(v[j].x, 0.f); v[j].y = fmaxf(v[j].y, 0.f); v[j].z = fmaxf(v[j].z, 0.f); v[j].w = fmaxf(v[j].w, 0.f); }
                 uint2 h, l;
-                split_h2x2(v[j].x, v[j].y, h.x, l.x);
-                split_h2x2(v[j].z, v[j].w, h.y, l.y);
+                split_f16x2(v[j].x, v[j].y, h.x, l.x);
+                split_f16x2(v[j].z, v[j].w, h.y, l.y);
                 *reinterpret_cast<uint2*>(xh + (lr + j * RJ) * XA + lc * 4) = h;
                 *reinterpret_cast<uint2*>(xl + (lr + j * RJ) * XA + lc * 4) = l;
             }
@@ -868,8 +670,8 @@ __global__ void __launch_bounds__(512, 1) conv1d_h2_kernel(ConvP P, long long ti
 #pragma unroll
             for (int k16 = 0; k16 < CI / 16; ++k16) {
                 uint32_t fh[4], fl[4];
-                ldsm_x4(fh, xh + r * XA + k16 * 16 + c8);
-                ldsm_x4(fl, xl + r * XA + k16 * 16 + c8);
+                ldmatrix_x4(fh, xh + r * XA + k16 * 16 + c8);
+                ldmatrix_x4(fl, xl + r * XA + k16 * 16 + c8);
                 const __half* bh = wh + (tap * CI + k16 * 16 + r) * XB + c8;
                 const __half* bl = wl + (tap * CI + k16 * 16 + r) * XB + c8;
 #pragma unroll
@@ -877,12 +679,12 @@ __global__ void __launch_bounds__(512, 1) conv1d_h2_kernel(ConvP P, long long ti
                     uint32_t qh[4], ql[4];
                     ldsm_x4_t(qh, bh + np * 16);
                     ldsm_x4_t(ql, bl + np * 16);
-                    mma_h(acc[2 * np], fl, qh[0], qh[1]);
-                    mma_h(acc[2 * np], fh, ql[0], ql[1]);
-                    mma_h(acc[2 * np], fh, qh[0], qh[1]);
-                    mma_h(acc[2 * np + 1], fl, qh[2], qh[3]);
-                    mma_h(acc[2 * np + 1], fh, ql[2], ql[3]);
-                    mma_h(acc[2 * np + 1], fh, qh[2], qh[3]);
+                    mma_16816(acc[2 * np], fl, qh[0], qh[1]);
+                    mma_16816(acc[2 * np], fh, ql[0], ql[1]);
+                    mma_16816(acc[2 * np], fh, qh[0], qh[1]);
+                    mma_16816(acc[2 * np + 1], fl, qh[2], qh[3]);
+                    mma_16816(acc[2 * np + 1], fh, ql[2], ql[3]);
+                    mma_16816(acc[2 * np + 1], fh, qh[2], qh[3]);
                 }
             }
         }
@@ -915,18 +717,12 @@ __global__ void __launch_bounds__(512, 1) conv1d_h2_kernel(ConvP P, long long ti
 template <int CI, int CO>
 int launch_conv_h2(const ConvP& P, int n, cudaStream_t stream) {
     constexpr size_t smem = ConvH2<CI, CO>::smem;
-    static bool attr_set[64] = {};
-    static int sms[64] = {};
-    int dev = 0;
-    JK_CHECK_CUDA(cudaGetDevice(&dev));
-    if (!attr_set[dev & 63]) {
-        JK_CHECK_CUDA(cudaFuncSetAttribute(conv1d_h2_kernel<CI, CO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        JK_CHECK_CUDA(cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
-        attr_set[dev & 63] = true;
-    }
+    int sms = 0;
+    if (int rc = set_max_smem_once<conv1d_h2_kernel<CI, CO>>((int)smem)) return rc;
+    if (int rc = sm_count(&sms)) return rc;
     const long long per_clip = (P.t_out + 15) / 16, total = per_clip * n;
     constexpr int WARPS = ConvH2<CI, CO>::WARPS;
-    const unsigned grid = (unsigned)std::min<long long>((total + WARPS - 1) / WARPS, sms[dev & 63]);
+    const unsigned grid = (unsigned)std::min<long long>((total + WARPS - 1) / WARPS, sms);
     conv1d_h2_kernel<CI, CO><<<grid, WARPS * 32, smem, stream>>>(P, per_clip, total);
     JK_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -1130,23 +926,15 @@ extern "C" int jk_conv1d_cl(const jk_conv_args* a, jk_stream_t stream_) {
         const int span = (a->in_stride == 1 && hi - lo <= 16) ? hi - lo : -1;        // one staging window covers every tap
         const size_t nsm = (((size_t)a->n_taps * a->c_in * a->c_out + 3) & ~(size_t)3) * 4 +
                            (size_t)(256 + std::max(span, 0)) * (a->c_in + 4) * 4;
-        static bool narrow_attr[64] = {};
-        int dev = 0;
-        JK_CHECK_CUDA(cudaGetDevice(&dev));
-        if (!narrow_attr[dev & 63]) {
-            JK_CHECK_CUDA(cudaFuncSetAttribute(conv1d_cl_narrow_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-            narrow_attr[dev & 63] = true;
-        }
+        if (int rc = set_max_smem_once<conv1d_cl_narrow_kernel>(200 * 1024)) return rc;
         conv1d_cl_narrow_kernel<<<g, 256, nsm, stream>>>(P, span, lo);
         JK_CHECK_CUDA(cudaGetLastError());
         return 0;
     }
-    static const bool conv_exact = getenv("JK_CONV_EXACT") != nullptr;      // A/B: keep the FMA tile kernel for flagged convs
-    if (a->tensor_cores && !conv_exact && (a->c_in == 32 || a->c_in == 64) && (a->c_out == 32 || a->c_out == 64) &&
+    if (a->tensor_cores && (a->c_in == 32 || a->c_in == 64) && (a->c_out == 32 || a->c_out == 64) &&
         (((uintptr_t)a->in | (uintptr_t)a->out | (uintptr_t)a->bias | (uintptr_t)a->res) & 15) == 0) {
-        // wgmma + TMA tap-GEMM (vqvae_t5.cu) for stride-1 inputs of >= 128 positions; JK_CONV_T5=0 keeps the mma.sync kernel
-        static const bool t5 = !(getenv("JK_CONV_T5") && atoi(getenv("JK_CONV_T5")) == 0);
-        if (t5 && a->in_stride == 1 && a->n_taps <= 3 && a->t_in >= 128 && a->t_out >= 1)
+        // wgmma + TMA tap-GEMM (vqvae_t5.cu) for stride-1 inputs of >= 128 positions, the mma.sync kernel for the rest
+        if (a->in_stride == 1 && a->n_taps <= 3 && a->t_in >= 128 && a->t_out >= 1)
             return jk::conv_t5(a->in, a->t_in, a->c_in, a->out, a->t_out, a->c_out, a->w, a->bias, a->res, a->n_taps, a->tap_off,
                                a->out_stride, a->out_offset, a->relu_in, a->scale, a->n, stream);
         if (a->c_in == 64 && a->c_out == 64) return launch_conv_h2<64, 64>(P, a->n, stream);
@@ -1155,8 +943,7 @@ extern "C" int jk_conv1d_cl(const jk_conv_args* a, jk_stream_t stream_) {
         return launch_conv_h2<32, 32>(P, a->n, stream);
     }
     if ((a->c_out == 64 || a->c_out == 32) && a->c_in % 4 == 0 && a->c_in >= 4 && a->c_in <= 64 &&
-        (((uintptr_t)a->in | (uintptr_t)a->out | (uintptr_t)a->w | (uintptr_t)a->bias | (uintptr_t)a->res) & 15) == 0 &&
-        !getenv("JK_NO_TILE_CONV")) {
+        (((uintptr_t)a->in | (uintptr_t)a->out | (uintptr_t)a->w | (uintptr_t)a->bias | (uintptr_t)a->res) & 15) == 0) {
         bool took = false;
         const int rc = a->c_out == 64 ? launch_conv_tile<64>(P, a->n, stream, &took) : launch_conv_tile<32>(P, a->n, stream, &took);
         if (rc) return rc;
@@ -1172,7 +959,7 @@ extern "C" int jk_resblock_cl(const float* x, float* out, float* tmp, const floa
                               const float* b2, int n, int64_t T, int C, int Cs, int dilation, float res_scale,
                               jk_stream_t stream) {
     JK_REQUIRE(x && out && w1 && w2, "null argument");
-    if (C == Cs && b1 && b2 && x != out && T > 0 && !getenv("JK_NO_FUSED_RESBLOCK")) {   // the VQ-VAE's own shapes: one fused launch
+    if (C == Cs && b1 && b2 && x != out && T > 0) {   // the VQ-VAE's own shapes: one fused launch
         if (C == 64) return launch_resblock_fused<64>(x, out, w1, b1, w2, b2, n, T, dilation, res_scale, (cudaStream_t)stream);
         if (C == 32) return launch_resblock_fused<32>(x, out, w1, b1, w2, b2, n, T, dilation, res_scale, (cudaStream_t)stream);
     }
@@ -1194,15 +981,8 @@ extern "C" int jk_resblock_tc(const float* x, float* out, const float* w1, const
                               int n, int64_t T, int C, int dilation, float res_scale, jk_stream_t stream) {
     JK_REQUIRE(x && out && w1 && w2 && b1 && b2, "null argument");
     JK_REQUIRE(x != out && T > 0 && n > 0, "x and out must differ, T and n must be positive");
-    static const bool tf32 = getenv("JK_RESBLOCK_TF32") != nullptr;      // the round-2 3xTF32 kernel, kept for A/B runs
-    if (tf32) {
-        if (C == 64) return launch_resblock_tc<64>(x, out, w1, b1, w2, b2, n, T, dilation, res_scale, (cudaStream_t)stream);
-        if (C == 32) return launch_resblock_tc<32>(x, out, w1, b1, w2, b2, n, T, dilation, res_scale, (cudaStream_t)stream);
-    }
-    // wgmma + TMA version (vqvae_t5.cu): whole 128-position MMA tiles, TMA needs 16-byte aligned rows.  JK_RESBLOCK_T5=0
-    // keeps the mma.sync kernel (A/B runs).
-    static const bool t5 = !(getenv("JK_RESBLOCK_T5") && atoi(getenv("JK_RESBLOCK_T5")) == 0);
-    if (t5 && (C == 64 || C == 32) && T >= 128 && (((uintptr_t)x | (uintptr_t)out) & 15) == 0)
+    // wgmma + TMA version (vqvae_t5.cu): whole 128-position MMA tiles, TMA needs 16-byte aligned rows
+    if ((C == 64 || C == 32) && T >= 128 && (((uintptr_t)x | (uintptr_t)out) & 15) == 0)
         return jk::resblock_t5(x, out, w1, b1, w2, b2, n, T, C, dilation, res_scale, (cudaStream_t)stream);
     if (C == 64) return launch_resblock_h2<64>(x, out, w1, b1, w2, b2, n, T, dilation, res_scale, (cudaStream_t)stream);
     if (C == 32) return launch_resblock_h2<32>(x, out, w1, b1, w2, b2, n, T, dilation, res_scale, (cudaStream_t)stream);
@@ -1235,13 +1015,6 @@ extern "C" int jk_pack_conv_weight_split(const float* packed, void* split, int k
 
 extern "C" int jk_conv1d_tc_wide(const jk_conv_args* a, const void* w_split, jk_stream_t stream) {
     JK_REQUIRE(a && a->in && a->out && w_split, "null argument");
-    static const bool conv_exact = getenv("JK_CONV_EXACT") != nullptr;      // A/B: the exact FMA kernel, as for narrow convs
-    if (conv_exact) {
-        JK_REQUIRE(a->w, "jk_conv1d_tc_wide: JK_CONV_EXACT needs the packed fp32 weight in w");
-        jk_conv_args e = *a;
-        e.tensor_cores = 0;
-        return jk_conv1d_cl(&e, stream);
-    }
     JK_REQUIRE(a->c_in % 64 == 0 && a->c_out % 64 == 0 && a->c_in > 0 && a->c_out > 0 && (a->c_in > 64 || a->c_out > 64),
                "jk_conv1d_tc_wide: c_in and c_out must be multiples of 64 and one of them above 64 (got %d -> %d)", a->c_in, a->c_out);
     JK_REQUIRE(a->in_stride == 1, "jk_conv1d_tc_wide: the input stride must be 1 (got %d)", a->in_stride);

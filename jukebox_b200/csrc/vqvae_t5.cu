@@ -27,24 +27,13 @@ using namespace jk;
 
 namespace {
 
-#ifndef JK_T5_PREFETCH
-#define JK_T5_PREFETCH 1
-#endif
 constexpr int kBM = 128;                  // positions per tile = two wgmma M blocks of 64
-// converter groups of 4 warps (group g converts the taps whose counter is g mod 2): two for C = 32, one for C = 64
-// (C = 64 has no shared memory left for a deeper fp32 ring); JK_T5_CONV_GROUPS overrides both
-template <int C>
-struct T5Groups {
-#ifdef JK_T5_CONV_GROUPS
-    static constexpr int value = JK_T5_CONV_GROUPS;
-#else
-    static constexpr int value = C == 64 ? 1 : 2;
-#endif
-};
-constexpr float kWScaleT5 = 256.f, kWInvT5 = 1.f / 256.f;
 
 template <int C>
 struct T5 {
+    // converter groups of 4 warps (group g converts the taps whose counter is g mod 2): two for C = 32, one for C = 64
+    // (C = 64 has no shared memory left for a deeper fp32 ring); + 8 consumer warps and the producer warp
+    static constexpr int kGroups = C == 64 ? 1 : 2, kThreads = 32 * (9 + 4 * kGroups);
     static constexpr int kWBlock = C * 128;                 // one K block of a weight plane: C rows x 128 bytes
     static constexpr int kW1 = 3 * kWBlock, kW2 = kWBlock;   // bytes per plane
     static constexpr int kATile = kBM * 128;                 // one operand plane of a tap tile (128-byte rows)
@@ -73,8 +62,8 @@ __device__ __forceinline__ void stage_rows(float* stage, const float (&acc)[C / 
     for (int j = 0; j < C / 4; ++j) {                     // j = 2 i + h: columns 8 i + 2 (lane % 4) + {0, 1}, row + 8 h
         const int row = row0 + 8 * (j & 1), col = 8 * (j >> 1) + 2 * (lane & 3);
         float2 o;
-        o.x = scale * fmaf(acc[2 * j], kWInvT5, bias[col]);
-        o.y = scale * fmaf(acc[2 * j + 1], kWInvT5, bias[col + 1]);
+        o.x = scale * fmaf(acc[2 * j], kWInv, bias[col]);
+        o.y = scale * fmaf(acc[2 * j + 1], kWInv, bias[col + 1]);
         *reinterpret_cast<float2*>(stage + row * C + (((col >> 2) ^ (row & 7)) << 2) + (col & 3)) = o;
     }
 }
@@ -91,8 +80,8 @@ __device__ __forceinline__ void convert_tap(const uint8_t* fsrc, uint8_t* ah, in
 #pragma unroll
     for (int j = 0; j < PER; ++j) {
         if (relu) { v[j].x = fmaxf(v[j].x, 0.f); v[j].y = fmaxf(v[j].y, 0.f); v[j].z = fmaxf(v[j].z, 0.f); v[j].w = fmaxf(v[j].w, 0.f); }
-        t5_split2(v[j].x, v[j].y, h[j].x, l[j].x);
-        t5_split2(v[j].z, v[j].w, h[j].y, l[j].y);
+        split_f16x2(v[j].x, v[j].y, h[j].x, l[j].x);
+        split_f16x2(v[j].z, v[j].w, h[j].y, l[j].y);
     }
 #pragma unroll
     for (int j = 0; j < PER; ++j) {
@@ -117,12 +106,12 @@ __device__ __forceinline__ void mma_tap(float (&acc)[CO / 2], uint32_t ah, uint3
 }
 
 template <int C>
-__global__ void __launch_bounds__(32 * (9 + 4 * T5Groups<C>::value), 1)
+__global__ void __launch_bounds__(T5<C>::kThreads, 1)
 resblock_t5_kernel(const __grid_constant__ CUtensorMap map_x, const float* __restrict__ x, float* __restrict__ out,
                    const float* __restrict__ w1, const float* __restrict__ b1, const float* __restrict__ w2,
                    const float* __restrict__ b2, long long T, int dil, float rs, int tiles_per_clip, int total_tiles) {
     using L = T5<C>;
-    constexpr int kGroups = T5Groups<C>::value, kThreadsT5 = 32 * (9 + 4 * kGroups), kProducer = 8 + 4 * kGroups;
+    constexpr int kGroups = L::kGroups, kThreadsT5 = L::kThreads, kProducer = 8 + 4 * kGroups;
     extern __shared__ __align__(1024) uint8_t sm[];
     uint64_t* bars = reinterpret_cast<uint64_t*>(sm + L::offBar);
     uint64_t *f_full = bars, *f_empty = bars + 4, *a_full = bars + 8, *a_empty = bars + 10;
@@ -139,25 +128,19 @@ resblock_t5_kernel(const __grid_constant__ CUtensorMap map_x, const float* __res
     }
     for (int i = tid; i < 3 * C * C; i += kThreadsT5) {        // w1[(tap * C + ci) * C + co] -> B1[tap block][row co][k ci]
         const int tap = i / (C * C), ci = (i / C) % C, co = i % C;
-        unsigned short h, l;
-        const float v = kWScaleT5 * __ldg(w1 + i);
-        asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(h) : "f"(v));
-        const float rem = v - __half2float(__ushort_as_half(h));
-        asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(l) : "f"(rem));
+        __half h, l;
+        split_f16(kWScale * __ldg(w1 + i), h, l);
         const uint32_t o = tap * L::kWBlock + sw_off(co, ci >> 3) + (ci & 7) * 2;
-        *reinterpret_cast<unsigned short*>(sm + L::offW1h + o) = h;
-        *reinterpret_cast<unsigned short*>(sm + L::offW1l + o) = l;
+        *reinterpret_cast<__half*>(sm + L::offW1h + o) = h;
+        *reinterpret_cast<__half*>(sm + L::offW1l + o) = l;
     }
     for (int i = tid; i < C * C; i += kThreadsT5) {            // w2[ci * C + co] -> B2[row co][k ci]
         const int ci = i / C, co = i % C;
-        unsigned short h, l;
-        const float v = kWScaleT5 * __ldg(w2 + i);
-        asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(h) : "f"(v));
-        const float rem = v - __half2float(__ushort_as_half(h));
-        asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(l) : "f"(rem));
+        __half h, l;
+        split_f16(kWScale * __ldg(w2 + i), h, l);
         const uint32_t o = sw_off(co, ci >> 3) + (ci & 7) * 2;
-        *reinterpret_cast<unsigned short*>(sm + L::offW2h + o) = h;
-        *reinterpret_cast<unsigned short*>(sm + L::offW2l + o) = l;
+        *reinterpret_cast<__half*>(sm + L::offW2h + o) = h;
+        *reinterpret_cast<__half*>(sm + L::offW2l + o) = l;
     }
     for (int i = tid; i < 2 * C; i += kThreadsT5) bias[i] = i < C ? __ldg(b1 + i) : __ldg(b2 + i - C);
     fence_async_smem();                                       // the weight planes are read by the tensor core (async proxy)
@@ -177,15 +160,11 @@ resblock_t5_kernel(const __grid_constant__ CUtensorMap map_x, const float* __res
                     asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];" ::"l"(
                                      reinterpret_cast<uint64_t>(&map_x)), "r"(0), "r"(t0 + (tap - 1) * dil), "r"(nb) : "memory");
             };
-#if JK_T5_PREFETCH
             prefetch(first + stride);
-#endif
             uint32_t kt = 0;
             for (int tile = first; tile < total_tiles; tile += stride) {
                 const int nb = tile / tiles_per_clip, t0 = (tile - nb * tiles_per_clip) * kBM;
-#if JK_T5_PREFETCH
                 prefetch(tile + 2 * stride);
-#endif
                 for (int tap = 0; tap < 3; ++tap, ++kt) {
                     const int s = kt % FS;
                     mbar_wait(&f_empty[s], ((kt / FS) & 1) ^ 1);
@@ -246,9 +225,9 @@ resblock_t5_kernel(const __grid_constant__ CUtensorMap map_x, const float* __res
 #pragma unroll
             for (int j = 0; j < C / 4; ++j) {                 // j = 2 i + h: register 2 (i & 1) + h of k-step i / 2
                 const int col = 8 * (j >> 1) + 2 * (lane & 3);
-                const float a0 = fmaxf(fmaf(acc[2 * j], kWInvT5, bias[col]), 0.f);
-                const float a1 = fmaxf(fmaf(acc[2 * j + 1], kWInvT5, bias[col + 1]), 0.f);
-                t5_split2(a0, a1, hh[j >> 2][j & 3], hl[j >> 2][j & 3]);
+                const float a0 = fmaxf(fmaf(acc[2 * j], kWInv, bias[col]), 0.f);
+                const float a1 = fmaxf(fmaf(acc[2 * j + 1], kWInv, bias[col + 1]), 0.f);
+                split_f16x2(a0, a1, hh[j >> 2][j & 3], hl[j >> 2][j & 3]);
             }
             // this thread's share of the residual rows of its warpgroup (coalesced), requested while the k1 conv runs
             const float* xin = x + ((size_t)nb * T + t0) * C;
@@ -343,14 +322,11 @@ conv_t5_kernel(const __grid_constant__ CUtensorMap map_x, ConvT5P P, int tiles_p
     }
     for (int i = tid; i < ntap * CI * CO; i += kConvThreads) {  // w[(tap * CI + ci) * CO + co] -> B[tap][row co][k ci]
         const int tap = i / (CI * CO), ci = (i / CO) % CI, co = i % CO;
-        unsigned short h, l;
-        const float v = kWScaleT5 * __ldg(P.w + i);
-        asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(h) : "f"(v));
-        const float rem = v - __half2float(__ushort_as_half(h));
-        asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(l) : "f"(rem));
+        __half h, l;
+        split_f16(kWScale * __ldg(P.w + i), h, l);
         const uint32_t o = tap * L::kWBlock + sw_off(co, ci >> 3) + (ci & 7) * 2;
-        *reinterpret_cast<unsigned short*>(sm + L::offWh + o) = h;
-        *reinterpret_cast<unsigned short*>(sm + L::offWl + o) = l;
+        *reinterpret_cast<__half*>(sm + L::offWh + o) = h;
+        *reinterpret_cast<__half*>(sm + L::offWl + o) = l;
     }
     for (int i = tid; i < CO; i += kConvThreads) bias[i] = P.bias ? __ldg(P.bias + i) : 0.f;
     fence_async_smem();
@@ -488,8 +464,8 @@ __device__ __forceinline__ void convert_block_inplace(uint8_t* st, int ct, bool 
 #pragma unroll
     for (int j = 0; j < PER; ++j) {
         if (relu) { v[j].x = fmaxf(v[j].x, 0.f); v[j].y = fmaxf(v[j].y, 0.f); v[j].z = fmaxf(v[j].z, 0.f); v[j].w = fmaxf(v[j].w, 0.f); }
-        t5_split2(v[j].x, v[j].y, h[j].x, l[j].x);
-        t5_split2(v[j].z, v[j].w, h[j].y, l[j].y);
+        split_f16x2(v[j].x, v[j].y, h[j].x, l[j].x);
+        split_f16x2(v[j].z, v[j].w, h[j].y, l[j].y);
     }
     named_sync(1);
 #pragma unroll
@@ -603,8 +579,8 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
                         const int col = 8 * i + 2 * (lane & 3);
                         const float2 b = bb ? __ldg(reinterpret_cast<const float2*>(bb + col)) : make_float2(0.f, 0.f);
                         float2 o;
-                        o.x = P.scale * fmaf(acc[4 * i + 2 * h], kWInvT5, b.x);
-                        o.y = P.scale * fmaf(acc[4 * i + 2 * h + 1], kWInvT5, b.y);
+                        o.x = P.scale * fmaf(acc[4 * i + 2 * h], kWInv, b.x);
+                        o.y = P.scale * fmaf(acc[4 * i + 2 * h + 1], kWInv, b.y);
                         if (rb) {
                             const float2 r = __ldg(reinterpret_cast<const float2*>(rb + ro + col));
                             o.x += r.x; o.y += r.y;
@@ -622,14 +598,11 @@ __global__ void pack_split_kernel(const float* __restrict__ packed, unsigned sho
     const long long total = (long long)K * c_out;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int kk = (int)(i / c_out), co = (int)(i % c_out);   // coalesced reads of the packed weight
-        unsigned short h, l;
-        const float v = kWScaleT5 * __ldg(packed + i);
-        asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(h) : "f"(v));
-        const float rem = v - __half2float(__ushort_as_half(h));
-        asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(l) : "f"(rem));
+        __half h, l;
+        split_f16(kWScale * __ldg(packed + i), h, l);
         const size_t o = (size_t)co * K + kk;
-        split[o] = h;
-        split[(size_t)K * c_out + o] = l;
+        split[o] = __half_as_ushort(h);
+        split[(size_t)K * c_out + o] = __half_as_ushort(l);
     }
 }
 
@@ -647,19 +620,13 @@ int launch_t5(const float* x, float* out, const float* w1, const float* b1, cons
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     JK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for a [%d, %lld, %d] fp32 tensor", (int)r, n, T, C);
-    static bool attr_set[64] = {};
-    static int sms[64] = {};
-    int dev = 0;
-    JK_CHECK_CUDA(cudaGetDevice(&dev));
-    if (!attr_set[dev & 63]) {
-        JK_CHECK_CUDA(cudaFuncSetAttribute(resblock_t5_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, T5<C>::smem));
-        JK_CHECK_CUDA(cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
-        attr_set[dev & 63] = true;
-    }
+    int sms = 0;
+    if (int rc = set_max_smem_once<resblock_t5_kernel<C>>(T5<C>::smem)) return rc;
+    if (int rc = sm_count(&sms)) return rc;
     const long long per_clip = (T + kBM - 1) / kBM, total = per_clip * n;
     JK_REQUIRE(total < (1ll << 31) && T + 4096 < (1ll << 31), "clip too long for 32-bit tile coordinates");
-    const unsigned grid = (unsigned)std::min<long long>(total, sms[dev & 63]);
-    resblock_t5_kernel<C><<<grid, 32 * (9 + 4 * T5Groups<C>::value), T5<C>::smem, stream>>>(map, x, out, w1, b1, w2, b2, T, dil, rs, (int)per_clip, (int)total);
+    const unsigned grid = (unsigned)std::min<long long>(total, sms);
+    resblock_t5_kernel<C><<<grid, T5<C>::kThreads, T5<C>::smem, stream>>>(map, x, out, w1, b1, w2, b2, T, dil, rs, (int)per_clip, (int)total);
     JK_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -678,18 +645,12 @@ int launch_conv_t5(const ConvT5P& P, int n, cudaStream_t stream) {
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     JK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for a [%d, %lld, %d] fp32 tensor", (int)r, n, P.t_in, CI);
-    static bool attr_set[64] = {};
-    static int sms[64] = {};
-    int dev = 0;
-    JK_CHECK_CUDA(cudaGetDevice(&dev));
-    if (!attr_set[dev & 63]) {
-        JK_CHECK_CUDA(cudaFuncSetAttribute((conv_t5_kernel<CI, CO>), cudaFuncAttributeMaxDynamicSharedMemorySize, T5C<CI, CO>::smem));
-        JK_CHECK_CUDA(cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
-        attr_set[dev & 63] = true;
-    }
+    int sms = 0;
+    if (int rc = set_max_smem_once<conv_t5_kernel<CI, CO>>(T5C<CI, CO>::smem)) return rc;
+    if (int rc = sm_count(&sms)) return rc;
     const long long per_clip = (P.t_out + kBM - 1) / kBM, total = per_clip * n;
     JK_REQUIRE(total < (1ll << 31) && P.t_in + 4096 < (1ll << 31), "clip too long for 32-bit tile coordinates");
-    const unsigned grid = (unsigned)std::min<long long>(total, sms[dev & 63]);
+    const unsigned grid = (unsigned)std::min<long long>(total, sms);
     conv_t5_kernel<CI, CO><<<grid, kConvThreads, T5C<CI, CO>::smem, stream>>>(map, P, (int)per_clip, (int)total);
     JK_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -721,18 +682,12 @@ int launch_conv_wide(const float* in, long long t_in, const void* w_split, const
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         JK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for a [2 x %d, %lld] fp16 split weight", (int)r, P.c_out, K);
     }
-    static bool attr_set[64] = {};
-    static int sms[64] = {};
-    int dev = 0;
-    JK_CHECK_CUDA(cudaGetDevice(&dev));
-    if (!attr_set[dev & 63]) {
-        JK_CHECK_CUDA(cudaFuncSetAttribute(conv_wide_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, T5W<BN>::smem));
-        JK_CHECK_CUDA(cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
-        attr_set[dev & 63] = true;
-    }
+    int sms = 0;
+    if (int rc = set_max_smem_once<conv_wide_kernel<BN>>(T5W<BN>::smem)) return rc;
+    if (int rc = sm_count(&sms)) return rc;
     const long long per_clip = (P.t_out + kBM - 1) / kBM, n_tiles_n = P.c_out / BN, total = per_clip * n * n_tiles_n;
     JK_REQUIRE(total < (1ll << 31) && t_in + 4096 < (1ll << 31), "clip too long for 32-bit tile coordinates");
-    const unsigned grid = (unsigned)std::min<long long>(total, sms[dev & 63]);
+    const unsigned grid = (unsigned)std::min<long long>(total, sms);
     conv_wide_kernel<BN><<<grid, kWideThreads, T5W<BN>::smem, stream>>>(map_x, map_w, P, (int)per_clip, (int)n_tiles_n, (int)total);
     JK_CHECK_CUDA(cudaGetLastError());
     return 0;

@@ -1,8 +1,6 @@
 """Encoder / Decoder conv stacks (reference: jukebox/vqvae/encdec.py), channels-last [N, T, C]."""
 import torch.nn as nn
 
-import os
-
 from .ops_cl import Conv1d, ConvTranspose1d
 from .resnet import Resnet1D, use_tensor_cores
 
@@ -51,9 +49,8 @@ class DecoderConvBock(nn.Module):
                     ConvTranspose1d(width, input_emb_width if i == (down_t - 1) else width, filter_t, stride_t, pad_t)))
         self.model = nn.Sequential(*blocks)
         # decoder side: nothing downstream needs a fixed FMA order, so the residual blocks take the tensor-core kernel
-        # (JK_VQVAE_EXACT=1 keeps the exact-FMA kernel everywhere, e.g. to compare the two)
-        if not os.environ.get("JK_VQVAE_EXACT"):
-            use_tensor_cores(self)
+        # (use_tensor_cores(module, False) gives the exact-FMA route, e.g. to compare the two)
+        use_tensor_cores(self)
 
     def forward(self, x):
         for m in self.model:

@@ -20,8 +20,8 @@ class ResConv1DBlock(nn.Module):
             nn.init.zeros_(self.model[-1].weight)
             nn.init.zeros_(self.model[-1].bias)
         self.res_scale = res_scale
-        # decoder-side stacks (Decoder, Conditioner) run this block on the tensor cores (3xTF32, jk_resblock_tc); the
-        # encoder feeds the bit-exact codebook argmin and keeps the exact-FMA kernel.  Set by `use_tensor_cores`.
+        # decoder-side stacks (Decoder, Conditioner) run this block on the tensor cores (fp16 x 3 split, jk_resblock_tc);
+        # the encoder feeds the bit-exact codebook argmin and keeps the exact-FMA kernel.  Set by `use_tensor_cores`.
         self.tensor_cores = False
 
     def forward(self, x):

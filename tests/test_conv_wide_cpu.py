@@ -70,6 +70,5 @@ def test_only_the_decoder_side_sets_tensor_cores():
     dec = [m for m in vq.decoders.modules() if hasattr(m, "tensor_cores")]
     assert enc and dec
     assert not any(m.tensor_cores for m in enc)
-    if not os.environ.get("JK_VQVAE_EXACT"):
-        blocks = [m for d in vq.decoders for m in d.level_blocks.modules() if hasattr(m, "tensor_cores")]
-        assert blocks and all(m.tensor_cores for m in blocks)
+    blocks = [m for d in vq.decoders for m in d.level_blocks.modules() if hasattr(m, "tensor_cores")]
+    assert blocks and all(m.tensor_cores for m in blocks)

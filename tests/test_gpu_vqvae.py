@@ -114,7 +114,7 @@ def test_tensor_core_resblock_matches_exact_fma_kernel(C, dil, T):
     """jk_resblock_tc (split-precision tensor-core block, decoder side) against jk_resblock_cl (exact fp32 FMAs): same block
     (resnet.py:27-44), fp32-level agreement; ragged T, dilations beyond the tile, both channel counts.  T >= 128 runs the
     wgmma / TMA kernel (vqvae_t5.cu: 128-position MMA tiles, out-of-range rows zero-filled by the tensor map), shorter
-    clips the fp16 x 3 mma.sync kernel (JK_RESBLOCK_T5=0 / JK_RESBLOCK_TF32=1 select the older kernels for A/B runs)"""
+    clips (T = 64, 65) the fp16 x 3 mma.sync kernel"""
     import ctypes as Cc
     from jukebox_b200._lib import lib, check, ptr, stream_ptr
     g = torch.Generator(device="cuda").manual_seed(C + dil)

@@ -9,15 +9,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench  # noqa: E402
 
-if os.environ.get("JK_VARIANT"):      # A/B runs: an older build of the library (variants/*.so) that may predate newer entry points
-    import ctypes
-    from jukebox_b200 import _lib
-    _lib.LIB_PATH = os.path.join(ROOT, "variants", os.environ["JK_VARIANT"] + ".so")
-    probe = ctypes.CDLL(_lib.LIB_PATH)
-    for name in list(_lib.SIGNATURES):
-        if not hasattr(probe, name):
-            del _lib.SIGNATURES[name]
-
 with contextlib.redirect_stdout(sys.stderr):
     wl = bench.SMALL if "--small" in sys.argv else bench.WORKLOADS[os.environ.get("JK_WORKLOAD", "1b_lyrics")]
     prior, _ = bench.build_prior(wl)

@@ -7,9 +7,6 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-if os.environ.get("JK_VARIANT"):      # A/B runs: variants/*.so
-    from jukebox_b200 import _lib as _l
-    _l.LIB_PATH = os.path.join(ROOT, "variants", os.environ["JK_VARIANT"] + ".so")
 from jukebox_b200._lib import lib, check, ptr, stream_ptr  # noqa: E402
 
 for C, T, dil in ((64, 4096, 3), (64, 32768, 27), (32, 32768, 9), (64, 262144, 243)):
