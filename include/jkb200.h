@@ -289,17 +289,19 @@ int jk_conv1d_tc_wide(const jk_conv_args* a, const void* w_split, jk_stream_t st
 
 /* ResConv1DBlock (vqvae/resnet.py:27-44): out = x + res_scale * (W2.relu(W1 *_dil relu(x) + b1) + b2)
  * x, out [n, T, C] (x != out); w1 packed [3, C, Cs]; w2 packed [1, Cs, C].  For C == Cs in {32, 64} (every
- * ResConv1DBlock of the reference's VQ-VAEs) this is ONE launch with the hidden activation kept in shared memory and
- * tmp may be NULL; other shapes run as two jk_conv1d_cl launches through tmp [n, T, Cs]. */
+ * ResConv1DBlock of the reference's VQ-VAEs) with x, out, w1, w2, b1 and b2 16-byte aligned this is ONE launch with the
+ * hidden activation kept in shared memory and tmp may be NULL; other shapes and pointers run as two jk_conv1d_cl launches
+ * through tmp [n, T, Cs], and without tmp they are an error. */
 int jk_resblock_cl(const float* x, float* out, float* tmp, const float* w1, const float* b1, const float* w2,
                    const float* b2, int n, int64_t T, int C, int Cs, int dilation, float res_scale,
                    jk_stream_t stream);
 
 /* The same ResConv1DBlock on the tensor cores for the DECODER side (Decoder stacks of vqvae/encdec.py:87-131 and the
  * upsampler Conditioner, prior/conditioners.py:8-48), C == Cs in {32, 64}: fp16 x 3 split (hi / lo fp16 operands, weights
- * scaled by 2^8 before their split, hi.w_hi + lo.w_hi + hi.w_lo accumulated in fp32), on wgmma + TMA for T >= 128 and
- * 16-byte aligned x / out, on mma.sync m16n8k16 otherwise; i.e. fp32 accuracy up to the dropped lo.w_lo term but NOT the
- * FMA order of jk_resblock_cl.  The encoder, whose output feeds the bit-exact codebook argmin, must keep jk_resblock_cl. */
+ * scaled by 2^8 before their split, hi.w_hi + lo.w_hi + hi.w_lo accumulated in fp32), on wgmma + TMA for T >= 128, on
+ * mma.sync m16n8k16 for shorter clips; i.e. fp32 accuracy up to the dropped lo.w_lo term but NOT the FMA order of
+ * jk_resblock_cl.  x and out must be 16-byte aligned and b1, b2 8-byte aligned; other pointers are an error (nothing is
+ * launched).  The encoder, whose output feeds the bit-exact codebook argmin, must keep jk_resblock_cl. */
 int jk_resblock_tc(const float* x, float* out, const float* w1, const float* b1, const float* w2, const float* b2,
                    int n, int64_t T, int C, int dilation, float res_scale, jk_stream_t stream);
 

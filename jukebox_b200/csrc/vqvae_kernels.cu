@@ -219,8 +219,9 @@ __global__ void __launch_bounds__(256) conv1d_cl_kernel(ConvP P) {
 // and re-read it: 2 x 4 x C bytes per position of 5 x 4 x C).  Each thread owns 8 positions x 4 channels; per
 // 4 k-steps it issues 8 + 4 LDS.128 for 128 FMAs (the generic kernel: 20 LDS for 64), with the position
 // mapping (ty + TY * i) chosen so that the lanes of a warp read at most TX-strided rows 1 apart: no bank
-// conflicts with the 4-float row padding.  fp32 FMAs in the generic kernel's order (tap, then input channel),
-// so both paths agree to the last bit on everything before the residual add.
+// conflicts with the 4-float row padding.  fp32 FMAs in the generic kernel's order (tap, then input channel), so both
+// paths agree to the last bit on everything before the residual add; the add itself is rounded differently (the two
+// agree bitwise for a power-of-two res_scale, and within one rounding of x + res_scale * y otherwise).
 // ---------------------------------------------------------------------------------------
 template <int C>
 __global__ void __launch_bounds__(256, 1)
@@ -425,7 +426,8 @@ int launch_resblock_fused(const float* x, float* out, const float* w1, const flo
 // ---------------------------------------------------------------------------------------
 // ResConv1DBlock on the tensor cores, for the DECODER side (Decoder / Conditioner stacks: their outputs are audio and
 // conditioning, never an argmin input, so summation order is free; the encoder keeps the exact-FMA kernel above).  This
-// kernel takes the shapes resblock_t5_kernel (vqvae_t5.cu) does not: clips under 128 positions, unaligned pointers.
+// kernel takes the clips under 128 positions, which resblock_t5_kernel (vqvae_t5.cu) does not; like it, it needs 16-byte
+// aligned x / out (and 8-byte aligned b1 / b2), which jk_resblock_tc checks.
 // The fp16 x 3 split of split_tma.cuh on mma.sync.m16n8k16: x = hi + lo with hi = fp16(x), lo = fp16(x - hi): 22 mantissa
 // bits, the same as a 3xTF32 split (fp16 and TF32 both carry 11 significant bits), products hi.w_hi + lo.w_hi + hi.w_lo
 // accumulated in fp32.  Against 3xTF32 on m16n8k8: an MMA covers k = 16 instead of 8 at the same issue cost, operands are
@@ -959,11 +961,15 @@ extern "C" int jk_resblock_cl(const float* x, float* out, float* tmp, const floa
                               const float* b2, int n, int64_t T, int C, int Cs, int dilation, float res_scale,
                               jk_stream_t stream) {
     JK_REQUIRE(x && out && w1 && w2, "null argument");
-    if (C == Cs && b1 && b2 && x != out && T > 0) {   // the VQ-VAE's own shapes: one fused launch
+    // the fused kernel reads x, w1, w2, b1, b2 and writes out as float4: other pointers take the two launches below, whose
+    // dispatch checks alignment before every vector access
+    const bool vec4 = (((uintptr_t)x | (uintptr_t)out | (uintptr_t)w1 | (uintptr_t)w2 | (uintptr_t)b1 | (uintptr_t)b2) & 15) == 0;
+    if (C == Cs && b1 && b2 && x != out && T > 0 && vec4) {   // the VQ-VAE's own shapes: one fused launch
         if (C == 64) return launch_resblock_fused<64>(x, out, w1, b1, w2, b2, n, T, dilation, res_scale, (cudaStream_t)stream);
         if (C == 32) return launch_resblock_fused<32>(x, out, w1, b1, w2, b2, n, T, dilation, res_scale, (cudaStream_t)stream);
     }
-    JK_REQUIRE(tmp, "tmp ([n, T, Cs] floats) is required for shapes without the fused kernel");
+    JK_REQUIRE(tmp, "jk_resblock_cl: tmp ([n, T, Cs] floats) is required unless C == Cs in {32, 64} and x, out, w1, w2, b1, b2 "
+                    "are 16-byte aligned (the fused kernel)");
     jk_conv_args a;
     a.tensor_cores = 0;
     a.in = x; a.t_in = T; a.c_in = C; a.out = tmp; a.t_out = T; a.c_out = Cs; a.w = w1; a.bias = b1; a.res = nullptr;
@@ -981,8 +987,11 @@ extern "C" int jk_resblock_tc(const float* x, float* out, const float* w1, const
                               int n, int64_t T, int C, int dilation, float res_scale, jk_stream_t stream) {
     JK_REQUIRE(x && out && w1 && w2 && b1 && b2, "null argument");
     JK_REQUIRE(x != out && T > 0 && n > 0, "x and out must differ, T and n must be positive");
-    // wgmma + TMA version (vqvae_t5.cu): whole 128-position MMA tiles, TMA needs 16-byte aligned rows
-    if ((C == 64 || C == 32) && T >= 128 && (((uintptr_t)x | (uintptr_t)out) & 15) == 0)
+    // both kernels read x and write out in 16-byte (t5) or 8- and 16-byte (h2) vectors, and the h2 kernel reads b1 / b2 as float2
+    JK_REQUIRE((((uintptr_t)x | (uintptr_t)out) & 15) == 0 && (((uintptr_t)b1 | (uintptr_t)b2) & 7) == 0,
+               "jk_resblock_tc: x and out must be 16-byte aligned, b1 and b2 8-byte aligned");
+    // wgmma + TMA version (vqvae_t5.cu): whole 128-position MMA tiles
+    if ((C == 64 || C == 32) && T >= 128)
         return jk::resblock_t5(x, out, w1, b1, w2, b2, n, T, C, dilation, res_scale, (cudaStream_t)stream);
     if (C == 64) return launch_resblock_h2<64>(x, out, w1, b1, w2, b2, n, T, dilation, res_scale, (cudaStream_t)stream);
     if (C == 32) return launch_resblock_h2<32>(x, out, w1, b1, w2, b2, n, T, dilation, res_scale, (cudaStream_t)stream);
