@@ -216,6 +216,37 @@ int jk_prior_prefill_capacity(const jk_prior* p, int* max_positions);
 int jk_prior_config_prefill_capacity(const jk_prior_config* cfg, int* max_positions);
 int jk_prior_prefill(jk_prior* p, const jk_prefill_args* args, jk_stream_t stream);
 
+/* The attention of one prefill layer on its own: the code jk_prior_prefill runs per layer (forward output and recorded
+ * weights), for tests and for callers that hold q / K / V themselves.  Per sample b, head h and query position p < P,
+ * over the keys of p's pattern (attn_func 0 dense, 1 block, 2 transpose, 3 previous block, 7 prime: positions < P;
+ * 6 encoder-decoder: every encoder row):
+ *   s_j = fp16(fp16(q . k_j) * dh^-1/2);  out = fp16(sum_j fp16(exp(s_j - max s)) v_j / sum_j exp(s_j - max s))
+ * (exponentials fp32; a query without keys gives 0) and, when w is set, the weights of jk_attn_record. */
+typedef struct jk_prefill_attn_args {
+    const void* qkv;          /* fp16 [n * P][q_stride]: q | k | v of each row, q_stride = 3 * heads * dh (attn_func 6:
+                                 q only, q_stride = heads * dh) */
+    const void* k_cache;      /* attn_func 6: fp16 [n][heads][enc_rows][dh_pad]; else NULL */
+    const void* v_cache;
+    void* out;                /* fp16 [n * P][heads * dh], or NULL */
+    void* w;                  /* recorded weights, fp16 [n][heads][P][ld], or NULL (zeroed first, keys >= ld skipped) */
+    int32_t ld;
+    int32_t n, P, heads, dh, dh_pad;   /* dh_pad: row length of the caches, dh <= dh_pad, a multiple of 16 */
+    int32_t attn_func, bc, prime;      /* bc: block length (1, 2, 3); prime: the padded prime length (7) */
+    int32_t enc_rows;                  /* attn_func 6: encoder rows of the caches */
+    int32_t route;                     /* 0: the prefill's own choice of kernel; 1: the scalar kernels */
+} jk_prefill_attn_args;
+/* the kernels a call ran: tensor_cores 0 = the scalar kernels (tile_dh, stage_bytes 0); 1 = mma.sync kernels of head
+ * tile tile_dh (32, 64, 128, 160, 256) staging K / V in stage_bytes (16 or 4) chunks */
+typedef struct jk_prefill_attn_route {
+    int32_t tensor_cores;
+    int32_t tile_dh;
+    int32_t stage_bytes;
+} jk_prefill_attn_route;
+/* qkv, out and the caches must be 16-byte aligned; neither out nor w, an unknown attn_func, a pattern parameter < 1,
+ * dh > dh_pad or dh_pad % 16 != 0, or a scalar-route shape with (dh + max(P, enc_rows)) * 4 > 64 KB is an error, and
+ * nothing is written.  taken (may be NULL) receives the route. */
+int jk_prefill_attention_f16(const jk_prefill_attn_args* a, jk_prefill_attn_route* taken, jk_stream_t stream);
+
 /* one token position; increments the device-side position counter */
 int jk_prior_step(jk_prior* p, const jk_step_args* a, jk_stream_t stream);
 /* current position (host copy of the device counter as tracked by the calls made so far); -1 after a truncated prefill
@@ -230,10 +261,17 @@ int jk_prior_debug_buffer(const jk_prior* p, int which, const void** ptr, size_t
 
 /* Conv1D at prefill / training shape on the tensor cores (wgmma + TMA): y[M, N] = x[M, K] . w + b, fp16 in,
  * fp32 accumulate, fp16 out (transformer/ops.py:83-101).  w_t is the weight TRANSPOSED: [N, K] row-major fp16;
- * bias fp32 [N] or NULL; K must be a multiple of 64.  Used for c_enc_kv(encoder_kv)
- * (factored_attention.py:273-287) inside jk_prior_set_encoder_kv. */
+ * bias fp32 [N] or NULL; K >= 64 and K % 8 == 0 (a K tail past the last 64-wide block reads zeros); x, w_t and y
+ * 16-byte aligned.  Used for c_enc_kv(encoder_kv) (factored_attention.py:273-287) inside jk_prior_set_encoder_kv. */
 int jk_conv1d_prefill_f16(const void* x, const void* w_t, const float* bias, void* y, int M, int N, int K,
                           jk_stream_t stream);
+/* The GEMM of the chunked prefill with its epilogues, the same kernel as above; with y = fp16(acc + bias) rounded once:
+ *   epi 0: y;   1: quick_gelu with the reference's fp16 roundings (ops.py:33-35),
+ *               z = fp16(1.702 y), sg = fp16(1 / (1 + exp(-z))), out = fp16(y * sg);   2: fp16(res + y)
+ * res: fp16 [M, N], read by epi 2 only.  K as above; x, w_t, y and res (when set) 16-byte aligned; epi 2 without res,
+ * another epi or a constraint not met is an error, checked before anything is launched. */
+int jk_prefill_gemm_f16(const void* x, const void* w_t, const float* bias, const void* res, void* y, int M, int N, int K,
+                        int epi, jk_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * VQ-VAE.  Tensors are channels-last: [N, T, C] fp32.

@@ -74,6 +74,16 @@ class PrefillArgs(C.Structure):
                 ("n_capture", C.c_int32)]
 
 
+class PrefillAttnArgs(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("qkv", "k_cache", "v_cache", "out", "w")] + \
+               [(n, C.c_int32) for n in
+                ("ld", "n", "P", "heads", "dh", "dh_pad", "attn_func", "bc", "prime", "enc_rows", "route")]
+
+
+class PrefillAttnRoute(C.Structure):
+    _fields_ = [("tensor_cores", C.c_int32), ("tile_dh", C.c_int32), ("stage_bytes", C.c_int32)]
+
+
 class ConvArgs(C.Structure):
     _fields_ = [("inp", C.c_void_p), ("t_in", C.c_int64), ("c_in", C.c_int32),
                 ("out", C.c_void_p), ("t_out", C.c_int64), ("c_out", C.c_int32),
@@ -105,7 +115,9 @@ SIGNATURES = {
     "jk_prior_position": (_I, [_P, C.POINTER(C.c_int)]),
     "jk_prior_has_logits_gemm": (_I, [_P, C.POINTER(C.c_int)]),
     "jk_prior_debug_buffer": (_I, [_P, _I, C.POINTER(_P), C.POINTER(C.c_size_t)]),
+    "jk_prefill_attention_f16": (_I, [C.POINTER(PrefillAttnArgs), C.POINTER(PrefillAttnRoute), _P]),
     "jk_conv1d_prefill_f16": (_I, [_P, _P, _P, _P, _I, _I, _I, _P]),
+    "jk_prefill_gemm_f16": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "jk_sample_categorical": (_I, [_P, _L, _I, _I, _F, C.c_uint64, _I, _P, _L, _P]),
     "jk_sample_categorical_scored": (_I, [_P, _L, _P, _L, _I, _I, _F, C.c_uint64, _I, _P, _L, _P, _L, _P]),
     "jk_xout_split_bytes": (_I, [_I, _I, C.POINTER(C.c_size_t)]),

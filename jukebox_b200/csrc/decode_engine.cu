@@ -1988,10 +1988,7 @@ extern "C" int jk_prior_create(const jk_prior_config* cfg, void* arena, size_t a
         const int nowait = getenv("JK_NOWAIT") ? atoi(getenv("JK_NOWAIT")) : 0;
         JK_CHECK_CUDA(cudaMemcpyToSymbol(jk_nowait, &nowait, sizeof(int)));
     }
-    {   // reference: scale = 1/sqrt(sqrt(dh)); w.mul_(scale*scale)  (factored_attention.py:83-88)
-        double sc = 1.0 / sqrt(sqrt((double)L.dh));
-        E.scale2 = (float)(sc * sc);
-    }
+    E.scale2 = attn_scale2(L.dh);
     E.cols = (const ushort2*)(A + L.off_cols);
     p->d_cols = (ushort2*)(A + L.off_cols);
     p->d_goff = (uint32_t*)(A + L.off_goff);

@@ -52,6 +52,13 @@ struct EngineDev {
     LayerDev layer[JK_MAX_DEPTH];
 };
 
+// the attention scores' scale dh^-1/2, as the reference applies it to q and k in two halves:
+// scale = 1/sqrt(sqrt(dh)); w.mul_(scale*scale)  (factored_attention.py:83-88)
+inline float attn_scale2(int dh) {
+    const double sc = 1.0 / sqrt(sqrt((double)dh));
+    return (float)(sc * sc);
+}
+
 // prefill_gemm.cu: Y = epi(X . W^T + bias [, res]) on wgmma; w_t is [N, K] fp16.
 //   epi 0: fp16(acc + b)   1: fp16(quick_gelu(fp16(acc + b)))   2: fp16(res + fp16(acc + b))
 int gemm_f16_tc(const void* x, const void* w_t, const float* bias, const void* res, void* y, int M, int N, int K,

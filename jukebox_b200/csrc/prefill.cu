@@ -551,12 +551,20 @@ int launch_attn_mma(const AttnFwd& A, const AttnSeqs& Q, int nseq, int n, __half
     return 0;
 }
 
-// the layer's attention (w == nullptr) or its recorded weights on the tensor cores: returns 1 if the tensor-core kernel
-// took the layer, 0 if the shape is left to attn_fwd_kernel / attn_record_kernel, < 0 on error
-int attn_mma(const AttnFwd& A, int n, __half* w, int ld, cudaStream_t stream) {
-    static const bool off = getenv("JK_PREFILL_SCALAR_ATTN") != nullptr;
-    if (off || A.dh % 2 != 0 || A.dh > 256) return 0;
+// the kernels that take a layer's attention: the tensor-core kernels for even dh <= 256 (16-byte staging when every head
+// row is 16-byte aligned, 4-byte words otherwise), the scalar kernels for other head sizes or when `scalar` asks for them
+jk_prefill_attn_route attn_route(const AttnFwd& A, bool scalar) {
+    jk_prefill_attn_route r = {0, 0, 0};
+    if (scalar || A.dh % 2 != 0 || A.dh > 256) return r;
     const bool w16 = A.dh % 8 == 0 && A.S % 8 == 0 && A.dhp % 8 == 0;
+    r.tensor_cores = 1;
+    r.stage_bytes = w16 ? 16 : 4;
+    r.tile_dh = !w16 ? (A.dh <= 160 ? 160 : 256) : A.dh <= 32 ? 32 : A.dh <= 64 ? 64 : A.dh <= 128 ? 128 : 256;
+    return r;
+}
+
+// the layer's attention (w == nullptr) or its recorded weights on the tensor cores, route r (attn_route, tensor_cores 1)
+int attn_mma(const AttnFwd& A, const jk_prefill_attn_route& r, int n, __half* w, int ld, cudaStream_t stream) {
     AttnSeqs Q;
     Q.attn_func = A.attn_func; Q.bc = A.bc; Q.P = A.P; Q.prime = A.prime; Q.enc_rows = A.enc_rows;
     int nseq = 1, maxq = A.P;
@@ -566,13 +574,46 @@ int attn_mma(const AttnFwd& A, int n, __half* w, int ld, cudaStream_t stream) {
         default: break;
     }
     Q.tiles_per_seq = (maxq + 63) / 64;
-    int rc;
-    if (!w16) rc = A.dh <= 160 ? launch_attn_mma<160, false>(A, Q, nseq, n, w, ld, stream) : launch_attn_mma<256, false>(A, Q, nseq, n, w, ld, stream);
-    else if (A.dh <= 32) rc = launch_attn_mma<32, true>(A, Q, nseq, n, w, ld, stream);
-    else if (A.dh <= 64) rc = launch_attn_mma<64, true>(A, Q, nseq, n, w, ld, stream);
-    else if (A.dh <= 128) rc = launch_attn_mma<128, true>(A, Q, nseq, n, w, ld, stream);
-    else rc = launch_attn_mma<256, true>(A, Q, nseq, n, w, ld, stream);
-    return rc ? rc : 1;
+    if (r.stage_bytes == 4) return r.tile_dh == 160 ? launch_attn_mma<160, false>(A, Q, nseq, n, w, ld, stream)
+                                                    : launch_attn_mma<256, false>(A, Q, nseq, n, w, ld, stream);
+    switch (r.tile_dh) {
+        case 32: return launch_attn_mma<32, true>(A, Q, nseq, n, w, ld, stream);
+        case 64: return launch_attn_mma<64, true>(A, Q, nseq, n, w, ld, stream);
+        case 128: return launch_attn_mma<128, true>(A, Q, nseq, n, w, ld, stream);
+        default: return launch_attn_mma<256, true>(A, Q, nseq, n, w, ld, stream);
+    }
+}
+
+// dynamic shared memory of the scalar kernels: q and one score per key
+size_t scalar_attn_smem(const AttnFwd& A) { return (size_t)(A.dh + std::max(A.P, A.enc_rows)) * 4; }
+constexpr size_t kScalarAttnSmemMax = 64 * 1024;
+
+// One layer's attention, as the prefill runs it: the forward output into A.a (when set) and, when w is set, the recorded
+// weights w [n][H][P][ld] (zeroed first: entries outside the pattern and rows without keys stay 0).  Both take route r.
+int layer_attention(const AttnFwd& A, const jk_prefill_attn_route& r, int n, __half* w, int ld, cudaStream_t stream) {
+    const size_t smem = scalar_attn_smem(A);
+    if (!r.tensor_cores) {
+        if (int rc = set_max_smem_once<attn_fwd_kernel>((int)kScalarAttnSmemMax)) return rc;
+        if (int rc = set_max_smem_once<attn_record_kernel>((int)kScalarAttnSmemMax)) return rc;
+    }
+    if (A.a) {
+        if (r.tensor_cores) {
+            if (int rc = attn_mma(A, r, n, nullptr, 0, stream)) return rc;
+        } else {
+            attn_fwd_kernel<<<dim3(A.P, A.H, n), kFwdThreads, smem, stream>>>(A);
+            JK_CHECK_CUDA(cudaGetLastError());
+        }
+    }
+    if (w) {
+        JK_CHECK_CUDA(cudaMemsetAsync(w, 0, (size_t)n * A.H * A.P * ld * sizeof(__half), stream));
+        if (r.tensor_cores) {
+            if (int rc = attn_mma(A, r, n, w, ld, stream)) return rc;
+        } else {
+            attn_record_kernel<<<dim3(A.P, A.H, n), kFwdThreads, smem, stream>>>(A, w, ld);
+            JK_CHECK_CUDA(cudaGetLastError());
+        }
+    }
+    return 0;
 }
 
 // ---- K, V of the given positions -> the caches the decode kernel attends -------------------------------
@@ -689,6 +730,36 @@ extern "C" int jk_pool_rows_f32(const float* x, int n, int P, int width, int t0,
     return launch_act_rows<float>(x, n, P, width, t0, t1, x_cond, x_cond ? x_cond_len : 1, 1, out, (cudaStream_t)stream);
 }
 
+extern "C" int jk_prefill_attention_f16(const jk_prefill_attn_args* a, jk_prefill_attn_route* taken, jk_stream_t stream) {
+    JK_REQUIRE(a, "null argument");
+    const int f = a->attn_func;
+    JK_REQUIRE(f == 0 || f == 1 || f == 2 || f == 3 || f == 6 || f == 7, "attn_func %d (0, 1, 2, 3, 6 or 7)", f);
+    JK_REQUIRE(a->n >= 1 && a->P >= 1 && a->heads >= 1 && a->dh >= 1, "empty shape (n %d, P %d, heads %d, dh %d)", a->n, a->P,
+               a->heads, a->dh);
+    JK_REQUIRE(a->dh <= a->dh_pad && a->dh_pad % 16 == 0, "dh_pad %d: a multiple of 16, at least dh %d", a->dh_pad, a->dh);
+    JK_REQUIRE(f < 1 || f > 3 || a->bc >= 1, "attn_func %d needs a block length bc >= 1 (got %d)", f, a->bc);
+    JK_REQUIRE(f != 7 || a->prime >= 1, "attn_func 7 needs prime >= 1 (got %d)", a->prime);
+    JK_REQUIRE(f != 6 || (a->enc_rows >= 1 && a->k_cache && a->v_cache), "attn_func 6 needs enc_rows >= 1 (got %d) and both caches",
+               a->enc_rows);
+    JK_REQUIRE(!a->w || a->ld >= 1, "recorded weights need ld >= 1 (got %d)", a->ld);
+    JK_REQUIRE(a->out || a->w, "neither out nor w: nothing to compute");
+    JK_REQUIRE(a->qkv, "null qkv");
+    JK_REQUIRE((((uintptr_t)a->qkv | (uintptr_t)a->out | (uintptr_t)a->k_cache | (uintptr_t)a->v_cache) & 15) == 0,
+               "qkv, out and the caches must be 16-byte aligned");
+    JK_REQUIRE(a->route == 0 || a->route == 1, "route %d (0: the prefill's choice, 1: the scalar kernels)", a->route);
+    AttnFwd A;
+    A.qkv = (const __half*)a->qkv; A.a = (__half*)a->out; A.kc = (const __half*)a->k_cache; A.vc = (const __half*)a->v_cache;
+    A.P = a->P; A.S = a->heads * a->dh; A.H = a->heads; A.dh = a->dh; A.bc = a->bc; A.attn_func = f; A.prime = a->prime;
+    A.q_stride = f == 6 ? A.S : 3 * A.S; A.enc_rows = f == 6 ? a->enc_rows : 0; A.dhp = a->dh_pad; A.scale2 = attn_scale2(a->dh);
+    const jk_prefill_attn_route r = attn_route(A, a->route == 1);
+    JK_REQUIRE(r.tensor_cores || scalar_attn_smem(A) <= kScalarAttnSmemMax,
+               "the scalar kernels hold dh + max(P, enc_rows) = %d floats in shared memory (at most %d)",
+               a->dh + std::max(A.P, A.enc_rows), (int)(kScalarAttnSmemMax / 4));
+    if (int rc = layer_attention(A, r, a->n, (__half*)a->w, a->ld, (cudaStream_t)stream)) return rc;
+    if (taken) *taken = r;
+    return 0;
+}
+
 extern "C" int jk_prior_prefill_capacity(const jk_prior* p, int* max_positions) {
     JK_REQUIRE(p && max_positions, "null argument");
     *max_positions = p->pf_len;
@@ -748,10 +819,7 @@ extern "C" int jk_prior_prefill(jk_prior* p, const jk_prefill_args* a, jk_stream
         JK_CHECK_CUDA(cudaGetLastError());
     }
     const unsigned ln_grid = (unsigned)((rows + 7) / 8);
-    const size_t fwd_smem = (size_t)(E.dh + std::max(P, E.enc_dims)) * 4;
-    if (int rc = set_max_smem_once<attn_fwd_kernel>(64 * 1024)) return rc;
-    if (int rc = set_max_smem_once<attn_record_kernel>(64 * 1024)) return rc;
-    JK_REQUIRE(fwd_smem <= 64 * 1024, "prefill attention tile too large");
+    JK_REQUIRE((size_t)(E.dh + std::max(P, E.enc_dims)) * 4 <= kScalarAttnSmemMax, "prefill attention tile too large");
     for (int l = 0; l < depth; ++l) {
         const LayerDev& LD = E.layer[l];
         ln_rows_kernel<<<ln_grid, 256, 0, stream>>>(p->pf_x, LD.ln0_g, LD.ln0_b, p->pf_xn, rows, W);
@@ -764,22 +832,11 @@ extern "C" int jk_prior_prefill(jk_prior* p, const jk_prefill_args* a, jk_stream
         A.qkv = p->pf_qkv; A.a = p->pf_a; A.P = P; A.S = S; A.H = H; A.dh = E.dh; A.bc = E.bc; A.attn_func = LD.attn_func;
         A.prime = E.prime_pad; A.scale2 = E.scale2; A.q_stride = q_stride; A.kc = LD.kc; A.vc = LD.vc; A.enc_rows = E.enc_dims;
         A.dhp = E.dh_pad;
-        rc = attn_mma(A, n, nullptr, 0, stream);        // tensor cores when the head geometry allows (dh even, dh <= 256)
-        if (rc < 0) return rc;
-        if (rc == 0) {
-            attn_fwd_kernel<<<dim3(P, H, n), kFwdThreads, fwd_smem, stream>>>(A);
-            JK_CHECK_CUDA(cudaGetLastError());
-        }
-        if (const jk_attn_record* r = rec[l]) {         // reads q / K only: before the next layer overwrites pf_qkv
-            __half* w = (__half*)r->w;
-            JK_CHECK_CUDA(cudaMemsetAsync(w, 0, (size_t)n * H * P * r->ld * sizeof(__half), stream));
-            rc = attn_mma(A, n, w, r->ld, stream);
-            if (rc < 0) return rc;
-            if (rc == 0) {
-                attn_record_kernel<<<dim3(P, H, n), kFwdThreads, fwd_smem, stream>>>(A, w, r->ld);
-                JK_CHECK_CUDA(cudaGetLastError());
-            }
-        }
+        // tensor cores when the head geometry allows (dh even, dh <= 256); the recorded weights read q / K only, so they
+        // are taken here, before the next layer overwrites pf_qkv
+        const jk_attn_record* r = rec[l];
+        rc = layer_attention(A, attn_route(A, false), n, r ? (__half*)r->w : nullptr, r ? r->ld : 0, stream);
+        if (rc) return rc;
         if (!enc) {
             const size_t cnt = (size_t)rows * S;
             kv_scatter_kernel<<<(unsigned)((cnt + 255) / 256), 256, 0, stream>>>(p->pf_qkv, LD.kc, LD.vc, n, P, S, H, E.dh, E.dh_pad,

@@ -161,7 +161,7 @@ int jk::gemm_f16_tc(const void* x, const void* w_t, const float* bias, const voi
     JK_REQUIRE(x && w_t && y, "null argument");
     JK_REQUIRE(M >= 1 && N >= 1 && K >= BK && K % 8 == 0, "prefill GEMM needs K >= %d and K %% 8 == 0 (16-byte rows for TMA); got M %d N %d K %d", BK, M, N, K);
     JK_REQUIRE((((uintptr_t)x | (uintptr_t)w_t | (uintptr_t)y | (uintptr_t)res) & 15) == 0, "operands must be 16-byte aligned");
-    JK_REQUIRE(epi >= 0 && epi <= 2 && (epi != 2 || res), "bad epilogue");
+    JK_REQUIRE(epi >= 0 && epi <= 2 && (epi != 2 || res), "bad epilogue %d (0, 1, or 2 with res)", epi);
     CUtensorMap mx, mw;
     int rc = make_map(&mx, x, M, K);
     if (rc) return rc;
@@ -178,4 +178,9 @@ int jk::gemm_f16_tc(const void* x, const void* w_t, const float* bias, const voi
 extern "C" int jk_conv1d_prefill_f16(const void* x, const void* w_t, const float* bias, void* y, int M, int N, int K,
                                      jk_stream_t stream_) {
     return jk::gemm_f16_tc(x, w_t, bias, nullptr, y, M, N, K, 0, (cudaStream_t)stream_);
+}
+
+extern "C" int jk_prefill_gemm_f16(const void* x, const void* w_t, const float* bias, const void* res, void* y, int M, int N,
+                                   int K, int epi, jk_stream_t stream_) {
+    return jk::gemm_f16_tc(x, w_t, bias, res, y, M, N, K, epi, (cudaStream_t)stream_);
 }

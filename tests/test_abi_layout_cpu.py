@@ -13,7 +13,8 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PAIRS = {"jk_prior_config": "PriorConfig", "jk_layer_weights": "LayerWeights", "jk_prior_plan_info": "PlanInfo",
          "jk_step_args": "StepArgs", "jk_prefill_args": "PrefillArgs", "jk_conv_args": "ConvArgs",
-         "jk_f32_layer": "F32Layer", "jk_f32_args": "F32Args"}
+         "jk_f32_layer": "F32Layer", "jk_f32_args": "F32Args", "jk_prefill_attn_args": "PrefillAttnArgs",
+         "jk_prefill_attn_route": "PrefillAttnRoute"}
 
 
 def _fields(header, name):
