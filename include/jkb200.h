@@ -394,6 +394,24 @@ int jk_xout_logprob_workspace_bytes(int m, int width, int bins, size_t* bytes);
 int jk_xout_logprob(const float* h, int m, int width, const void* w_split, int bins, const int64_t* targets,
                     float* logp, float* lse, void* workspace, size_t workspace_bytes, jk_stream_t stream);
 
+/* Statistics of the predictive distribution p = softmax(z) from the activations, with no logits tensor (csrc/score.cu):
+ *   entropy[m]           = lse[m] - sum_b p[m, b] z[m, b]                      (nats; fp32, accumulated in fp64)
+ *   logp[m]              = z[m, targets[m]] - lse[m]                           (when targets is given)
+ *   topk_ids[m, 0..k)    = the k bins of largest z[m, :], by descending z, ties to the lower bin   (int64)
+ *   topk_logp[m, 0..k)   = z[m, topk_ids[m, j]] - lse[m]
+ *   lse[m]               = log sum_b exp(z[m, b])
+ * h, width, w_split (jk_pack_xout_split's layout) and the product are jk_xout_logprob's; logp and lse are its results bit
+ * for bit.  targets and logp are both NULL or both given; topk_ids and topk_logp may each be NULL (k = 0: no top-k);
+ * lse may be NULL; 0 <= k <= JK_XOUT_STATS_MAX_K and k <= bins.  It needs jk_xout_stats_workspace_bytes of 256-byte
+ * aligned device memory and synchronises the stream for the same range check as jk_xout_logprob: an out-of-range
+ * activation or target is an error, and the outputs are then nan (ids -1), never a wrong number.  A row's result does not
+ * depend on the other rows. */
+#define JK_XOUT_STATS_MAX_K 16
+int jk_xout_stats_workspace_bytes(int m, int width, int bins, int k, size_t* bytes);
+int jk_xout_stats(const float* h, int m, int width, const void* w_split, int bins, const int64_t* targets, int k,
+                  float* logp, float* entropy, int64_t* topk_ids, float* topk_logp, float* lse, void* workspace,
+                  size_t workspace_bytes, jk_stream_t stream);
+
 /* top-k / nucleus filtering in front of the sampler (transformer/ops.py:113-142 `filter_logits`, applied to
  * logits / temp as autoregressive.py:232-234 does): out[r, v] = logits[r, v] / temp if v stays, else -inf.
  * top_k > 0: the k largest stay; top_p > 0: the smallest prefix of the sorted row whose softmax mass exceeds top_p

@@ -13,6 +13,7 @@ LIB_PATH = os.path.join(_HERE, "libjkb200.so")
 
 JK_MAX_DEPTH = 96
 JK_MAX_BATCH = 32
+JK_XOUT_STATS_MAX_K = 16        # jkb200.h: the largest top-k jk_xout_stats returns
 
 
 class PriorConfig(C.Structure):
@@ -124,6 +125,8 @@ SIGNATURES = {
     "jk_pack_xout_split": (_I, [_P, _P, _I, _I, _P]),
     "jk_xout_logprob_workspace_bytes": (_I, [_I, _I, _I, C.POINTER(C.c_size_t)]),
     "jk_xout_logprob": (_I, [_P, _I, _I, _P, _I, _P, _P, _P, _P, C.c_size_t, _P]),
+    "jk_xout_stats_workspace_bytes": (_I, [_I, _I, _I, _I, C.POINTER(C.c_size_t)]),
+    "jk_xout_stats": (_I, [_P, _I, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P, _P, C.c_size_t, _P]),
     "jk_filter_logits": (_I, [_P, _L, _I, _I, _F, _I, _F, _P, _L, _P]),
     "jk_vq_argmin": (_I, [_P, _P, _P, _P, _L, _I, _I, _P]),
     "jk_vq_gather": (_I, [_P, _P, _P, _L, _I, _I, _P]),

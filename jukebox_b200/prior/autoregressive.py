@@ -159,26 +159,48 @@ class ConditionalAutoregressive2D(nn.Module):
         capacity, in batches the engine takes; fp32: the fp32 path), + cond, then x_out and the log-softmax at the target
         in one fused kernel (jk_xout_logprob) - no logits tensor."""
         from ..score import xout_logprob
-        from .._lib import JK_MAX_BATCH
         assert not self.only_encode
         with t.no_grad():
-            x = self.preprocess(x)
+            x = self.preprocess(x).contiguous()
             N, D = x.shape
             assert D == self.input_dims, f"logprob scores whole sequences of {self.input_dims} tokens, got {D}"
-            assert (0 <= x).all() and (x < self.bins).all()
-            x_cond, y_cond = self._check_conds(N, x_cond, y_cond)
-            x = x.contiguous()
-            if fp16:
-                part = lambda v, i: None if v is None else v[i:i + JK_MAX_BATCH]
-                acts = t.cat([self._acts_fp16(x[i:i + JK_MAX_BATCH], part(x_cond, i), part(y_cond, i),
-                                              part(encoder_kv, i)) for i in range(0, N, JK_MAX_BATCH)])
-            else:
-                from ..transformer import f32
-                h = f32.embed(self, x, y_cond, x_cond, N, D, 0)
-                acts = self.transformer(h, encoder_kv=encoder_kv, fp16=False)
-            if self.add_cond_after_transformer and x_cond is not None:
-                acts = acts + x_cond
+            acts = self._head_acts(x, x_cond, y_cond, encoder_kv, fp16)
             return xout_logprob(acts.reshape(N * D, self.width), self.x_out.weight, x.view(-1)).view(N, D)
+
+    def token_stats(self, x, x_cond=None, y_cond=None, encoder_kv=None, fp16=True, top_k=0):
+        """Statistics of the model's prediction at every position of the tokens x [N, D] (2 <= D <= input_dims; the stack
+        is causal, so a prefix is scored as in the full window): a score.TokenStats of logp [N, D] (the log-likelihood of
+        x, as `logprob`), entropy [N, D] in nats, topk_ids [N, D, top_k] / topk_logp (the most likely tokens, ties to the
+        lower id) and lse [N, D].  The activations are logprob's; x_out and the statistics run in one fused kernel
+        (jk_xout_stats) - no logits tensor.  x_cond is [N, input_dims or 1, width]: a short window reads its first D rows."""
+        from ..score import xout_stats, TokenStats
+        assert not self.only_encode
+        with t.no_grad():
+            x = self.preprocess(x).contiguous()
+            N, D = x.shape
+            assert 1 < D <= self.input_dims, f"windows of 2 .. {self.input_dims} tokens, got {D}"
+            acts = self._head_acts(x, x_cond, y_cond, encoder_kv, fp16)
+            st = xout_stats(acts.reshape(N * D, self.width), self.x_out.weight, x.view(-1), top_k=top_k)
+            return TokenStats(*(None if v is None else v.view(N, D, *v.shape[1:]) for v in st))
+
+    def _head_acts(self, x, x_cond, y_cond, encoder_kv, fp16):
+        """what x_out reads for the tokens x [N, D]: the stack's output (fp16: the decode engine, in batches it takes;
+        fp32: the fp32 path) + x_cond where the prior adds it behind the stack.  Shared by logprob and token_stats."""
+        from .._lib import JK_MAX_BATCH
+        N, D = x.shape
+        assert (0 <= x).all() and (x < self.bins).all()
+        x_cond, y_cond = self._check_conds(N, x_cond, y_cond)
+        if fp16:
+            part = lambda v, i: None if v is None else v[i:i + JK_MAX_BATCH]
+            acts = t.cat([self._acts_fp16(x[i:i + JK_MAX_BATCH], part(x_cond, i), part(y_cond, i),
+                                          part(encoder_kv, i)) for i in range(0, N, JK_MAX_BATCH)])
+        else:
+            from ..transformer import f32
+            h = f32.embed(self, x, y_cond, x_cond, N, D, 0)
+            acts = self.transformer(h, encoder_kv=encoder_kv, fp16=False)
+        if self.add_cond_after_transformer and x_cond is not None:
+            acts = acts + (x_cond[:, :D] if x_cond.shape[1] > 1 else x_cond)
+        return acts
 
     def forward(self, x, x_cond=None, y_cond=None, encoder_kv=None, fp16=False, loss_full=False, encode=False,
                 get_preds=False, get_acts=False, get_sep_loss=False):

@@ -349,6 +349,30 @@ class SimplePrior(nn.Module):
                 prime = -lp.view(N, L).mean(1) / ln2
             return gen, prime
 
+    def token_stats(self, z, z_conds=[], y=None, fp16=True, top_k=0):
+        """Per-code statistics of the model's prediction for codes z [N, D] (2 <= D <= n_ctx) of this level, conditioned
+        exactly as score conditions a window: a score.TokenStats of logp / entropy / lse [N, D] and, with top_k,
+        topk_ids / topk_logp [N, D, top_k] (ConditionalAutoregressive2D.token_stats).  A single_enc_dec prior takes its
+        lyric head into the causal pass and returns the music positions only; its top-k ids are shifted into this
+        level's code space as sampled tokens are, and an id of the lyric vocabulary comes back as -1 (its
+        log-probability stays: the model put that mass there)."""
+        from ..score import TokenStats
+        with t.no_grad():
+            x_cond, y_cond, lyric = self.get_cond(z_conds, y)
+            if self.copy_input:
+                lyric = z[:, :self.n_tokens]
+            if not self.single_enc_dec:
+                enc = self.get_encoder_kv(lyric, fp16=fp16)
+                return self.prior.token_stats(z, x_cond, y_cond, enc, fp16=fp16, top_k=top_k)
+            seq, x_cond = self.prior_preprocess([lyric, z], [None, x_cond])
+            st = self.prior.token_stats(seq, x_cond, y_cond, fp16=fp16, top_k=top_k)
+            pl, shift = self.prior.prime_len, self.spaces.shift[-1]
+            st = TokenStats(*(None if v is None else v[:, pl:] for v in st))
+            if top_k:
+                ids = st.topk_ids - shift
+                st = st._replace(topk_ids=t.where(ids >= 0, ids, t.full_like(ids, -1)))
+            return st
+
     def layer_acts(self, z, z_conds=[], y=None, layers=(), fp16=True, pool=True):
         """Representations of codes z [N, D] (D <= n_ctx) of this level, conditioned exactly as z_forward / score
         condition them: {layer: fp32 [N, width]} (pool: the mean over the window's codes) or [N, D, width], the outputs

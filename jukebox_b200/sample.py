@@ -88,6 +88,50 @@ class LevelRun:
         return self.zs
 
 
+# ---- whole-song statistics ----------------------------------------------------------------------------------
+def song_windows(total_length, n_ctx, hop_length):
+    """(window, t0, t1) for each window of plan_windows(0, total_length, n_ctx, hop_length) that draws tokens: sampling
+    a level from nothing draws tokens [t0, t1) in that window, with [window.start, t0) as its context.  The [t0, t1)
+    partition [0, total_length)."""
+    out, have = [], 0
+    for win in plan_windows(0, total_length, n_ctx, hop_length):
+        end = win.start + win.sample_tokens
+        if end > have:
+            out.append((win, have, end))
+            have = end
+    return out
+
+
+def song_token_stats(prior, zs, labels, level, hop_length, fp16=True, top_k=0, max_batch_size=16):
+    """Statistics of every code of a level, each scored the way sampling drew it: token t is scored in the window of
+    plan_windows(0, T, n_ctx, hop_length) that drew it, conditioned on that window's labels (get_y) and upper-level
+    codes (get_z_conds), with the window's earlier codes as its context.  zs: the codes of every level (zs[level]
+    [N, T]); labels: this level's labels, as sample_level takes them.  Items go through the engine in pieces of
+    max_batch_size, as LevelRun runs them.  Returns a score.TokenStats of [N, T] logp / entropy / lse and, with top_k,
+    [N, T, top_k] topk_ids / topk_logp (SimplePrior.token_stats)."""
+    from .score import TokenStats
+    z = zs[level]
+    N, T = z.shape
+    cols = []
+    for win, t0, t1 in song_windows(T, prior.n_ctx, hop_length):
+        context = z[:, win.start:t1]
+        upper = prior.get_z_conds(zs, win.start, win.start + prior.n_ctx)
+        y = prior.get_y(labels, win.start)
+        pieces = zip(split_batch(context, N, max_batch_size), split_batch(upper, N, max_batch_size),
+                     split_batch(y, N, max_batch_size))
+        done = []
+        for ctx_i, upper_i, y_i in pieces:
+            if upper_i is not None:
+                upper_i = [u.contiguous() for u in upper_i]
+            done.append(prior.token_stats(ctx_i.contiguous(), upper_i, y_i, fp16=fp16, top_k=top_k))
+        cols.append(TokenStats(*(None if v[0] is None else t.cat(v, dim=0)[:, t0 - win.start:] for v in zip(*done))))
+    if not cols:
+        e = t.empty(N, 0, device=z.device)
+        k = t.empty(N, 0, top_k, device=z.device)
+        return TokenStats(e, e.clone(), k.long() if top_k else None, k if top_k else None, e.clone())
+    return TokenStats(*(None if v[0] is None else t.cat(v, dim=1) for v in zip(*cols)))
+
+
 # ---- the reference's entry points -------------------------------------------------------------------------
 def sample_partial_window(zs, labels, sampling_kwargs, level, prior, tokens_to_sample, hps):
     """`tokens_to_sample` new tokens at `level`, the context sliding once it is full"""
