@@ -8,15 +8,15 @@ are overwritten by earlier ones, exactly as the reference's reversed loop does.
 The forward pass is SimplePrior.z_forward with the sampling fp16 flag, as in the reference (sample.py:118-119 ->
 get_alignment):
   fp16=True  - the fp16 prefill records the layer's weights on the tensor cores (csrc/prefill.cu, fp16 weights, the
-               reference's fp16 mode); as many items per call as one engine takes (items_per_pass), since prefill rows
-               are independent and the weights are the same bits as item by item.  A window longer than the prefill
-               capacity (JK_PREFILL_MAX) records on the fp32 path instead;
+               reference's fp16 mode); as many items per call as one prefill takes (items_per_prefill of the prior's
+               autoregressive model), since prefill rows are independent and the weights are the same bits as item by
+               item; an engine built for fewer items is rebuilt once, on the first window, and serves every later one.
+               A window longer than the prefill capacity (JK_PREFILL_MAX) records on the fp32 path instead;
   fp16=False - the fp32 forward-mode path (Transformer.forward(sample=False) -> csrc/f32_path.cu), item by item.
 """
 import numpy as np
 import torch as t
 
-from ._lib import JK_MAX_BATCH
 from .utils.sample_utils import get_starts
 
 
@@ -28,26 +28,15 @@ def pad_to_context(z, n_ctx):
     return z, pad
 
 
-def items_per_pass(prior, bs, fp16):
-    """items of one z_forward call: in fp16 the most that one engine of this prior takes (up to JK_MAX_BATCH; 5b_lyrics
-    takes 16, the 16-row kernel), so that they record in one prefill - an engine built for fewer samples is rebuilt once,
-    on the first window, and serves every later one; in fp32 one, like the reference"""
-    if not fp16 or bs == 1:
-        return 1
-    tr = prior.prior.transformer
-    for n in sorted({min(bs, JK_MAX_BATCH), min(bs, JK_MAX_BATCH // 2)}, reverse=True):
-        if tr.prefill_capacity(n) > 0:
-            return n
-    return 1
-
-
 def hop_weights(prior, z_window, y, fp16):
     """[bs, n_ctx, n_tokens] weights (fp32 array) of the alignment head for one window; each z_forward call records a
-    [items, heads, n_ctx, keys] tensor"""
+    [items, heads, n_ctx, keys] tensor: in fp16 as many items as one prefill takes (item by item when the prior has no
+    prefill), in fp32 one, like the reference"""
     layer, head = prior.alignment_layer, prior.alignment_head
     rows = []
-    step = items_per_pass(prior, z_window.shape[0], fp16)
-    for i in range(0, z_window.shape[0], step):
+    bs = z_window.shape[0]
+    step = (prior.prior.items_per_prefill(bs) or 1) if fp16 and bs > 1 else 1
+    for i in range(0, bs, step):
         ws = prior.z_forward(z_window[i:i + step], [], y[i:i + step], fp16=fp16, get_attn_weights={layer})
         assert len(ws) == 1
         rows.append(ws[0][:, head].float())

@@ -89,11 +89,15 @@ class ConditionalAutoregressive2D(nn.Module):
         return x.view(N, -1)
 
     # ---- engine plumbing ------------------------------------------------------------------
+    def _configure_engine(self):
+        """the engine also computes this model's logits (none for an only_encode model) and adds x_cond where the model
+        adds it"""
+        self.transformer.configure_engine(bins=0 if self.only_encode else self.bins,
+                                          add_cond_after=self.add_cond_after_transformer)
+
     def _engine(self, n_samples):
-        tr = self.transformer
-        tr.configure_engine(bins=0 if self.only_encode else self.bins,
-                            add_cond_after=self.add_cond_after_transformer)
-        eng = tr.engine(n_samples)
+        self._configure_engine()
+        eng = self.transformer.engine(n_samples)
         x_out = None if self.only_encode else self.x_out.weight
         start = None if self.y_cond else self.start_token
         # the key lives ON the engine object: a freshly built engine (drop_engine after .cuda() /
@@ -104,6 +108,17 @@ class ConditionalAutoregressive2D(nn.Module):
             eng.set_embeddings(x_emb=self.x_emb.weight, pos_emb=self.pos_emb.pos_emb, x_out=x_out,
                                start_token=None if start is None else start.view(-1))
             eng._emb_key = key
+        return eng
+
+    def _fresh_engine(self, n, encoder_kv):
+        """the engine for n items at position 0 with empty caches, and the lyric encoder's keys encoder_kv [n, ...]
+        loaded when a layer attends to them (attn_func 6)"""
+        eng = self._engine(n)
+        tr = self.transformer
+        tr.del_cache()
+        if any(b.attn_func == 6 for b in tr._attn_mods):
+            assert encoder_kv is not None
+            eng.set_encoder_kv(encoder_kv)
         return eng
 
     def _check_conds(self, N, x_cond, y_cond):
@@ -122,6 +137,28 @@ class ConditionalAutoregressive2D(nn.Module):
         else:
             assert x_cond is None      # zeros in the reference; NULL for the kernel
         return x_cond, y_cond
+
+    def _given(self, x, x_cond, y_cond, whole):
+        """the given tokens of a teacher-forced pass, checked: x [N, D] of ids in [0, bins), a whole window of input_dims
+        tokens when `whole`, else a causal prefix of 2 <= D <= input_dims; x_cond / y_cond as _check_conds takes them.
+        Returns (x contiguous int64, x_cond, y_cond)."""
+        x = self.preprocess(x)
+        N, D = x.shape
+        if whole:
+            assert D == self.input_dims, f"whole sequences of {self.input_dims} tokens, got {D}"
+        else:
+            assert 1 < D <= self.input_dims, f"windows of 2 .. {self.input_dims} tokens, got {D}"
+        assert (0 <= x).all() and (x < self.bins).all()
+        x_cond, y_cond = self._check_conds(N, x_cond, y_cond)
+        return x.contiguous(), x_cond, y_cond
+
+    def _add_x_cond(self, acts, x_cond, t0, t1):
+        """acts [N, t1 - t0, width] of positions [t0, t1) + x_cond where this model adds it behind the stack
+        (add_cond_after_transformer, reference autoregressive.py:226-227); x_cond [N, input_dims or 1, width]: one row
+        serves every position"""
+        if not self.add_cond_after_transformer or x_cond is None:
+            return acts
+        return acts + (x_cond[:, t0:t1] if x_cond.shape[1] > 1 else x_cond)
 
     def _run(self, n_samples, prime, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds, sample_tokens,
              get_logprobs=False):
@@ -156,15 +193,14 @@ class ConditionalAutoregressive2D(nn.Module):
     def logprob(self, x, x_cond=None, y_cond=None, encoder_kv=None, fp16=True):
         """log-likelihood in nats of every token of whole sequences x [N, input_dims] given the ones before it, fp32
         [N, input_dims]: the activations of `forward` (fp16: the decode engine's prefill, or its steps beyond the prefill
-        capacity, in batches the engine takes; fp32: the fp32 path), + cond, then x_out and the log-softmax at the target
-        in one fused kernel (jk_xout_logprob) - no logits tensor."""
+        capacity, in pieces of items the engine takes; fp32: the fp32 path), + cond, then x_out and the log-softmax at the
+        target in one fused kernel (jk_xout_logprob) - no logits tensor."""
         from ..score import xout_logprob
         assert not self.only_encode
         with t.no_grad():
-            x = self.preprocess(x).contiguous()
+            x, x_cond, y_cond = self._given(x, x_cond, y_cond, whole=True)
             N, D = x.shape
-            assert D == self.input_dims, f"logprob scores whole sequences of {self.input_dims} tokens, got {D}"
-            acts = self._head_acts(x, x_cond, y_cond, encoder_kv, fp16)
+            acts = self._add_x_cond(self._stack_out(x, x_cond, y_cond, encoder_kv, fp16), x_cond, 0, D)
             return xout_logprob(acts.reshape(N * D, self.width), self.x_out.weight, x.view(-1)).view(N, D)
 
     def token_stats(self, x, x_cond=None, y_cond=None, encoder_kv=None, fp16=True, top_k=0):
@@ -176,31 +212,11 @@ class ConditionalAutoregressive2D(nn.Module):
         from ..score import xout_stats, TokenStats
         assert not self.only_encode
         with t.no_grad():
-            x = self.preprocess(x).contiguous()
+            x, x_cond, y_cond = self._given(x, x_cond, y_cond, whole=False)
             N, D = x.shape
-            assert 1 < D <= self.input_dims, f"windows of 2 .. {self.input_dims} tokens, got {D}"
-            acts = self._head_acts(x, x_cond, y_cond, encoder_kv, fp16)
+            acts = self._add_x_cond(self._stack_out(x, x_cond, y_cond, encoder_kv, fp16), x_cond, 0, D)
             st = xout_stats(acts.reshape(N * D, self.width), self.x_out.weight, x.view(-1), top_k=top_k)
             return TokenStats(*(None if v is None else v.view(N, D, *v.shape[1:]) for v in st))
-
-    def _head_acts(self, x, x_cond, y_cond, encoder_kv, fp16):
-        """what x_out reads for the tokens x [N, D]: the stack's output (fp16: the decode engine, in batches it takes;
-        fp32: the fp32 path) + x_cond where the prior adds it behind the stack.  Shared by logprob and token_stats."""
-        from .._lib import JK_MAX_BATCH
-        N, D = x.shape
-        assert (0 <= x).all() and (x < self.bins).all()
-        x_cond, y_cond = self._check_conds(N, x_cond, y_cond)
-        if fp16:
-            part = lambda v, i: None if v is None else v[i:i + JK_MAX_BATCH]
-            acts = t.cat([self._acts_fp16(x[i:i + JK_MAX_BATCH], part(x_cond, i), part(y_cond, i),
-                                          part(encoder_kv, i)) for i in range(0, N, JK_MAX_BATCH)])
-        else:
-            from ..transformer import f32
-            h = f32.embed(self, x, y_cond, x_cond, N, D, 0)
-            acts = self.transformer(h, encoder_kv=encoder_kv, fp16=False)
-        if self.add_cond_after_transformer and x_cond is not None:
-            acts = acts + (x_cond[:, :D] if x_cond.shape[1] > 1 else x_cond)
-        return acts
 
     def forward(self, x, x_cond=None, y_cond=None, encoder_kv=None, fp16=False, loss_full=False, encode=False,
                 get_preds=False, get_acts=False, get_sep_loss=False):
@@ -213,24 +229,17 @@ class ConditionalAutoregressive2D(nn.Module):
         records in the same prefill when the window fits one prefill call (D <= prefill_capacity), else it takes the
         fp32 path.  No gradients: training is out of scope, the loss is an evaluation."""
         with t.no_grad():
-            x = self.preprocess(x)
+            x, x_cond, y_cond = self._given(x, x_cond, y_cond, whole=True)
             N, D = x.shape
-            assert D == self.input_dims, f"forward runs whole sequences of {self.input_dims} tokens, got {D}"
-            assert (0 <= x).all() and (x < self.bins).all()
-            x_cond, y_cond = self._check_conds(N, x_cond, y_cond)
-            x = x.contiguous()
             if fp16 and self.transformer._record_layers:     # asked before an engine is built: else the fp32 path
-                self.transformer.configure_engine(bins=0 if self.only_encode else self.bins,
-                                                  add_cond_after=self.add_cond_after_transformer)
+                self._configure_engine()
                 fp16 = 1 < D <= self.transformer.prefill_capacity(N)
             if fp16:
-                acts = self._acts_fp16(x, x_cond, y_cond, encoder_kv)
+                acts = t.empty(N, D, self.width, dtype=t.float32, device=x.device)
+                self._prefill(x, x_cond, y_cond, encoder_kv, h_out=acts, record=True)
             else:
-                from ..transformer import f32
-                h = f32.embed(self, x, y_cond, x_cond, N, D, 0)
-                acts = self.transformer(h, encoder_kv=encoder_kv, fp16=False)
-            if self.add_cond_after_transformer and x_cond is not None:
-                acts = acts + x_cond
+                acts = self._f32_pass(x, x_cond, y_cond, encoder_kv)
+            acts = self._add_x_cond(acts, x_cond, 0, D)
             if self.only_encode:
                 return acts
             from ..transformer import f32
@@ -253,10 +262,9 @@ class ConditionalAutoregressive2D(nn.Module):
         """items one fp16 prefill of this model takes: up to JK_MAX_BATCH, or half that when only the 16-row engine fits
         (5b_lyrics); 0 when the configuration has no prefill"""
         from .._lib import JK_MAX_BATCH
-        tr = self.transformer
-        tr.configure_engine(bins=0 if self.only_encode else self.bins, add_cond_after=self.add_cond_after_transformer)
+        self._configure_engine()
         for n in sorted({min(N, JK_MAX_BATCH), min(N, max(1, JK_MAX_BATCH // 2))}, reverse=True):
-            if tr.prefill_capacity(n) > 0:
+            if self.transformer.prefill_capacity(n) > 0:
                 return n
         return 0
 
@@ -269,26 +277,20 @@ class ConditionalAutoregressive2D(nn.Module):
         returns; with add_cond, x_cond is added as `forward` adds it (add_cond_after_transformer).  x_cond is
         [N, input_dims or 1, width]: a short window reads its first D rows.
         fp16: the decode engine's prefill, stopped after the deepest requested layer, with the layers' rows taken (and
-        averaged) inside it (jk_act_capture); items in batches of one engine; a window beyond the prefill capacity is an
+        averaged) inside it (jk_act_capture); items in pieces of one engine; a window beyond the prefill capacity is an
         error.  fp32: the fp32 path up to the deepest layer, averaged by the same kernel (jk_pool_rows_f32)."""
         from .. import _lib
         from ..engine import Capture
         layers = sorted(set(int(l) for l in layers))
         assert layers and 0 <= layers[0] and layers[-1] < self.depth, f"layers {layers} outside [0, {self.depth})"
         with t.no_grad():
-            x = self.preprocess(x)
+            x, x_cond, y_cond = self._given(x, x_cond, y_cond, whole=False)
             N, D = x.shape
-            assert 1 < D <= self.input_dims, f"windows of 2 .. {self.input_dims} tokens, got {D}"
             assert 0 <= t0 < D, f"t0 {t0} outside [0, {D})"
-            assert (0 <= x).all() and (x < self.bins).all()
-            x_cond, y_cond = self._check_conds(N, x_cond, y_cond)
-            x = x.contiguous()
             addc = bool(add_cond) and self.add_cond_after_transformer and x_cond is not None
             dev, W = x.device, self.width
             if not fp16:
-                from ..transformer import f32
-                h = f32.embed(self, x, y_cond, x_cond, N, D, 0)
-                outs = self.transformer(h, encoder_kv=encoder_kv, fp16=False, layers=layers)
+                outs = self._f32_pass(x, x_cond, y_cond, encoder_kv, layers=layers)
                 res = {}
                 for l, o in outs.items():
                     if pool:
@@ -299,9 +301,7 @@ class ConditionalAutoregressive2D(nn.Module):
                             _lib.ptr(res[l]), _lib.stream_ptr()))
                     else:
                         o = o[:, t0:]
-                        if addc:
-                            o = o + (x_cond[:, t0:D] if x_cond.shape[1] > 1 else x_cond)
-                        res[l] = o.contiguous()
+                        res[l] = (self._add_x_cond(o, x_cond, t0, D) if add_cond else o).contiguous()
                 return res
             step = self.items_per_prefill(N)
             cap = self.transformer.prefill_capacity(step) if step else 0
@@ -309,48 +309,66 @@ class ConditionalAutoregressive2D(nn.Module):
                 raise RuntimeError(f"layer_acts(fp16=True): a window of {D} positions exceeds the prefill capacity "
                                    f"{cap} of this model; use fp16=False")
             res = {l: t.empty((N, W) if pool else (N, D - t0, W), dtype=t.float32, device=dev) for l in layers}
-            tr = self.transformer
-            part = lambda v, i: None if v is None else v[i:i + step].contiguous()
-            for i in range(0, N, step):
-                n = min(step, N - i)
-                eng = self._engine(n)
-                tr.del_cache()
-                if any(b.attn_func == 6 for b in tr._attn_mods):
-                    assert encoder_kv is not None
-                    eng.set_encoder_kv(encoder_kv[i:i + n])
-                bufs = {l: t.empty((n, W) if pool else (n, D - t0, W), dtype=t.float32, device=dev) for l in layers}
-                eng.prefill(n, D, tokens=x[i:i + n], y_cond=part(y_cond, i), x_cond=part(x_cond, i),
-                            n_layers=layers[-1] + 1, capture={l: Capture(b, t0, D, pool, addc) for l, b in bufs.items()})
-                tr.del_cache()
-                for l, b in bufs.items():
-                    res[l][i:i + n] = b
+            self._prefill_items(x, x_cond, y_cond, encoder_kv, n_layers=layers[-1] + 1,
+                                capture={l: Capture(b, t0, D, pool, addc) for l, b in res.items()})
             return res
 
-    def _acts_fp16(self, x, x_cond, y_cond, encoder_kv):
-        """the causal stack over given tokens on the fp16 decode engine: position by position it computes exactly the
-        forward pass (reference check_sample, factored_attention.py:424-455).  The recorded layers' attention weights come
-        from the prefill (fp16, Transformer.store_ws)."""
+    # ---- teacher-forced passes over given tokens ------------------------------------------------------------------
+    def _stack_out(self, x, x_cond, y_cond, encoder_kv, fp16):
+        """the stack's output fp32 [N, D, width] over the given tokens x [N, D] of any number of items (x_cond not yet
+        added behind it): fp16 - the decode engine, in pieces (_prefill_items); fp32 - the fp32 path to the last layer"""
+        if not fp16:
+            return self._f32_pass(x, x_cond, y_cond, encoder_kv, layers=[self.depth - 1])[self.depth - 1]
+        acts = t.empty(*x.shape, self.width, dtype=t.float32, device=x.device)
+        self._prefill_items(x, x_cond, y_cond, encoder_kv, h_out=acts)
+        return acts
+
+    def _f32_pass(self, x, x_cond, y_cond, encoder_kv, layers=None):
+        """the given tokens x [N, D] through f32.embed and the fp32 path (csrc/f32_path.cu).  With layers: {layer: its
+        output [N, D, width]}, stopped after the deepest (F32Path.run_layers, any 2 <= D <= input_dims).  Without: forward
+        mode's output of a whole window, which records the attention of the recorded layers (Transformer.forward)."""
+        from ..transformer import f32
+        N, D = x.shape
+        h = f32.embed(self, x, y_cond, x_cond, N, D, 0)
+        return self.transformer(h, encoder_kv=encoder_kv, fp16=False, layers=layers)
+
+    def _prefill_items(self, x, x_cond, y_cond, encoder_kv, h_out=None, n_layers=0, capture=None):
+        """_prefill over any number of items, in consecutive pieces of the one batching rule: as many items as one
+        prefill takes (items_per_prefill: up to JK_MAX_BATCH, 16 for 5b_lyrics), or min(N, JK_MAX_BATCH) when no engine
+        size of this model has a prefill (those pieces step their tokens).  Items are independent rows: each piece writes
+        its own rows of h_out [N, ...] and of the capture buffers [N, ...]."""
+        from .._lib import JK_MAX_BATCH
+        N = x.shape[0]
+        n = self.items_per_prefill(N) or min(N, JK_MAX_BATCH)
+        rows = lambda v, i: None if v is None else v[i:i + n]
+        for i in range(0, N, n):
+            cap = None if capture is None else {l: c._replace(out=c.out[i:i + n]) for l, c in capture.items()}
+            self._prefill(x[i:i + n], rows(x_cond, i), rows(y_cond, i), rows(encoder_kv, i), h_out=rows(h_out, i),
+                          n_layers=n_layers, capture=cap)
+
+    def _prefill(self, x, x_cond, y_cond, encoder_kv, h_out=None, record=False, n_layers=0, capture=None):
+        """one teacher-forced pass of the given tokens x [N, D] on the fp16 decode engine: a fresh engine, one prefill
+        that fills whichever of h_out (the stack's output, fp32 [N, D, width]), the recorded layers' attention weights
+        (record: fp16, Transformer.store_ws), a stop after n_layers and the layer captures the caller asks for, then the
+        caches emptied.  Position by position the prefill computes exactly the forward pass (reference check_sample,
+        factored_attention.py:424-455).  A window beyond the prefill capacity steps its tokens, which gives h_out only."""
         N, D = x.shape
         tr = self.transformer
-        eng = self._engine(N)
-        tr.del_cache()
-        if any(b.attn_func == 6 for b in tr._attn_mods):
-            assert encoder_kv is not None
-            eng.set_encoder_kv(encoder_kv)
-        acts = t.empty(N, D, self.width, dtype=t.float32, device=x.device)
+        eng = self._fresh_engine(N, encoder_kv)
         if 1 < D <= eng.prefill_capacity:
-            ws = {i: t.empty(N, tr.n_head, D, tr.record_ld(i), dtype=t.float16, device=x.device) for i in tr._record_layers}
-            eng.prefill(N, D, tokens=x, y_cond=y_cond, x_cond=x_cond, h_out=acts, record=ws)
+            ws = {i: t.empty(N, tr.n_head, D, tr.record_ld(i), dtype=t.float16, device=x.device)
+                  for i in (tr._record_layers if record else ())}
+            eng.prefill(N, D, tokens=x, y_cond=y_cond, x_cond=x_cond, h_out=h_out, record=ws, n_layers=n_layers,
+                        capture=capture)
             if ws:
                 tr.store_ws(ws)
         else:
-            assert not tr._record_layers, "attention is recorded by the prefill"
+            assert not (record and tr._record_layers) and not capture, "attention and captures come from the prefill"
             for i in range(D):
                 out = t.empty(N, self.width, dtype=t.float32, device=x.device)
                 eng.step(N, tokens=x, y_cond=y_cond, x_cond=x_cond, h_out=out)
-                acts[:, i] = out
-        self.transformer.del_cache()
-        return acts
+                h_out[:, i] = out
+        tr.del_cache()
 
 
 class SamplingWindow:
@@ -375,12 +393,8 @@ class SamplingWindow:
         assert P < self.sample_tokens <= ca.input_dims, \
             f"need given tokens {P} < sample_tokens {self.sample_tokens} <= input_dims {ca.input_dims}"
         dev = ca.x_emb.weight.device
-        self.eng = eng = ca._engine(N)
-        self.tr = tr = ca.transformer
-        tr.del_cache()
-        if any(b.attn_func == 6 for b in tr._attn_mods):
-            assert encoder_kv is not None
-            eng.set_encoder_kv(encoder_kv)
+        self.eng = eng = ca._fresh_engine(N, encoder_kv)
+        self.tr = ca.transformer
         self.tokens = t.zeros(N, self.sample_tokens, dtype=t.long, device=dev)
         if P:
             assert (0 <= prime).all() and (prime < ca.bins).all()
@@ -419,8 +433,7 @@ class SamplingWindow:
                     from ..transformer import f32
                     h = t.empty(N, P, ca.width, dtype=t.float32, device=dev)
                     eng.prefill(N, P, tokens=self.tokens, y_cond=self.y_cond, x_cond=self.x_cond, h_out=h)
-                    if ca.add_cond_after_transformer and self.x_cond is not None:
-                        h = h + (self.x_cond[:, :P] if self.x_cond.shape[1] > 1 else self.x_cond)
+                    h = ca._add_x_cond(h, self.x_cond, 0, P)
                     if get_preds:
                         self.preds[:, :P] = f32.linear_nk(h.view(N * P, ca.width), ca.x_out.weight).view(N, P, ca.bins)
                     if get_logprobs:
@@ -518,8 +531,7 @@ class SamplingWindowF32:
                 self.tr.check_cache(N, sample_t, False)
                 h = f32.embed(ca, tokens, self.y_cond, self.x_cond, N, 1, sample_t)
                 h = self.tr(h, encoder_kv=self.encoder_kv, sample=True, fp16=False)
-                if ca.add_cond_after_transformer and self.x_cond is not None:
-                    h = h + (self.x_cond[:, sample_t:sample_t + 1] if self.x_cond.shape[1] > 1 else self.x_cond)
+                h = ca._add_x_cond(h, self.x_cond, sample_t, sample_t + 1)
                 if self.get_preds or self.get_logprobs or sample_t >= P:
                     x = f32.linear_nk(h.view(N, ca.width), ca.x_out.weight)
                     if self.get_preds:

@@ -291,6 +291,19 @@ class SimplePrior(nn.Module):
         logits = f32.linear_nk(encoder_kv.float().reshape(N * L, W), self.prime_x_out.weight)
         return F.cross_entropy(logits, prime_t.reshape(-1)) / float(np.log(2.))
 
+    def _condition(self, z, z_conds, y, fp16):
+        """one window of codes z [N, D] and what it is conditioned on: the upper-level codes and labels (get_cond), the
+        lyric tokens (with copy_input the window's own head), merged ahead of the codes for a single_enc_dec prior, else
+        turned into the lyric encoder's keys.  Returns (the token sequence self.prior reads, x_cond, y_cond, encoder_kv or
+        None, the lyric tokens, the length of the sequence's lyric head: prime_len for single_enc_dec, else 0)."""
+        x_cond, y_cond, lyric = self.get_cond(z_conds, y)
+        if self.copy_input:
+            lyric = z[:, :self.n_tokens]
+        if self.single_enc_dec:
+            seq, x_cond = self.prior_preprocess([lyric, z], [None, x_cond])
+            return seq, x_cond, y_cond, None, lyric, self.prior.prime_len
+        return z, x_cond, y_cond, self.get_encoder_kv(lyric, fp16=fp16), lyric, 0
+
     def z_forward(self, z, z_conds=[], y=None, fp16=False, get_preds=False, get_attn_weights=False):
         """Evaluation forward over one full window of codes (reference prior.py:312-349): returns (loss, metrics), or -
         with get_attn_weights (True or a set of layer indices) - the recorded attention weights of those layers, which
@@ -300,17 +313,13 @@ class SimplePrior(nn.Module):
         tr = self.prior.transformer
         if get_attn_weights:
             tr.set_record_attn(get_attn_weights)
-        x_cond, y_cond, lyric = self.get_cond(z_conds, y)
-        if self.copy_input:
-            lyric = z[:, :self.n_tokens]
+        seq, x_cond, y_cond, enc, lyric, _ = self._condition(z, z_conds, y, fp16)
         if self.single_enc_dec:
-            seq, x_cond = self.prior_preprocess([lyric, z], [None, x_cond])
             (prime_loss, gen_loss), preds = self.prior(seq, x_cond, y_cond, fp16=fp16, get_sep_loss=True,
                                                        get_preds=get_preds)
         else:
-            enc = self.get_encoder_kv(lyric, fp16=fp16)
             prime_loss = self.get_prime_loss(enc, lyric) if enc is not None else t.tensor(0.0, device=z.device)
-            gen_loss, preds = self.prior(z, x_cond, y_cond, enc, fp16=fp16, get_preds=get_preds)
+            gen_loss, preds = self.prior(seq, x_cond, y_cond, enc, fp16=fp16, get_preds=get_preds)
         if get_attn_weights:
             ws = tr.ws
             tr.set_record_attn(False)
@@ -332,16 +341,12 @@ class SimplePrior(nn.Module):
         from ..score import xout_logprob
         ln2 = float(np.log(2.))
         with t.no_grad():
-            x_cond, y_cond, lyric = self.get_cond(z_conds, y)
-            if self.copy_input:
-                lyric = z[:, :self.n_tokens]
+            seq, x_cond, y_cond, enc, lyric, pl = self._condition(z, z_conds, y, fp16)
+            logp = self.prior.logprob(seq, x_cond, y_cond, enc, fp16=fp16)
             if self.single_enc_dec:
-                seq, x_cond = self.prior_preprocess([lyric, z], [None, x_cond])
-                bits = -self.prior.logprob(seq, x_cond, y_cond, fp16=fp16) / ln2
-                pl = self.prior.prime_len
+                bits = -logp / ln2
                 return bits[:, pl:].mean(1), bits[:, :pl].mean(1)
-            enc = self.get_encoder_kv(lyric, fp16=fp16)
-            gen = -self.prior.logprob(z, x_cond, y_cond, enc, fp16=fp16).mean(1) / ln2
+            gen = -logp.mean(1) / ln2
             prime = None
             if enc is not None:
                 N, L, W = enc.shape
@@ -358,18 +363,13 @@ class SimplePrior(nn.Module):
         log-probability stays: the model put that mass there)."""
         from ..score import TokenStats
         with t.no_grad():
-            x_cond, y_cond, lyric = self.get_cond(z_conds, y)
-            if self.copy_input:
-                lyric = z[:, :self.n_tokens]
+            seq, x_cond, y_cond, enc, _, pl = self._condition(z, z_conds, y, fp16)
+            st = self.prior.token_stats(seq, x_cond, y_cond, enc, fp16=fp16, top_k=top_k)
             if not self.single_enc_dec:
-                enc = self.get_encoder_kv(lyric, fp16=fp16)
-                return self.prior.token_stats(z, x_cond, y_cond, enc, fp16=fp16, top_k=top_k)
-            seq, x_cond = self.prior_preprocess([lyric, z], [None, x_cond])
-            st = self.prior.token_stats(seq, x_cond, y_cond, fp16=fp16, top_k=top_k)
-            pl, shift = self.prior.prime_len, self.spaces.shift[-1]
+                return st
             st = TokenStats(*(None if v is None else v[:, pl:] for v in st))
             if top_k:
-                ids = st.topk_ids - shift
+                ids = st.topk_ids - self.spaces.shift[-1]
                 st = st._replace(topk_ids=t.where(ids >= 0, ids, t.full_like(ids, -1)))
             return st
 
@@ -380,15 +380,8 @@ class SimplePrior(nn.Module):
         its lyric head into the causal pass but keeps only the music positions; a separate lyric encoder gives the
         encoder-decoder layers their keys as in score."""
         with t.no_grad():
-            x_cond, y_cond, lyric = self.get_cond(z_conds, y)
-            if self.copy_input:
-                lyric = z[:, :self.n_tokens]
-            if self.single_enc_dec:
-                seq, x_cond = self.prior_preprocess([lyric, z], [None, x_cond])
-                return self.prior.layer_acts(seq, x_cond, y_cond, layers=layers, fp16=fp16, pool=pool,
-                                             t0=self.prior.prime_len)
-            enc = self.get_encoder_kv(lyric, fp16=fp16)
-            return self.prior.layer_acts(z, x_cond, y_cond, enc, layers=layers, fp16=fp16, pool=pool)
+            seq, x_cond, y_cond, enc, _, pl = self._condition(z, z_conds, y, fp16)
+            return self.prior.layer_acts(seq, x_cond, y_cond, enc, layers=layers, fp16=fp16, pool=pool, t0=pl)
 
     def forward(self, x, y=None, fp16=False, decode=False, get_preds=False):
         """audio -> codes of every level -> z_forward at this level (reference prior.py:351-359)"""

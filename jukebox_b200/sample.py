@@ -47,6 +47,16 @@ def plan_windows(have, total_length, n_ctx, hop_length):
     return [Window(have + total_length - n_ctx, n_ctx)]
 
 
+def window_pieces(prior, zs, labels, level, start, end, max_batch):
+    """the items of the window whose context is zs[level][:, start:end], in pieces of max_batch: (context, upper-level
+    codes of the window made contiguous or None, labels or None) per piece, with the window's get_z_conds / get_y"""
+    z = zs[level]
+    pieces = lambda v: split_batch(v, z.shape[0], max_batch)
+    upper = prior.get_z_conds(zs, start, start + prior.n_ctx)
+    for ctx_i, upper_i, y_i in zip(pieces(z[:, start:end]), pieces(upper), pieces(prior.get_y(labels, start))):
+        yield ctx_i, None if upper_i is None else [u.contiguous() for u in upper_i], y_i
+
+
 class LevelRun:
     """One level of one sampling job: the codes sampled so far and what is needed to extend them."""
 
@@ -61,7 +71,7 @@ class LevelRun:
         return self.zs[self.level].shape[1]
 
     def run_window(self, win):
-        prior, level, n = self.prior, self.level, self.hps.n_samples
+        prior, level = self.prior, self.level
         context = self.zs[level][:, win.start:win.start + prior.n_ctx]
         given = context.shape[1]
         missing = win.sample_tokens - given
@@ -69,16 +79,10 @@ class LevelRun:
                    f"Conditioning on {given} tokens")
         if missing <= 0:
             return
-        upper = prior.get_z_conds(self.zs, win.start, win.start + prior.n_ctx)
-        y = prior.get_y(self.labels, win.start)
         extra = {} if win.sample_tokens == prior.n_ctx else dict(sample_tokens=win.sample_tokens)
-        pieces = zip(split_batch(context, n, self.max_batch), split_batch(upper, n, self.max_batch),
-                     split_batch(y, n, self.max_batch))
-        done = []
-        for ctx_i, upper_i, y_i in pieces:
-            if upper_i is not None:
-                upper_i = [u.contiguous() for u in upper_i]
-            done.append(prior.sample(n_samples=ctx_i.shape[0], z=ctx_i, z_conds=upper_i, y=y_i, **self.opts, **extra))
+        done = [prior.sample(n_samples=ctx_i.shape[0], z=ctx_i, z_conds=upper_i, y=y_i, **self.opts, **extra)
+                for ctx_i, upper_i, y_i in window_pieces(prior, self.zs, self.labels, level, win.start,
+                                                         win.start + prior.n_ctx, self.max_batch)]
         fresh = t.cat(done, dim=0)[:, -missing:]
         self.zs[level] = t.cat([self.zs[level], fresh], dim=1)
 
@@ -114,16 +118,8 @@ def song_token_stats(prior, zs, labels, level, hop_length, fp16=True, top_k=0, m
     N, T = z.shape
     cols = []
     for win, t0, t1 in song_windows(T, prior.n_ctx, hop_length):
-        context = z[:, win.start:t1]
-        upper = prior.get_z_conds(zs, win.start, win.start + prior.n_ctx)
-        y = prior.get_y(labels, win.start)
-        pieces = zip(split_batch(context, N, max_batch_size), split_batch(upper, N, max_batch_size),
-                     split_batch(y, N, max_batch_size))
-        done = []
-        for ctx_i, upper_i, y_i in pieces:
-            if upper_i is not None:
-                upper_i = [u.contiguous() for u in upper_i]
-            done.append(prior.token_stats(ctx_i.contiguous(), upper_i, y_i, fp16=fp16, top_k=top_k))
+        done = [prior.token_stats(ctx_i.contiguous(), upper_i, y_i, fp16=fp16, top_k=top_k)
+                for ctx_i, upper_i, y_i in window_pieces(prior, zs, labels, level, win.start, t1, max_batch_size)]
         cols.append(TokenStats(*(None if v[0] is None else t.cat(v, dim=0)[:, t0 - win.start:] for v in zip(*done))))
     if not cols:
         e = t.empty(N, 0, device=z.device)

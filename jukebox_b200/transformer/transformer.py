@@ -219,7 +219,7 @@ class Transformer(nn.Module):
             return {l: (o.half() if fp16_out else o) for l, o in outs.items()}
         if not sample or not fp16:
             # forward mode over activations (any fp16 flag: computed in fp32, a superset of the reference's fp16
-            # precision; the fp16 prefill starts from tokens, ConditionalAutoregressive2D._acts_fp16) and fp32 sampling:
+            # precision; the fp16 prefill starts from tokens, ConditionalAutoregressive2D._prefill) and fp32 sampling:
             # csrc/f32_path.cu
             out = self._forward_f32(x, encoder_kv, sample)
             return out.half() if fp16_out else out

@@ -178,7 +178,7 @@ def test_recording_leaves_the_forward_pass_unchanged(tag):
 
 
 @pytest.mark.parametrize("tag", ["single_enc_dec", "sep_enc_dec"])
-def test_batched_alignment_windows_equal_item_by_item(tag, monkeypatch):
+def test_batched_alignment_windows_per_prefill_equal_item_by_item(tag, monkeypatch):
     from jukebox_b200 import align
     fx = Fixture(f"align_{tag}")
     prior = _make_prior(fx)
@@ -186,10 +186,10 @@ def test_batched_alignment_windows_equal_item_by_item(tag, monkeypatch):
     z, y = torch.from_numpy(fx["z"]).cuda(), torch.from_numpy(fx["y"]).cuda()
     z = torch.cat([z, z.flip(1), (z + 1) % prior.l_bins])          # 6 items
     y = torch.cat([y, y, y.flip(0)])
-    assert align.items_per_pass(prior, z.shape[0], True) == z.shape[0]
+    assert prior.prior.items_per_prefill(z.shape[0]) == z.shape[0]
     batched = align.hop_weights(prior, z, y, True)
     w32 = align.hop_weights(prior, z, y, False)
-    monkeypatch.setattr(align, "items_per_pass", lambda prior, bs, fp16: 1)
+    monkeypatch.setattr(prior.prior, "items_per_prefill", lambda N: 1)
     single = align.hop_weights(prior, z, y, True)
     assert batched.shape == single.shape == w32.shape == (z.shape[0], prior.n_ctx, prior.n_tokens)
     assert np.array_equal(batched, single)

@@ -218,3 +218,24 @@ def test_score_matches_z_forward(tag, fp16):
         msg += f", prime bits rel {rp:.1e}"
         assert rp <= 1e-5, msg
     print(msg)
+
+
+def test_logprob_of_more_items_than_a_16_row_engine_takes():
+    """20 items on a stack of 5b_lyrics' width, heads and m_attn, whose engines take at most 16 rows (jk_prior_plan at
+    132 SMs: K split 1, so a 32-row activation tile does not fit in shared memory): logprob and token_stats score them
+    in pieces of 16 and 4, bit for bit the items scored 16 at a time"""
+    from jukebox_b200.prior.autoregressive import ConditionalAutoregressive2D
+    torch.manual_seed(0)
+    with torch.device("cuda"):
+        m = ConditionalAutoregressive2D((64,), 256, width=4800, depth=2, heads=8, attn_order=0, blocks=8,
+                                        init_scale=0.1).eval()
+    assert m.items_per_prefill(20) == 16
+    g = torch.Generator(device="cuda").manual_seed(2)
+    x = torch.randint(0, 256, (20, 64), device="cuda", generator=g)
+    lp = m.logprob(x)
+    assert lp.shape == (20, 64) and bool(torch.isfinite(lp).all())
+    assert torch.equal(lp, torch.cat([m.logprob(x[:16]), m.logprob(x[16:])]))
+    st = m.token_stats(x[:, :40], top_k=4)
+    for a, b0, b1 in zip(st, m.token_stats(x[:16, :40], top_k=4), m.token_stats(x[16:, :40], top_k=4)):
+        assert torch.equal(a, torch.cat([b0, b1]))
+    assert m.transformer._engine.max_batch == 16

@@ -230,3 +230,25 @@ def test_song_token_stats_matches_the_sampler():
         one = prior.token_stats(zs[0][:, win.start:t1].contiguous(), [u.contiguous() for u in upper], None, top_k=4)
         for a, b in zip(one, whole):
             assert torch.equal(a[:, t0 - win.start:], b[:, t0:t1])
+
+
+@pytest.mark.parametrize("tag", ["single_enc_dec", "upsampler"])
+def test_fp32_token_stats_of_a_prefix_are_the_full_windows(tag):
+    """token_stats(fp16=False) of a causal prefix of D codes: the first D positions of the fp32 full window, within the
+    fp32 path's summation-order noise (tests/test_gpu_acts.py: 2e-5 of the activations' range; a log-probability moves
+    by at most twice a logit's error)"""
+    fx = Fixture(f"prior_{tag}")
+    prior = _make_prior(fx)
+    y = torch.from_numpy(fx["y"]).cuda() if "y" in fx else None
+    z_conds = [torch.from_numpy(fx["z_cond"]).cuda()] if "z_cond" in fx else []
+    tokens = torch.from_numpy(fx["tokens"]).cuda()
+    z = prior.prior_postprocess(tokens) if prior.single_enc_dec else tokens
+    full = prior.token_stats(z, z_conds, y, fp16=False, top_k=4)
+    D = 40
+    short = prior.token_stats(z[:, :D].contiguous(), z_conds, y, fp16=False, top_k=4)
+    assert short.logp.shape == (z.shape[0], D) and short.topk_ids.shape == (z.shape[0], D, 4)
+    for name in ("logp", "entropy", "lse", "topk_logp"):
+        a, b = getattr(short, name), getattr(full, name)[:, :D]
+        d = float((a - b).abs().max())
+        print(f"prior_{tag} fp32 prefix of {D}: |d {name}| {d:.2e}")
+        assert d <= 4e-5 * max(1.0, float(b.abs().max())), (name, d)

@@ -81,7 +81,7 @@ def test_oracle_entropy_and_topk():
 
 
 # ---- host flow -----------------------------------------------------------------------------------------------------
-def test_token_stats_shares_logprob_activations(monkeypatch):
+def test_token_stats_shares_logprob_prefill(monkeypatch):
     """token_stats and logprob read the same activations (one helper); a prefix reads the first D rows of x_cond"""
     import jukebox_b200.prior.autoregressive as ar
     import jukebox_b200.score as score
@@ -89,9 +89,9 @@ def test_token_stats_shares_logprob_activations(monkeypatch):
                                        x_cond=True, y_cond=True).eval()
     seen = []
 
-    def fake_acts(x, x_cond, y_cond, encoder_kv):
+    def fake_prefill(x, x_cond, y_cond, encoder_kv, h_out=None, **kw):
         seen.append((tuple(x.shape), tuple(x_cond.shape)))
-        return torch.arange(x.shape[1], dtype=torch.float)[None, :, None].expand(x.shape[0], x.shape[1], 64).clone()
+        h_out.copy_(torch.arange(x.shape[1], dtype=torch.float)[None, :, None].expand(x.shape[0], x.shape[1], 64))
     got = {}
 
     def fake_stats(h, w, targets=None, top_k=0):
@@ -103,7 +103,7 @@ def test_token_stats_shares_logprob_activations(monkeypatch):
     def fake_logprob(h, w, targets):
         got["h_lp"] = h.clone()
         return torch.zeros(h.shape[0])
-    monkeypatch.setattr(m, "_acts_fp16", fake_acts)
+    monkeypatch.setattr(m, "_prefill", fake_prefill)
     monkeypatch.setattr(score, "xout_stats", fake_stats)
     monkeypatch.setattr(score, "xout_logprob", fake_logprob)
     x = torch.randint(0, 16, (2, 24))

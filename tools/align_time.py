@@ -7,9 +7,9 @@ Geometry: the top-level priors of 1b_lyrics and 5b_lyrics at their full width, h
 synthetic weights (bench.synth_fill, the scale rules of oracle/synth.py).  The stacks are cut to the first layers that
 contain a layer of the alignment layer's kind (1b_lyrics: 16 layers, layer 15 is a prime layer like layer 63; 5b_lyrics:
 19 layers, layer 18 is an encoder-decoder layer like layer 68), so that the fp32 route fits a short run; the time per
-layer is reported beside the window time.  The fp16 route runs the window's items in one z_forward call
-(align.items_per_pass), the fp32 route item by item, as get_alignment does.  Prints one JSON line per (model, route)
-and the GPU's name and power limit.
+layer is reported beside the window time.  The fp16 route runs the window's items in one z_forward call (as many as
+one prefill takes), the fp32 route item by item, as get_alignment does.  Prints one JSON line per (model, route) and
+the GPU's name and power limit.
 """
 import argparse
 import json
@@ -96,9 +96,9 @@ def main():
                 if m is not None:
                     m.transformer.drop_engine()                # free the route's engines / fp32 state before the next
             torch.cuda.empty_cache()
-            r = dict(model=wl, route="fp16" if fp16 else "fp32", items=a.items,
-                     items_per_call=align.items_per_pass(prior, a.items, fp16), engine_batch=eng_batch,
-                     n_ctx=prior.n_ctx, layers=depth,
+            per_call = (prior.prior.items_per_prefill(a.items) or 1) if fp16 else 1
+            r = dict(model=wl, route="fp16" if fp16 else "fp32", items=a.items, items_per_call=per_call,
+                     engine_batch=eng_batch, n_ctx=prior.n_ctx, layers=depth,
                      recorded_layer=layer, attn_func=tr._attn_mods[layer].attn_func, window_s=round(s, 4),
                      per_layer_ms=round(1e3 * s / depth, 2), gpu=gpu)
             print(json.dumps(r), flush=True)
