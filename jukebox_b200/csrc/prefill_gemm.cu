@@ -16,7 +16,7 @@
 // W is supplied transposed ([N, K], K contiguous) - the engine packs it once at weight load - so both
 // operands are K-major, the layout wgmma reads without a transpose bit.
 #include "engine.cuh"
-#include <cuda.h>
+#include "split_tma.cuh"
 
 using namespace jk;
 
@@ -26,14 +26,6 @@ constexpr int BM = 128, BN = 128, BK = 64, STAGES = 3;   // 3 x 32 KB: two CTAs 
 constexpr int kTileBytes = BM * BK * 2;                  // 16 KB per operand tile
 constexpr int kGemmThreads = 288;                        // two consumer warpgroups + one producer warp
 constexpr int kGemmSmem = STAGES * 2 * kTileBytes + 1024 + 256;
-
-__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-            smem_u32(smem_dst)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-        : "memory");
-}
 
 // The decode kernel's epilogues (decode_engine.cu gemm_phase), same fp16 rounding points:
 //   0  Conv1D output rounded once from the fp32 accumulator           (ops.py:83-96)
@@ -123,35 +115,13 @@ prefill_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
     }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(p);
-    }
-    return fn;
-}
-
 // 2-D fp16 row-major [rows, K] tensor, box = [128 rows x 64 columns], 128-byte swizzle, zero fill out of bounds
 int make_map(CUtensorMap* map, const void* base, int rows, int K) {
-    EncodeTiledFn enc = get_encode();
-    JK_REQUIRE(enc, "cuTensorMapEncodeTiled is not available from the driver");
-    cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)K * 2};
-    cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)BM};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    JK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for a [%d, %d] fp16 tensor", (int)r, rows, K);
-    return 0;
+    const cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
+    const cuuint64_t strides[1] = {(cuuint64_t)K * 2};
+    const cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)BM};
+    return encode_tensor_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, base, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                             CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
 
 }  // namespace

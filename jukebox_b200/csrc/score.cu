@@ -2,11 +2,11 @@
 //
 //   logp[m] = z[m, target[m]] - log sum_b exp(z[m, b]),   z = h . x_out^T  (prior/autoregressive.py: x_out, no bias)
 //
-// without the [M, bins] logits ever reaching HBM.  The product is the split-precision one of conv_wide_kernel
-// (vqvae_t5.cu): hi.w_hi + hi.w_lo + lo.w_hi of fp16 halves (22 significant bits per operand), x_out scaled by 2^8
-// before its split so that the weight remainders stay normal, warpgroup MMAs with fp32 accumulation, and every 64-wide
-// K block's partial promoted into an fp32 register sum with ordinary adds (the tensor core's own accumulation alone
-// drifts to ~2e-5 of the output scale over long K).
+// without the [M, bins] logits ever reaching HBM.  The head kernel runs conv_wide_kernel's streamed-weight pipeline
+// (streamed_pipeline, split_tma.cuh) with its own loads and epilogue (HeadJob): hi.w_hi + hi.w_lo + lo.w_hi of fp16
+// halves (22 significant bits per operand), x_out scaled by 2^8 before its split so that the weight remainders stay
+// normal, warpgroup MMAs with fp32 accumulation, and every 64-wide K block's partial promoted into an fp32 register sum
+// with ordinary adds (the tensor core's own accumulation alone drifts to ~2e-5 of the output scale over long K).
 //
 // Work items are (128 rows x 128 bins) tiles, numbered row-tile major so that the CTAs working on the bin tiles of one
 // row tile at the same time share its activation rows in L2.  One persistent CTA per SM, four roles over mbarriers:
@@ -32,14 +32,7 @@ using namespace jk;
 
 namespace {
 
-constexpr int kBM = 128, kBN = 128, kBK = 64, kS = 3, kScoreThreads = 512;
-constexpr float kF16Max = 65504.f;
-constexpr int kA = kBM * kBK * 4;                 // fp32 activation block; after conversion hi plane | lo plane
-constexpr int kAPlane = kBM * 128;
-constexpr int kB = kBN * 128;                     // one weight plane: 128 bins x 64 fp16
-constexpr int kStage = kA + 2 * kB;
-constexpr int kOffBar = kS * kStage;
-constexpr int kSmem = kOffBar + 128 + 1024;       // barriers, and slack to align the ring to 1024 bytes
+constexpr int kBN = 128, kBK = 64, kS = 3;
 constexpr int kWsHead = 256;                      // workspace: status word, then the pairs, the target logits, a pad
 
 struct ScoreP {
@@ -57,33 +50,6 @@ struct StatsP {
     int* topi;                                    // [M][n_bt][k] their bins (ties: lower bin first; -1 past the tile)
     int k;
 };
-
-// fp32 block [128][64] at st -> hi plane at st, lo plane at st + 16 KB (128 converter threads); false if a value lies
-// outside the fp16 range
-__device__ __forceinline__ bool convert_block(uint8_t* st, int ct) {
-    constexpr int CH = 16, PER = kBM * CH / 128;
-    const float4* f = reinterpret_cast<const float4*>(st);
-    float4 v[PER];
-#pragma unroll
-    for (int j = 0; j < PER; ++j) v[j] = f[ct + j * 128];
-    uint2 h[PER], l[PER];
-    bool ok = true;
-#pragma unroll
-    for (int j = 0; j < PER; ++j) {
-        ok &= fabsf(v[j].x) <= kF16Max && fabsf(v[j].y) <= kF16Max && fabsf(v[j].z) <= kF16Max && fabsf(v[j].w) <= kF16Max;
-        split_f16x2(v[j].x, v[j].y, h[j].x, l[j].x);
-        split_f16x2(v[j].z, v[j].w, h[j].y, l[j].y);
-    }
-    named_sync(1);
-#pragma unroll
-    for (int j = 0; j < PER; ++j) {
-        const int item = ct + j * 128, r = item / CH, c4 = item % CH;
-        const uint32_t o = sw_off(r, c4 >> 1) + (c4 & 1) * 8;
-        *reinterpret_cast<uint2*>(st + o) = h[j];
-        *reinterpret_cast<uint2*>(st + kAPlane + o) = l[j];
-    }
-    return ok;
-}
 
 // the k largest logits of one row of a tile (the four lanes of a quad, columns c0 + 8 i + e of acc[4 i + 2 h + e]) by
 // k rounds of argmax over what is not yet taken, ties to the lower bin; lane 0 of the quad writes them
@@ -120,136 +86,84 @@ __device__ __forceinline__ void tile_topk(const float (&acc)[kBN / 2], int h, co
     }
 }
 
+// the head on the streamed-weight pipeline (split_tma.cuh): an item is (128 rows x 128 bins), a K block the fp32
+// activations [128 x 64] and the hi / lo x_out rows [128 x 64] of its bin tile
 template <bool kStats>
-__global__ void __launch_bounds__(kScoreThreads, 1)
+struct HeadJob {
+    using Ring = StreamRing<kBN, kS>;                        // 3 stages of 64 KB
+    static constexpr bool kCheck = true, relu = false;
+    const CUtensorMap *map_a, *map_w;                        // activations [rows, W] fp32, the split x_out
+    ScoreP P;
+    StatsP S;
+    int n_kb, bins_pad;
+    struct Tile { int mt, bt; };
+
+    __device__ __forceinline__ unsigned* status() const { return P.status; }
+
+    __device__ __forceinline__ Tile tile(int item) const {
+        const int mt = item / P.n_bt, bt = item - mt * P.n_bt;
+        return {mt, bt};
+    }
+    __device__ __forceinline__ void load(uint8_t* st, const Tile& t, int kb, uint64_t* bar) const {
+        tma_load_2d(st, map_a, kb * kBK, t.mt * kBM, bar);          // rows >= M arrive as zeros
+        tma_load_2d(st + Ring::kA, map_w, kb * kBK, t.bt * kBN, bar);
+        tma_load_2d(st + Ring::kA + Ring::kB, map_w, kb * kBK, bins_pad + t.bt * kBN, bar);
+    }
+    // ---- per row: (max, sum exp) over this tile's bins, and the target's logit where it falls here.  The four lanes of
+    // a quad hold the tile's 128 columns of two rows (d[4 i + 2 h + e]: row + 8 h, column 8 i + 2 (lane % 4) + e); they
+    // combine in a fixed shuffle order ----
+    __device__ __forceinline__ void epilogue(const float (&acc)[kBN / 2], const Tile& t, int rq, int lane) const {
+        const int c0 = t.bt * kBN + 2 * (lane & 3);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int r = t.mt * kBM + rq + 8 * h;
+            float mx = -INFINITY;
+#pragma unroll
+            for (int i = 0; i < kBN / 8; ++i)
+#pragma unroll
+                for (int e = 0; e < 2; ++e)
+                    if (c0 + 8 * i + e < P.bins) mx = fmaxf(mx, acc[4 * i + 2 * h + e] * kWInv);
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            const long long tg = r < P.M && (!kStats || P.targets) ? __ldg(P.targets + r) : -1;
+            float se = 0.f, u = 0.f;
+#pragma unroll
+            for (int i = 0; i < kBN / 8; ++i)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int col = c0 + 8 * i + e;
+                    if (col < P.bins) {
+                        const float z = acc[4 * i + 2 * h + e] * kWInv;
+                        if constexpr (kStats) {
+                            const float ex = expf(z - mx);
+                            se += ex;
+                            u += (z - mx) * ex;
+                        } else {
+                            se += expf(z - mx);
+                        }
+                        if (col == tg) P.tlogit[r] = z;
+                    }
+                }
+            se += __shfl_xor_sync(0xffffffffu, se, 1);
+            se += __shfl_xor_sync(0xffffffffu, se, 2);
+            if ((lane & 3) == 0 && r < P.M) P.part[(size_t)r * P.n_bt + t.bt] = make_float2(mx, se);
+            if constexpr (kStats) {
+                u += __shfl_xor_sync(0xffffffffu, u, 1);
+                u += __shfl_xor_sync(0xffffffffu, u, 2);
+                if ((lane & 3) == 0 && r < P.M) S.u[(size_t)r * P.n_bt + t.bt] = u;
+                if (S.k) tile_topk(acc, h, P, S, r, t.bt, c0, lane);
+            }
+        }
+    }
+};
+
+template <bool kStats>
+__global__ void __launch_bounds__(kStreamThreads, 1)
 xout_head_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_w, ScoreP P,
                  StatsP S, int total_items) {
     extern __shared__ __align__(1024) uint8_t sm_raw[];
-    uint8_t* sm = sm_raw + ((1024u - (smem_u32(sm_raw) & 1023u)) & 1023u);   // TMA's 128-byte swizzle needs 1024-byte stages
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sm + kOffBar);
-    uint64_t *full = bars, *conv = bars + kS, *empty = bars + 2 * kS;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    if (tid == 0) {
-        for (int i = 0; i < kS; ++i) { mbar_init(&full[i], 1); mbar_init(&conv[i], 128); mbar_init(&empty[i], 2); }
-        mbar_fence_init();
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_h)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_w)) : "memory");
-    }
-    __syncthreads();
-    const int first = blockIdx.x, stride = gridDim.x, bins_pad = P.n_bt * kBN;
-
-    // register reallocation as in conv_wide_kernel: 2 x 128 x 184 + 128 x 104 + 128 x 40 = 65536
-    if (warp >= 12) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-        if (warp == 12 && lane == 0) {
-            uint32_t kt = 0;
-            for (int item = first; item < total_items; item += stride) {
-                const int mt = item / P.n_bt, bt = item - mt * P.n_bt;
-                for (int kb = 0; kb < P.n_kb; ++kb, ++kt) {
-                    const int s = kt % kS;
-                    mbar_wait(&empty[s], ((kt / kS) & 1) ^ 1);
-                    mbar_expect_tx(&full[s], (uint32_t)kStage);
-                    uint8_t* st = sm + s * kStage;
-                    tma_load_2d(st, &map_h, kb * kBK, mt * kBM, &full[s]);          // rows >= M arrive as zeros
-                    tma_load_2d(st + kA, &map_w, kb * kBK, bt * kBN, &full[s]);
-                    tma_load_2d(st + kA + kB, &map_w, kb * kBK, bins_pad + bt * kBN, &full[s]);
-                }
-            }
-        }
-    } else if (warp >= 8) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 104;");
-        const int ct = tid & 127;
-        bool ok = true;
-        uint32_t kt = 0;
-        for (int item = first; item < total_items; item += stride) {
-            for (int kb = 0; kb < P.n_kb; ++kb, ++kt) {
-                const int s = kt % kS;
-                mbar_wait(&full[s], (kt / kS) & 1);
-                ok &= convert_block(sm + s * kStage, ct);
-                fence_async_smem();                   // the planes are read by the tensor core (async proxy)
-                mbar_arrive(&conv[s]);
-            }
-        }
-        if (!ok) atomicOr(P.status, 1u);
-    } else {
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 184;");
-        const int wg = warp >> 2, wt = tid & 127, rq = wg * 64 + (wt >> 5) * 16 + (lane >> 2);
-        const uint32_t ring = smem_u32(sm);
-        uint32_t kt = 0;
-        for (int item = first; item < total_items; item += stride) {
-            const int mt = item / P.n_bt, bt = item - mt * P.n_bt;
-            float acc[kBN / 2];
-#pragma unroll
-            for (int i = 0; i < kBN / 2; ++i) acc[i] = 0.f;
-            for (int kb = 0; kb < P.n_kb; ++kb, ++kt) {
-                const int s = kt % kS;
-                const uint32_t ph = (kt / kS) & 1;
-                mbar_wait(&full[s], ph);              // weight planes (TMA)
-                mbar_wait(&conv[s], ph);              // activation planes (converters)
-                const uint32_t st = ring + s * kStage, ah = st + wg * (64 * 128), al = ah + kAPlane;
-                const uint32_t bh = st + kA, bl = bh + kB;
-                float part[kBN / 2];
-#pragma unroll
-                for (int i = 0; i < kBN / 2; ++i) part[i] = 0.f;
-                wgmma_fence();
-#pragma unroll
-                for (int k = 0; k < kBK / 16; ++k) {
-                    wgmma_ss<kBN>(part, wgmma_desc_sw128(al + k * 32), wgmma_desc_sw128(bh + k * 32));
-                    wgmma_ss<kBN>(part, wgmma_desc_sw128(ah + k * 32), wgmma_desc_sw128(bl + k * 32));
-                    wgmma_ss<kBN>(part, wgmma_desc_sw128(ah + k * 32), wgmma_desc_sw128(bh + k * 32));
-                }
-                wgmma_commit();
-                wgmma_wait<0>();
-                if (wt == 0) mbar_arrive(&empty[s]);  // the block has retired: free its stage
-#pragma unroll
-                for (int i = 0; i < kBN / 2; ++i) acc[i] += part[i];
-            }
-            // ---- per row: (max, sum exp) over this tile's bins, and the target's logit where it falls here.  The
-            // four lanes of a quad hold the tile's 128 columns of two rows (d[4 i + 2 h + e]: row + 8 h, column
-            // 8 i + 2 (lane % 4) + e); they combine in a fixed shuffle order ----
-            const int c0 = bt * kBN + 2 * (lane & 3);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int r = mt * kBM + rq + 8 * h;
-                float mx = -INFINITY;
-#pragma unroll
-                for (int i = 0; i < kBN / 8; ++i)
-#pragma unroll
-                    for (int e = 0; e < 2; ++e)
-                        if (c0 + 8 * i + e < P.bins) mx = fmaxf(mx, acc[4 * i + 2 * h + e] * kWInv);
-                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-                const long long tg = r < P.M && (!kStats || P.targets) ? __ldg(P.targets + r) : -1;
-                float se = 0.f, u = 0.f;
-#pragma unroll
-                for (int i = 0; i < kBN / 8; ++i)
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int col = c0 + 8 * i + e;
-                        if (col < P.bins) {
-                            const float z = acc[4 * i + 2 * h + e] * kWInv;
-                            if constexpr (kStats) {
-                                const float ex = expf(z - mx);
-                                se += ex;
-                                u += (z - mx) * ex;
-                            } else {
-                                se += expf(z - mx);
-                            }
-                            if (col == tg) P.tlogit[r] = z;
-                        }
-                    }
-                se += __shfl_xor_sync(0xffffffffu, se, 1);
-                se += __shfl_xor_sync(0xffffffffu, se, 2);
-                if ((lane & 3) == 0 && r < P.M) P.part[(size_t)r * P.n_bt + bt] = make_float2(mx, se);
-                if constexpr (kStats) {
-                    u += __shfl_xor_sync(0xffffffffu, u, 1);
-                    u += __shfl_xor_sync(0xffffffffu, u, 2);
-                    if ((lane & 3) == 0 && r < P.M) S.u[(size_t)r * P.n_bt + bt] = u;
-                    if (S.k) tile_topk(acc, h, P, S, r, bt, c0, lane);
-                }
-            }
-        }
-    }
+    const HeadJob<kStats> job{&map_h, &map_w, P, S, P.n_kb, P.n_bt * kBN};
+    streamed_pipeline(job, sm_raw, total_items);
 }
 
 // one thread per row: the row's pairs in bin-tile order -> lse, logp.  Status bit 0: an activation outside the fp16
@@ -379,6 +293,7 @@ int read_status(const unsigned* status, unsigned* out, cudaStream_t stream) {
 template <bool kStats>
 int launch_head(const float* h, int m, int width, const void* w_split, int bins, const int64_t* targets, char* ws,
                 size_t need, ScoreP& P, const StatsP& S, cudaStream_t stream) {
+    constexpr int kSmem = HeadJob<kStats>::Ring::smem;
     const int n_bt = n_bin_tiles(bins), bins_pad = n_bt * kBN;
     const long long total = (long long)((m + kBM - 1) / kBM) * n_bt;
     JK_REQUIRE(total < (1ll << 31), "too many rows");
@@ -399,35 +314,28 @@ int launch_head(const float* h, int m, int width, const void* w_split, int bins,
         hsrc = pad;
         rows = kBM;
     }
-    EncodeTiledFnT5 enc = t5_encode();
-    JK_REQUIRE(enc, "cuTensorMapEncodeTiled is not available from the driver");
     CUtensorMap map_h, map_w;
     {
-        cuuint64_t dims[2] = {(cuuint64_t)width, (cuuint64_t)rows};
-        cuuint64_t strides[1] = {(cuuint64_t)width * 4};
-        cuuint32_t box[2] = {kBK, kBM};
-        cuuint32_t estr[2] = {1, 1};
-        CUresult r = enc(&map_h, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(hsrc), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        JK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for [%d, %d] fp32 activations", (int)r, m, width);
+        const cuuint64_t dims[2] = {(cuuint64_t)width, (cuuint64_t)rows};
+        const cuuint64_t strides[1] = {(cuuint64_t)width * 4};
+        const cuuint32_t box[2] = {kBK, kBM};
+        if (int rc = encode_tensor_map(&map_h, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, hsrc, dims, strides, box,
+                                       CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
+            return rc;
     }
     {
-        cuuint64_t dims[2] = {(cuuint64_t)width, (cuuint64_t)2 * bins_pad};
-        cuuint64_t strides[1] = {(cuuint64_t)width * 2};
-        cuuint32_t box[2] = {kBK, kBN};
-        cuuint32_t estr[2] = {1, 1};
-        CUresult r = enc(&map_w, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(w_split), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        JK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for the [2 x %d, %d] fp16 split x_out", (int)r,
-                   bins_pad, width);
+        const cuuint64_t dims[2] = {(cuuint64_t)width, (cuuint64_t)2 * bins_pad};
+        const cuuint64_t strides[1] = {(cuuint64_t)width * 2};
+        const cuuint32_t box[2] = {kBK, kBN};
+        if (int rc = encode_tensor_map(&map_w, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, w_split, dims, strides, box,
+                                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
+            return rc;
     }
     int sms = 0;
     if (int rc = set_max_smem_once<xout_head_kernel<kStats>>(kSmem)) return rc;
     if (int rc = sm_count(&sms)) return rc;
     const unsigned grid = (unsigned)std::min<long long>(total, sms);
-    xout_head_kernel<kStats><<<grid, kScoreThreads, kSmem, stream>>>(map_h, map_w, P, S, (int)total);
+    xout_head_kernel<kStats><<<grid, kStreamThreads, kSmem, stream>>>(map_h, map_w, P, S, (int)total);
     JK_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -7,7 +7,8 @@
 // 22 significant bits) accumulated in fp32 - but the MMAs are warpgroup MMAs (wgmma m64nCk16) reading both operands
 // from swizzled shared memory, where mma.sync needs a ldmatrix per fragment and leaves the legacy tensor path saturated.
 //
-// One persistent CTA per SM walks tiles of 128 positions; three roles, connected by mbarriers only:
+// One persistent CTA per SM walks tiles of 128 positions; three roles, connected by mbarriers only.  The tap pipeline
+// below (tap_producer, tap_converter, tap_accumulate) is shared with conv_t5_kernel:
 //   last warp   TMA producer   cp.async.bulk.tensor.3d of the fp32 rows of one tap, [128 rows x C] of clip n starting at
 //                              t0 + (tap - 1) * dilation, into a ring.  Rows outside [0, T) arrive as zeros (the tensor
 //                              map's out-of-bounds fill IS the convolution's zero padding).
@@ -26,8 +27,6 @@
 using namespace jk;
 
 namespace {
-
-constexpr int kBM = 128;                  // positions per tile = two wgmma M blocks of 64
 
 template <int C>
 struct T5 {
@@ -48,13 +47,6 @@ struct T5 {
     static constexpr int smem = offBar + 256;
 };
 
-__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
-            smem_u32(smem_dst)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
 // scale * (acc / 2^8 + bias) of one consumer warpgroup's 64 rows -> stage[row][C], 16-byte chunks XOR-swizzled with row & 7
 template <int C>
 __device__ __forceinline__ void stage_rows(float* stage, const float (&acc)[C / 2], const float* bias, float scale, int row0, int lane) {
@@ -68,41 +60,105 @@ __device__ __forceinline__ void stage_rows(float* stage, const float (&acc)[C / 
     }
 }
 
-// fp32 tap tile -> (relu) -> hi / lo planes of operand slot s: one converter group of 128 threads (ct = 0..127)
-template <int C>
-__device__ __forceinline__ void convert_tap(const uint8_t* fsrc, uint8_t* ah, int a_tile, int ct, bool relu) {
-    constexpr int CH = C / 4, PER = kBM * CH / 128;         // float4 chunks per row, items per thread
-    const float4* f = reinterpret_cast<const float4*>(fsrc);
-    float4 v[PER];
-#pragma unroll
-    for (int j = 0; j < PER; ++j) v[j] = f[ct + j * 128];
-    uint2 h[PER], l[PER];
-#pragma unroll
-    for (int j = 0; j < PER; ++j) {
-        if (relu) { v[j].x = fmaxf(v[j].x, 0.f); v[j].y = fmaxf(v[j].y, 0.f); v[j].z = fmaxf(v[j].z, 0.f); v[j].w = fmaxf(v[j].w, 0.f); }
-        split_f16x2(v[j].x, v[j].y, h[j].x, l[j].x);
-        split_f16x2(v[j].z, v[j].w, h[j].y, l[j].y);
-    }
-#pragma unroll
-    for (int j = 0; j < PER; ++j) {
-        const int item = ct + j * 128, r = item / CH, c4 = item % CH;
-        const uint32_t o = sw_off(r, c4 >> 1) + (c4 & 1) * 8;
-        *reinterpret_cast<uint2*>(ah + o) = h[j];
-        *reinterpret_cast<uint2*>(ah + a_tile + o) = l[j];
+// ---- the tap pipeline -----------------------------------------------------------------
+// Barriers at bars: f_full[4] | f_empty[4] (fp32 ring, FS of them used) | a_full[2] | a_empty[2] (operand slots).
+template <int FS>
+__device__ __forceinline__ void tap_init(uint64_t* bars, const CUtensorMap* map) {
+    uint64_t *f_full = bars, *f_empty = bars + 4, *a_full = bars + 8, *a_empty = bars + 10;
+    for (int i = 0; i < FS; ++i) { mbar_init(&f_full[i], 1); mbar_init(&f_empty[i], 128); }
+    for (int i = 0; i < 2; ++i) { mbar_init(&a_full[i], 128); mbar_init(&a_empty[i], 2); }   // a_empty: one arrival per warpgroup
+    mbar_fence_init();
+    prefetch_tensormap(map);
+}
+
+// w[(tap * CI + ci) * CO + co] (n = taps * CI * CO values) -> 2^8 w split into the planes hi / lo [tap][row co][k ci]
+template <int CI, int CO, int kThreads>
+__device__ __forceinline__ void split_weight(const float* __restrict__ w, int n, uint8_t* hi, uint8_t* lo) {
+    for (int i = threadIdx.x; i < n; i += kThreads) {
+        const int tap = i / (CI * CO), ci = (i / CO) % CI, co = i % CO;
+        __half h, l;
+        split_f16(kWScale * __ldg(w + i), h, l);
+        const uint32_t o = tap * (CO * 128) + sw_off(co, ci >> 3) + (ci & 7) * 2;
+        *reinterpret_cast<__half*>(hi + o) = h;
+        *reinterpret_cast<__half*>(lo + o) = l;
     }
 }
 
-// accumulate one tap: C_IN / 16 k-steps x 3 products (lo.w_hi, hi.w_lo, hi.w_hi) of this warpgroup's 64 rows
-template <int CI, int CO>
-__device__ __forceinline__ void mma_tap(float (&acc)[CO / 2], uint32_t ah, uint32_t al, uint32_t bh, uint32_t bl) {
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < CI / 16; ++k) {
-        wgmma_ss<CO>(acc, wgmma_desc_sw128(al + k * 32), wgmma_desc_sw128(bh + k * 32));
-        wgmma_ss<CO>(acc, wgmma_desc_sw128(ah + k * 32), wgmma_desc_sw128(bl + k * 32));
-        wgmma_ss<CO>(acc, wgmma_desc_sw128(ah + k * 32), wgmma_desc_sw128(bh + k * 32));
+// one lane: the fp32 rows of every tap of every tile this CTA takes, at row t0 + off(tap) of clip nb.  kPrefetch: the
+// rows of the tiles this CTA takes next are pulled into L2 two iterations ahead
+template <class L, bool kPrefetch, class Off>
+__device__ __forceinline__ void tap_producer(const CUtensorMap* map, uint8_t* sm, uint64_t* bars, int ntap, Off off,
+                                             int tiles_per_clip, int total_tiles) {
+    constexpr int FS = L::kFS;
+    uint64_t *f_full = bars, *f_empty = bars + 4;
+    const int first = blockIdx.x, stride = gridDim.x;
+    auto prefetch = [&](int tile) {
+        if (tile >= total_tiles) return;
+        const int nb = tile / tiles_per_clip, t0 = (tile - nb * tiles_per_clip) * kBM;
+        for (int tap = 0; tap < ntap; ++tap)
+            asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];" ::"l"(
+                             reinterpret_cast<uint64_t>(map)), "r"(0), "r"(t0 + off(tap)), "r"(nb) : "memory");
+    };
+    if constexpr (kPrefetch) prefetch(first + stride);
+    uint32_t kt = 0;
+    for (int tile = first; tile < total_tiles; tile += stride) {
+        const int nb = tile / tiles_per_clip, t0 = (tile - nb * tiles_per_clip) * kBM;
+        if constexpr (kPrefetch) prefetch(tile + 2 * stride);
+        for (int tap = 0; tap < ntap; ++tap, ++kt) {
+            const int s = kt % FS;
+            mbar_wait(&f_empty[s], ((kt / FS) & 1) ^ 1);
+            mbar_expect_tx(&f_full[s], (uint32_t)L::kFTile);
+            tma_load_3d(sm + L::offF + s * L::kFTile, map, 0, t0 + off(tap), nb, &f_full[s]);
+        }
     }
-    wgmma_commit();
+}
+
+// fp32 tap tiles -> (relu) -> hi / lo planes of the operand slots, by kGroups groups of 128 threads (warps 8..).  With two
+// groups, group g takes the taps whose counter is g mod 2 - that is the operand slot g and the fp32 slots g (mod 2) - so
+// two taps are converted concurrently and every barrier still sees exactly the 128 arrivals of one group per use
+template <class L, int C, int kGroups>
+__device__ __forceinline__ void tap_converter(uint8_t* sm, uint64_t* bars, int ntap, bool relu, int total_tiles) {
+    constexpr int FS = L::kFS;
+    uint64_t *f_full = bars, *f_empty = bars + 4, *a_full = bars + 8, *a_empty = bars + 10;
+    const int cg = ((threadIdx.x >> 5) - 8) >> 2, ct = threadIdx.x & 127;
+    uint32_t kt = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        for (int tap = 0; tap < ntap; ++tap, ++kt) {
+            if (kGroups == 2 && (int)(kt & 1) != cg) continue;
+            const int s = kt & 1, fs = kt % FS;
+            mbar_wait(&f_full[fs], (kt / FS) & 1);
+            mbar_wait(&a_empty[s], ((kt >> 1) & 1) ^ 1);
+            convert_planes<C / 4, false, false>(sm + L::offF + fs * L::kFTile, sm + L::offA + s * 2 * L::kATile, ct, relu);
+            // The fp32 slot is released only here, after every loaded value has been consumed by the stores above (an
+            // arrive right behind the loads would let TMA refill the slot under them); the proxy fence also orders this
+            // thread's generic reads of the slot before the async-proxy writes of the refill.
+            fence_async_smem();
+            mbar_arrive(&a_full[s]);
+            mbar_arrive(&f_empty[fs]);
+        }
+    }
+}
+
+// one consumer warpgroup's rows of one tile: acc = sum over the taps of A(tap) . W(tap) (planes wh / wl, one K block per
+// tap); each tap's operand slot is freed as soon as wgmma.wait_group 1 says it retired
+template <class L, int CI, int CO>
+__device__ __forceinline__ void tap_accumulate(float (&acc)[CO / 2], uint32_t& kt, int ntap, uint8_t* sm, uint64_t* bars,
+                                               int wg, int wt, uint32_t wh, uint32_t wl) {
+    uint64_t *a_full = bars + 8, *a_empty = bars + 10;
+#pragma unroll
+    for (int i = 0; i < CO / 2; ++i) acc[i] = 0.f;
+    for (int tap = 0; tap < ntap; ++tap, ++kt) {
+        const int s = kt & 1;
+        mbar_wait(&a_full[s], (kt >> 1) & 1);
+        const uint32_t ah = smem_u32(sm + L::offA + s * 2 * L::kATile) + wg * (64 * 128), al = ah + L::kATile;
+        mma_tap<CI, CO>(acc, ah, al, wh + tap * L::kWBlock, wl + tap * L::kWBlock);
+        if (tap > 0) {                                // the previous tap has retired: free its operand slot
+            wgmma_wait<1>();
+            if (wt == 0) mbar_arrive(&a_empty[(kt - 1) & 1]);
+        }
+    }
+    wgmma_wait<0>();
+    if (wt == 0) mbar_arrive(&a_empty[(kt - 1) & 1]);
 }
 
 template <int C>
@@ -114,87 +170,26 @@ resblock_t5_kernel(const __grid_constant__ CUtensorMap map_x, const float* __res
     constexpr int kGroups = L::kGroups, kThreadsT5 = L::kThreads, kProducer = 8 + 4 * kGroups;
     extern __shared__ __align__(1024) uint8_t sm[];
     uint64_t* bars = reinterpret_cast<uint64_t*>(sm + L::offBar);
-    uint64_t *f_full = bars, *f_empty = bars + 4, *a_full = bars + 8, *a_empty = bars + 10;
-    constexpr int FS = L::kFS;
     float* bias = reinterpret_cast<float*>(sm + L::offBias);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
     // ---- once per CTA: barriers, weights (scaled, split, swizzled), biases ------------------------------------------
-    if (tid == 0) {
-        for (int i = 0; i < FS; ++i) { mbar_init(&f_full[i], 1); mbar_init(&f_empty[i], 128); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&a_full[i], 128); mbar_init(&a_empty[i], 2); }   // a_empty: one arrival per warpgroup
-        mbar_fence_init();
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_x)) : "memory");
-    }
-    for (int i = tid; i < 3 * C * C; i += kThreadsT5) {        // w1[(tap * C + ci) * C + co] -> B1[tap block][row co][k ci]
-        const int tap = i / (C * C), ci = (i / C) % C, co = i % C;
-        __half h, l;
-        split_f16(kWScale * __ldg(w1 + i), h, l);
-        const uint32_t o = tap * L::kWBlock + sw_off(co, ci >> 3) + (ci & 7) * 2;
-        *reinterpret_cast<__half*>(sm + L::offW1h + o) = h;
-        *reinterpret_cast<__half*>(sm + L::offW1l + o) = l;
-    }
-    for (int i = tid; i < C * C; i += kThreadsT5) {            // w2[ci * C + co] -> B2[row co][k ci]
-        const int ci = i / C, co = i % C;
-        __half h, l;
-        split_f16(kWScale * __ldg(w2 + i), h, l);
-        const uint32_t o = sw_off(co, ci >> 3) + (ci & 7) * 2;
-        *reinterpret_cast<__half*>(sm + L::offW2h + o) = h;
-        *reinterpret_cast<__half*>(sm + L::offW2l + o) = l;
-    }
+    if (tid == 0) tap_init<L::kFS>(bars, &map_x);
+    split_weight<C, C, kThreadsT5>(w1, 3 * C * C, sm + L::offW1h, sm + L::offW1l);
+    split_weight<C, C, kThreadsT5>(w2, C * C, sm + L::offW2h, sm + L::offW2l);
     for (int i = tid; i < 2 * C; i += kThreadsT5) bias[i] = i < C ? __ldg(b1 + i) : __ldg(b2 + i - C);
     fence_async_smem();                                       // the weight planes are read by the tensor core (async proxy)
     __syncthreads();
     const int first = blockIdx.x, stride = gridDim.x;
 
     if (warp == kProducer) {
-        // ================= TMA producer =================
-        if (lane == 0) {
-            // the rows of the tiles this CTA takes next are pulled into L2 two iterations ahead (every row is read three times,
-            // as the centre tap of one tile and the side taps of two others: whoever comes first pays the HBM latency), so
-            // that the ring's loads are L2 hits - a ring of 64 KB cannot cover an HBM round trip
-            auto prefetch = [&](int tile) {
-                if (tile >= total_tiles) return;
-                const int nb = tile / tiles_per_clip, t0 = (tile - nb * tiles_per_clip) * kBM;
-                for (int tap = 0; tap < 3; ++tap)
-                    asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];" ::"l"(
-                                     reinterpret_cast<uint64_t>(&map_x)), "r"(0), "r"(t0 + (tap - 1) * dil), "r"(nb) : "memory");
-            };
-            prefetch(first + stride);
-            uint32_t kt = 0;
-            for (int tile = first; tile < total_tiles; tile += stride) {
-                const int nb = tile / tiles_per_clip, t0 = (tile - nb * tiles_per_clip) * kBM;
-                prefetch(tile + 2 * stride);
-                for (int tap = 0; tap < 3; ++tap, ++kt) {
-                    const int s = kt % FS;
-                    mbar_wait(&f_empty[s], ((kt / FS) & 1) ^ 1);
-                    mbar_expect_tx(&f_full[s], (uint32_t)L::kFTile);
-                    tma_load_3d(sm + L::offF + s * L::kFTile, &map_x, 0, t0 + (tap - 1) * dil, nb, &f_full[s]);
-                }
-            }
-        }
+        // every row is read three times, as the centre tap of one tile and the side taps of two others: whoever comes first
+        // pays the HBM latency, so the L2 prefetch makes the ring's loads L2 hits - a ring of 64 KB cannot cover an HBM
+        // round trip
+        if (lane == 0)
+            tap_producer<L, true>(&map_x, sm, bars, 3, [dil](int tap) { return (tap - 1) * dil; }, tiles_per_clip, total_tiles);
     } else if (warp >= 8) {
-        // ================= converters: fp32 tap tile -> relu -> hi / lo planes =================
-        // kGroups groups of 128 threads; with two groups, group g takes the taps whose counter is g mod 2 - that is the
-        // operand slot g and the fp32 slots g (mod 2) - so two taps are converted concurrently and every barrier still
-        // sees exactly the 128 arrivals of one group per use
-        const int cg = (warp - 8) >> 2, ct = tid & 127;
-        uint32_t kt = 0;
-        for (int tile = first; tile < total_tiles; tile += stride) {
-            for (int tap = 0; tap < 3; ++tap, ++kt) {
-                if (kGroups == 2 && (int)(kt & 1) != cg) continue;
-                const int s = kt & 1, fs = kt % FS;
-                mbar_wait(&f_full[fs], (kt / FS) & 1);
-                mbar_wait(&a_empty[s], ((kt >> 1) & 1) ^ 1);
-                convert_tap<C>(sm + L::offF + fs * L::kFTile, sm + L::offA + s * 2 * L::kATile, L::kATile, ct, true);
-                // The fp32 slot is released only here, after every loaded value has been consumed by the stores above (an
-                // arrive right behind the loads would let TMA refill the slot under them); the proxy fence also orders this
-                // thread's generic reads of the slot before the async-proxy writes of the refill.
-                fence_async_smem();
-                mbar_arrive(&a_full[s]);
-                mbar_arrive(&f_empty[fs]);
-            }
-        }
+        tap_converter<L, C, kGroups>(sm, bars, 3, true, total_tiles);
     } else {
         // ================= consumers: conv1, hidden tile, conv2, output =================
         const int wg = warp >> 2, wt = tid & 127, row0 = wg * 64 + (wt >> 5) * 16 + (lane >> 2);
@@ -206,20 +201,7 @@ resblock_t5_kernel(const __grid_constant__ CUtensorMap map_x, const float* __res
         for (int tile = first; tile < total_tiles; tile += stride) {
             const int nb = tile / tiles_per_clip, t0 = (tile - nb * tiles_per_clip) * kBM;
             float acc[C / 2];
-#pragma unroll
-            for (int i = 0; i < C / 2; ++i) acc[i] = 0.f;
-            for (int tap = 0; tap < 3; ++tap, ++kt) {
-                const int s = kt & 1;
-                mbar_wait(&a_full[s], (kt >> 1) & 1);
-                const uint32_t ah = smem_u32(sm + L::offA + s * 2 * L::kATile) + wg * (64 * 128), al = ah + L::kATile;
-                mma_tap<C, C>(acc, ah, al, w1h + tap * L::kWBlock, w1l + tap * L::kWBlock);
-                if (tap > 0) {                                // the previous tap has retired: free its operand slot
-                    wgmma_wait<1>();
-                    if (wt == 0) mbar_arrive(&a_empty[(kt - 1) & 1]);
-                }
-            }
-            wgmma_wait<0>();
-            if (wt == 0) mbar_arrive(&a_empty[(kt - 1) & 1]);
+            tap_accumulate<L, C, C>(acc, kt, 3, sm, bars, wg, wt, w1h, w1l);
             // ---- hidden = relu(conv1 / 2^8 + b1) -> hi / lo A fragments of the k1 conv -------------------------------
             uint32_t hh[C / 16][4], hl[C / 16][4];
 #pragma unroll
@@ -272,8 +254,8 @@ resblock_t5_kernel(const __grid_constant__ CUtensorMap map_x, const float* __res
 }
 
 // ---------------------------------------------------------------------------------------
-// Tap-GEMM convolution on the same machinery, for the decoder-side convs BETWEEN the residual blocks (the k3 input conv of
-// a DecoderConvBock, the two 2-tap phases of its k4-s2 transposed convs; encdec.py:28-46):
+// Tap-GEMM convolution on the same tap pipeline, for the decoder-side convs BETWEEN the residual blocks (the k3 input conv
+// of a DecoderConvBock, the two 2-tap phases of its k4-s2 transposed convs; encdec.py:28-46):
 //   out[t * os + oo, :] = res + scale * (sum_j x[t + off_j, :] . W_j + b),   c_in, c_out in {32, 64}, <= 3 taps, stride-1 input.
 // Roles as in resblock_t5_kernel minus the hidden tile: two consumer warpgroups (warps 0-7) that accumulate in registers
 // and stage scale * (acc / 2^8 + b) through shared memory to add the residual / store whole rows coalesced, 4 converter
@@ -307,27 +289,13 @@ template <int CI, int CO>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_t5_kernel(const __grid_constant__ CUtensorMap map_x, ConvT5P P, int tiles_per_clip, int total_tiles) {
     using L = T5C<CI, CO>;
-    constexpr int FS = L::kFS;
     extern __shared__ __align__(1024) uint8_t sm[];
     uint64_t* bars = reinterpret_cast<uint64_t*>(sm + L::offBar);
-    uint64_t *f_full = bars, *f_empty = bars + 4, *a_full = bars + 8, *a_empty = bars + 10;
     float* bias = reinterpret_cast<float*>(sm + L::offBias);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int ntap = P.n_taps;
-    if (tid == 0) {
-        for (int i = 0; i < FS; ++i) { mbar_init(&f_full[i], 1); mbar_init(&f_empty[i], 128); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&a_full[i], 128); mbar_init(&a_empty[i], 2); }
-        mbar_fence_init();
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_x)) : "memory");
-    }
-    for (int i = tid; i < ntap * CI * CO; i += kConvThreads) {  // w[(tap * CI + ci) * CO + co] -> B[tap][row co][k ci]
-        const int tap = i / (CI * CO), ci = (i / CO) % CI, co = i % CO;
-        __half h, l;
-        split_f16(kWScale * __ldg(P.w + i), h, l);
-        const uint32_t o = tap * L::kWBlock + sw_off(co, ci >> 3) + (ci & 7) * 2;
-        *reinterpret_cast<__half*>(sm + L::offWh + o) = h;
-        *reinterpret_cast<__half*>(sm + L::offWl + o) = l;
-    }
+    if (tid == 0) tap_init<L::kFS>(bars, &map_x);
+    split_weight<CI, CO, kConvThreads>(P.w, ntap * CI * CO, sm + L::offWh, sm + L::offWl);
     for (int i = tid; i < CO; i += kConvThreads) bias[i] = P.bias ? __ldg(P.bias + i) : 0.f;
     fence_async_smem();
     __syncthreads();
@@ -335,33 +303,11 @@ conv_t5_kernel(const __grid_constant__ CUtensorMap map_x, ConvT5P P, int tiles_p
 
     if (warp == 12) {
         if (lane == 0) {
-            uint32_t kt = 0;
-            for (int tile = first; tile < total_tiles; tile += stride) {
-                const int nb = tile / tiles_per_clip, t0 = (tile - nb * tiles_per_clip) * kBM;
-                for (int tap = 0; tap < ntap; ++tap, ++kt) {
-                    const int s = kt % FS;
-                    mbar_wait(&f_empty[s], ((kt / FS) & 1) ^ 1);
-                    mbar_expect_tx(&f_full[s], (uint32_t)L::kFTile);
-                    const int off = tap == 0 ? P.tap_off[0] : tap == 1 ? P.tap_off[1] : P.tap_off[2];     // no local copy of the array
-                    tma_load_3d(sm + L::offF + s * L::kFTile, &map_x, 0, t0 + off, nb, &f_full[s]);
-                }
-            }
+            auto off = [&](int tap) { return tap == 0 ? P.tap_off[0] : tap == 1 ? P.tap_off[1] : P.tap_off[2]; };   // no local copy of the array
+            tap_producer<L, false>(&map_x, sm, bars, ntap, off, tiles_per_clip, total_tiles);
         }
     } else if (warp >= 8) {
-        const int ct = tid & 127;
-        const bool relu = P.relu_in != 0;
-        uint32_t kt = 0;
-        for (int tile = first; tile < total_tiles; tile += stride) {
-            for (int tap = 0; tap < ntap; ++tap, ++kt) {
-                const int s = kt & 1, fs = kt % FS;
-                mbar_wait(&f_full[fs], (kt / FS) & 1);
-                mbar_wait(&a_empty[s], ((kt >> 1) & 1) ^ 1);
-                convert_tap<CI>(sm + L::offF + fs * L::kFTile, sm + L::offA + s * 2 * L::kATile, L::kATile, ct, relu);
-                fence_async_smem();
-                mbar_arrive(&a_full[s]);
-                mbar_arrive(&f_empty[fs]);          // only now: the loaded values have been consumed (see resblock_t5_kernel)
-            }
-        }
+        tap_converter<L, CI, 1>(sm, bars, ntap, P.relu_in != 0, total_tiles);
     } else {
         const int wg = warp >> 2, wt = tid & 127, row0 = wg * 64 + (wt >> 5) * 16 + (lane >> 2);
         const uint32_t wh = smem_u32(sm + L::offWh), wl = smem_u32(sm + L::offWl);
@@ -371,20 +317,7 @@ conv_t5_kernel(const __grid_constant__ CUtensorMap map_x, ConvT5P P, int tiles_p
         for (int tile = first; tile < total_tiles; tile += stride) {
             const int nb = tile / tiles_per_clip, t0 = (tile - nb * tiles_per_clip) * kBM;
             float acc[CO / 2];
-#pragma unroll
-            for (int i = 0; i < CO / 2; ++i) acc[i] = 0.f;
-            for (int tap = 0; tap < ntap; ++tap, ++kt) {
-                const int s = kt & 1;
-                mbar_wait(&a_full[s], (kt >> 1) & 1);
-                const uint32_t ah = smem_u32(sm + L::offA + s * 2 * L::kATile) + wg * (64 * 128), al = ah + L::kATile;
-                mma_tap<CI, CO>(acc, ah, al, wh + tap * L::kWBlock, wl + tap * L::kWBlock);
-                if (tap > 0) {
-                    wgmma_wait<1>();
-                    if (wt == 0) mbar_arrive(&a_empty[(kt - 1) & 1]);
-                }
-            }
-            wgmma_wait<0>();
-            if (wt == 0) mbar_arrive(&a_empty[(kt - 1) & 1]);
+            tap_accumulate<L, CI, CO>(acc, kt, ntap, sm, bars, wg, wt, wh, wl);
             stage_rows<CO>(stage, acc, bias, P.scale, row0, lane);
             named_sync(1 + wg);
             {
@@ -412,27 +345,18 @@ conv_t5_kernel(const __grid_constant__ CUtensorMap map_x, ConvT5P P, int tiles_p
 }
 
 // ---------------------------------------------------------------------------------------
-// Wide tap-GEMM convolution on the same roles, for c_in, c_out multiples of 64 with one of them above 64 (the upsampler
-// Conditioner's 512 / 1024 / 1920 channels, prior/conditioners.py):
+// Wide tap-GEMM convolution on the streamed-weight pipeline (split_tma.cuh), for c_in, c_out multiples of 64 with one of
+// them above 64 (the upsampler Conditioner's 512 / 1024 / 1920 channels, prior/conditioners.py):
 //   out[t * os + oo, co0 .. co0 + BN) = res + scale * (sum_tap sum_ci x[t + off_tap, ci] . W[tap, ci, co] + b)
 // K = taps x c_in no longer fits one operand tile and the weights no longer fit in shared memory, so
 //   - a work item is 128 positions x BN output channels (BN = 128, or 64 when c_out is an odd multiple of 64).  Items are
 //     numbered position-tile major: the CTAs that work on the channel tiles of one position tile at the same time share
 //     its activation rows in L2;
-//   - the K loop runs over the 64-channel blocks of every tap through a kS-stage ring.  A stage holds the fp32 block
-//     [128 positions x 64 channels] as TMA delivers it - the converters turn it IN PLACE into its hi / lo fp16 planes
-//     (16 KB each) - and the hi / lo planes of the weight block [BN x 64], which TMA loads with the 128-byte swizzle
-//     straight from the split weight that jk_pack_conv_weight_split made once per weight load ([hi | lo][c_out][taps *
-//     c_in] fp16 of 2^8 w);
-//   - every K block's 12 wgmmas go into a zeroed partial accumulator that is then added to the item's fp32 sum with
-//     ordinary (round-to-nearest) adds.  The tensor core's own accumulation rounds each k16 step's sum towards zero, and
-//     over K = 5760 that bias grows to ~2e-5 of the output scale; promoted every 64 channels it stays at the exact
-//     kernel's level.  The second accumulator is what the register reallocation below pays for;
+//   - the K loop runs over the 64-channel blocks of every tap.  A stage's weight planes come straight from the split
+//     weight that jk_pack_conv_weight_split made once per weight load ([hi | lo][c_out][taps * c_in] fp16 of 2^8 w);
 //   - the epilogue writes scale * (acc / 2^8 + b) (+ res) from the accumulator fragments: the four lanes of a quad cover
 //     32 contiguous bytes of one row (whole sectors, also for the row-strided phases of a transposed conv), and shared
 //     memory is left to the ring.
-// Roles, four warpgroups: consumers 0-1 (rows 0-63 / 64-127 of the item, 184 registers), converters (warps 8-11, 104
-// registers), TMA producer (warp 12; warps 13-15 only hand their registers back, 40 each).
 // ---------------------------------------------------------------------------------------
 struct ConvWideP {
     const float* bias; const float* res; float* out;
@@ -442,155 +366,65 @@ struct ConvWideP {
 };
 
 template <int BN>
-struct T5W {
-    static constexpr int kS = BN == 128 ? 3 : 4;             // ring stages (what 227 KB of shared memory leaves room for)
-    static constexpr int kA = kBM * 64 * 4;                  // fp32 block; after conversion hi plane | lo plane (16 KB each)
-    static constexpr int kAPlane = kBM * 128;
-    static constexpr int kB = BN * 128;                      // one weight plane: BN rows x 64 fp16
-    static constexpr int kStage = kA + 2 * kB;
-    static constexpr int offBar = kS * kStage;
-    static constexpr int smem = offBar + 128 + 1024;         // barriers, and slack to align the ring to 1024 bytes
+struct ConvWideJob {
+    using Ring = StreamRing<BN, BN == 128 ? 3 : 4>;          // ring stages: what 227 KB of shared memory leaves room for
+    static constexpr bool kCheck = false;
+    const CUtensorMap *map_a, *map_w;                        // [c_in, t_in, n] fp32 activations, the split weight
+    ConvWideP P;
+    int tiles_per_clip, n_tiles_n, kb_per_tap, n_kb;
+    bool relu;
+    struct Tile { int nb, t0, co0; };
+
+    __device__ __forceinline__ Tile tile(int item) const {
+        const int mt = item / n_tiles_n, co0 = (item - mt * n_tiles_n) * BN;
+        const int nb = mt / tiles_per_clip, t0 = (mt - nb * tiles_per_clip) * kBM;
+        return {nb, t0, co0};
+    }
+    __device__ __forceinline__ void load(uint8_t* st, const Tile& t, int kb, uint64_t* bar) const {
+        const int tap = kb / kb_per_tap, c0 = (kb - tap * kb_per_tap) * 64;
+        const int off = tap == 0 ? P.tap_off[0] : tap == 1 ? P.tap_off[1] : P.tap_off[2];
+        // rows outside [0, T) of clip nb - a whole block of them when the dilation exceeds T - arrive as zeros
+        tma_load_3d(st, map_a, c0, t.t0 + off, t.nb, bar);
+        tma_load_2d(st + Ring::kA, map_w, tap * P.c_in + c0, t.co0, bar);
+        tma_load_2d(st + Ring::kA + Ring::kB, map_w, tap * P.c_in + c0, P.c_out + t.co0, bar);
+    }
+    // ---- out = res + scale * (acc / 2^8 + b), straight from the fragments ----
+    __device__ __forceinline__ void epilogue(const float (&acc)[BN / 2], const Tile& t, int rq, int lane) const {
+        const long long rows_out = P.t_out * P.out_stride;
+        float* ob = P.out + (size_t)t.nb * rows_out * P.c_out + t.co0;
+        const float* rb = P.res ? P.res + (size_t)t.nb * rows_out * P.c_out + t.co0 : nullptr;
+        const float* bb = P.bias ? P.bias + t.co0 : nullptr;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const long long tt = (long long)t.t0 + rq + 8 * h;
+            if (tt < P.t_out) {
+                const size_t ro = (size_t)(tt * P.out_stride + P.out_offset) * P.c_out;
+#pragma unroll
+                for (int i = 0; i < BN / 8; ++i) {
+                    const int col = 8 * i + 2 * (lane & 3);
+                    const float2 b = bb ? __ldg(reinterpret_cast<const float2*>(bb + col)) : make_float2(0.f, 0.f);
+                    float2 o;
+                    o.x = P.scale * fmaf(acc[4 * i + 2 * h], kWInv, b.x);
+                    o.y = P.scale * fmaf(acc[4 * i + 2 * h + 1], kWInv, b.y);
+                    if (rb) {
+                        const float2 r = __ldg(reinterpret_cast<const float2*>(rb + ro + col));
+                        o.x += r.x; o.y += r.y;
+                    }
+                    *reinterpret_cast<float2*>(ob + ro + col) = o;
+                }
+            }
+        }
+    }
 };
 
-// fp32 block [128][64] at st -> (relu) -> hi plane at st, lo plane at st + 16 KB, by the 128 converter threads: every
-// value is read into registers before the group barrier, so the planes can overwrite the block they come from
-__device__ __forceinline__ void convert_block_inplace(uint8_t* st, int ct, bool relu) {
-    constexpr int CH = 16, PER = kBM * CH / 128;            // float4 chunks per row, items per thread
-    const float4* f = reinterpret_cast<const float4*>(st);
-    float4 v[PER];
-#pragma unroll
-    for (int j = 0; j < PER; ++j) v[j] = f[ct + j * 128];
-    uint2 h[PER], l[PER];
-#pragma unroll
-    for (int j = 0; j < PER; ++j) {
-        if (relu) { v[j].x = fmaxf(v[j].x, 0.f); v[j].y = fmaxf(v[j].y, 0.f); v[j].z = fmaxf(v[j].z, 0.f); v[j].w = fmaxf(v[j].w, 0.f); }
-        split_f16x2(v[j].x, v[j].y, h[j].x, l[j].x);
-        split_f16x2(v[j].z, v[j].w, h[j].y, l[j].y);
-    }
-    named_sync(1);
-#pragma unroll
-    for (int j = 0; j < PER; ++j) {
-        const int item = ct + j * 128, r = item / CH, c4 = item % CH;
-        const uint32_t o = sw_off(r, c4 >> 1) + (c4 & 1) * 8;
-        *reinterpret_cast<uint2*>(st + o) = h[j];
-        *reinterpret_cast<uint2*>(st + kBM * 128 + o) = l[j];
-    }
-}
-
-constexpr int kWideThreads = 512;
-
 template <int BN>
-__global__ void __launch_bounds__(kWideThreads, 1)
+__global__ void __launch_bounds__(kStreamThreads, 1)
 conv_wide_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w, ConvWideP P,
                  int tiles_per_clip, int n_tiles_n, int total_items) {
-    using L = T5W<BN>;
-    constexpr int S = L::kS;
     extern __shared__ __align__(1024) uint8_t sm_raw[];
-    uint8_t* sm = sm_raw + ((1024u - (smem_u32(sm_raw) & 1023u)) & 1023u);   // TMA's 128-byte swizzle needs 1024-byte stages
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sm + L::offBar);
-    uint64_t *full = bars, *conv = bars + S, *empty = bars + 2 * S;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int kb_per_tap = P.c_in / 64, n_kb = P.n_taps * kb_per_tap;
-    if (tid == 0) {
-        // full: the producer's expect_tx (activation + weight bytes); conv: the 128 converter threads; empty: one arrival
-        // per consumer warpgroup once its MMAs on the stage have retired
-        for (int i = 0; i < S; ++i) { mbar_init(&full[i], 1); mbar_init(&conv[i], 128); mbar_init(&empty[i], 2); }
-        mbar_fence_init();
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_x)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_w)) : "memory");
-    }
-    __syncthreads();
-    const int first = blockIdx.x, stride = gridDim.x;
-
-    // register reallocation (setmaxnreg, whole warpgroups): the block launches with 128 per thread (65536 / 512);
-    // 2 x 128 x 184 + 128 x 104 + 128 x 40 = 65536
-    if (warp >= 12) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-        if (warp == 12 && lane == 0) {
-            uint32_t kt = 0;
-            for (int item = first; item < total_items; item += stride) {
-                const int mt = item / n_tiles_n, co0 = (item - mt * n_tiles_n) * BN;
-                const int nb = mt / tiles_per_clip, t0 = (mt - nb * tiles_per_clip) * kBM;
-                for (int kb = 0; kb < n_kb; ++kb, ++kt) {
-                    const int s = kt % S, tap = kb / kb_per_tap, c0 = (kb - tap * kb_per_tap) * 64;
-                    mbar_wait(&empty[s], ((kt / S) & 1) ^ 1);
-                    mbar_expect_tx(&full[s], (uint32_t)L::kStage);
-                    const int off = tap == 0 ? P.tap_off[0] : tap == 1 ? P.tap_off[1] : P.tap_off[2];
-                    uint8_t* st = sm + s * L::kStage;
-                    // rows outside [0, T) of clip nb - a whole block of them when the dilation exceeds T - arrive as zeros
-                    tma_load_3d(st, &map_x, c0, t0 + off, nb, &full[s]);
-                    tma_load_2d(st + L::kA, &map_w, tap * P.c_in + c0, co0, &full[s]);
-                    tma_load_2d(st + L::kA + L::kB, &map_w, tap * P.c_in + c0, P.c_out + co0, &full[s]);
-                }
-            }
-        }
-    } else if (warp >= 8) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 104;");
-        const int ct = tid & 127;
-        const bool relu = P.relu_in != 0;
-        uint32_t kt = 0;
-        for (int item = first; item < total_items; item += stride) {
-            for (int kb = 0; kb < n_kb; ++kb, ++kt) {
-                const int s = kt % S;
-                mbar_wait(&full[s], (kt / S) & 1);
-                convert_block_inplace(sm + s * L::kStage, ct, relu);
-                fence_async_smem();                   // the planes are read by the tensor core (async proxy)
-                mbar_arrive(&conv[s]);
-            }
-        }
-    } else {
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 184;");
-        const int wg = warp >> 2, wt = tid & 127, rq = wg * 64 + (wt >> 5) * 16 + (lane >> 2);
-        const uint32_t ring = smem_u32(sm);
-        uint32_t kt = 0;
-        for (int item = first; item < total_items; item += stride) {
-            const int mt = item / n_tiles_n, co0 = (item - mt * n_tiles_n) * BN;
-            const int nb = mt / tiles_per_clip, t0 = (mt - nb * tiles_per_clip) * kBM;
-            float acc[BN / 2];
-#pragma unroll
-            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-            for (int kb = 0; kb < n_kb; ++kb, ++kt) {
-                const int s = kt % S;
-                const uint32_t ph = (kt / S) & 1;
-                mbar_wait(&full[s], ph);              // weight planes (TMA)
-                mbar_wait(&conv[s], ph);              // activation planes (converters)
-                const uint32_t st = ring + s * L::kStage, ah = st + wg * (64 * 128), al = ah + L::kAPlane;
-                float part[BN / 2];
-#pragma unroll
-                for (int i = 0; i < BN / 2; ++i) part[i] = 0.f;
-                mma_tap<64, BN>(part, ah, al, st + L::kA, st + L::kA + L::kB);
-                wgmma_wait<0>();
-                if (wt == 0) mbar_arrive(&empty[s]);  // the block has retired: free its stage
-#pragma unroll
-                for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
-            }
-            // ---- out = res + scale * (acc / 2^8 + b), straight from the fragments ----
-            const long long rows_out = P.t_out * P.out_stride;
-            float* ob = P.out + (size_t)nb * rows_out * P.c_out + co0;
-            const float* rb = P.res ? P.res + (size_t)nb * rows_out * P.c_out + co0 : nullptr;
-            const float* bb = P.bias ? P.bias + co0 : nullptr;
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const long long t = (long long)t0 + rq + 8 * h;
-                if (t < P.t_out) {
-                    const size_t ro = (size_t)(t * P.out_stride + P.out_offset) * P.c_out;
-#pragma unroll
-                    for (int i = 0; i < BN / 8; ++i) {
-                        const int col = 8 * i + 2 * (lane & 3);
-                        const float2 b = bb ? __ldg(reinterpret_cast<const float2*>(bb + col)) : make_float2(0.f, 0.f);
-                        float2 o;
-                        o.x = P.scale * fmaf(acc[4 * i + 2 * h], kWInv, b.x);
-                        o.y = P.scale * fmaf(acc[4 * i + 2 * h + 1], kWInv, b.y);
-                        if (rb) {
-                            const float2 r = __ldg(reinterpret_cast<const float2*>(rb + ro + col));
-                            o.x += r.x; o.y += r.y;
-                        }
-                        *reinterpret_cast<float2*>(ob + ro + col) = o;
-                    }
-                }
-            }
-        }
-    }
+    const int kb_per_tap = P.c_in / 64;
+    const ConvWideJob<BN> job{&map_x, &map_w, P, tiles_per_clip, n_tiles_n, kb_per_tap, P.n_taps * kb_per_tap, P.relu_in != 0};
+    streamed_pipeline(job, sm_raw, total_items);
 }
 
 // packed fp32 [k, c_in, c_out] -> [hi | lo][c_out][k * c_in] fp16 of 2^8 w (row co, column tap * c_in + ci)
@@ -609,17 +443,8 @@ __global__ void pack_split_kernel(const float* __restrict__ packed, unsigned sho
 template <int C>
 int launch_t5(const float* x, float* out, const float* w1, const float* b1, const float* w2, const float* b2, int n,
               long long T, int dil, float rs, cudaStream_t stream) {
-    EncodeTiledFnT5 enc = t5_encode();
-    JK_REQUIRE(enc, "cuTensorMapEncodeTiled is not available from the driver");
     CUtensorMap map;
-    cuuint64_t dims[3] = {(cuuint64_t)C, (cuuint64_t)T, (cuuint64_t)n};
-    cuuint64_t strides[2] = {(cuuint64_t)C * 4, (cuuint64_t)T * C * 4};
-    cuuint32_t box[3] = {(cuuint32_t)C, (cuuint32_t)kBM, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    JK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for a [%d, %lld, %d] fp32 tensor", (int)r, n, T, C);
+    if (int rc = encode_rows_map(&map, x, n, T, C, C)) return rc;
     int sms = 0;
     if (int rc = set_max_smem_once<resblock_t5_kernel<C>>(T5<C>::smem)) return rc;
     if (int rc = sm_count(&sms)) return rc;
@@ -634,17 +459,8 @@ int launch_t5(const float* x, float* out, const float* w1, const float* b1, cons
 
 template <int CI, int CO>
 int launch_conv_t5(const ConvT5P& P, int n, cudaStream_t stream) {
-    EncodeTiledFnT5 enc = t5_encode();
-    JK_REQUIRE(enc, "cuTensorMapEncodeTiled is not available from the driver");
     CUtensorMap map;
-    cuuint64_t dims[3] = {(cuuint64_t)CI, (cuuint64_t)P.t_in, (cuuint64_t)n};
-    cuuint64_t strides[2] = {(cuuint64_t)CI * 4, (cuuint64_t)P.t_in * CI * 4};
-    cuuint32_t box[3] = {(cuuint32_t)CI, (cuuint32_t)kBM, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(P.in), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    JK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for a [%d, %lld, %d] fp32 tensor", (int)r, n, P.t_in, CI);
+    if (int rc = encode_rows_map(&map, P.in, n, P.t_in, CI, CI)) return rc;
     int sms = 0;
     if (int rc = set_max_smem_once<conv_t5_kernel<CI, CO>>(T5C<CI, CO>::smem)) return rc;
     if (int rc = sm_count(&sms)) return rc;
@@ -658,37 +474,23 @@ int launch_conv_t5(const ConvT5P& P, int n, cudaStream_t stream) {
 
 template <int BN>
 int launch_conv_wide(const float* in, long long t_in, const void* w_split, const ConvWideP& P, int n, cudaStream_t stream) {
-    EncodeTiledFnT5 enc = t5_encode();
-    JK_REQUIRE(enc, "cuTensorMapEncodeTiled is not available from the driver");
+    constexpr int kSmem = ConvWideJob<BN>::Ring::smem;
     CUtensorMap map_x, map_w;
-    {
-        cuuint64_t dims[3] = {(cuuint64_t)P.c_in, (cuuint64_t)t_in, (cuuint64_t)n};
-        cuuint64_t strides[2] = {(cuuint64_t)P.c_in * 4, (cuuint64_t)t_in * P.c_in * 4};
-        cuuint32_t box[3] = {64, (cuuint32_t)kBM, 1};
-        cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = enc(&map_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(in), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        JK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for a [%d, %lld, %d] fp32 tensor", (int)r, n, t_in, P.c_in);
-    }
-    {
-        const long long K = (long long)P.n_taps * P.c_in;
-        cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)2 * P.c_out};
-        cuuint64_t strides[1] = {(cuuint64_t)K * 2};
-        cuuint32_t box[2] = {64, (cuuint32_t)BN};
-        cuuint32_t estr[2] = {1, 1};
-        CUresult r = enc(&map_w, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(w_split), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        JK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for a [2 x %d, %lld] fp16 split weight", (int)r, P.c_out, K);
-    }
+    if (int rc = encode_rows_map(&map_x, in, n, t_in, P.c_in, 64)) return rc;
+    const long long K = (long long)P.n_taps * P.c_in;
+    const cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)2 * P.c_out};
+    const cuuint64_t strides[1] = {(cuuint64_t)K * 2};
+    const cuuint32_t box[2] = {64, (cuuint32_t)BN};
+    if (int rc = encode_tensor_map(&map_w, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, w_split, dims, strides, box,
+                                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
+        return rc;
     int sms = 0;
-    if (int rc = set_max_smem_once<conv_wide_kernel<BN>>(T5W<BN>::smem)) return rc;
+    if (int rc = set_max_smem_once<conv_wide_kernel<BN>>(kSmem)) return rc;
     if (int rc = sm_count(&sms)) return rc;
     const long long per_clip = (P.t_out + kBM - 1) / kBM, n_tiles_n = P.c_out / BN, total = per_clip * n * n_tiles_n;
     JK_REQUIRE(total < (1ll << 31) && t_in + 4096 < (1ll << 31), "clip too long for 32-bit tile coordinates");
     const unsigned grid = (unsigned)std::min<long long>(total, sms);
-    conv_wide_kernel<BN><<<grid, kWideThreads, T5W<BN>::smem, stream>>>(map_x, map_w, P, (int)per_clip, (int)n_tiles_n, (int)total);
+    conv_wide_kernel<BN><<<grid, kStreamThreads, kSmem, stream>>>(map_x, map_w, P, (int)per_clip, (int)n_tiles_n, (int)total);
     JK_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -1,5 +1,6 @@
 """CPU checks of the wide tensor-core convolutions (jk_conv1d_tc_wide): the library exports the new entry points with the
-ctypes signatures of jukebox_b200/_lib.py, the new kernels do not spill (nvcc -Xptxas -v for sm_90a), and only the
+ctypes signatures of jukebox_b200/_lib.py, the split-precision TMA kernels (vqvae_t5.cu, score.cu) use no stack and do
+not spill (nvcc -Xptxas -v for sm_90a), and only the
 decoder side of a VQ-VAE sets `tensor_cores` (the encoder's output feeds the bit-exact codebook argmin)."""
 import ctypes
 import os
@@ -37,29 +38,38 @@ def test_split_byte_count():
     assert _lib.lib().jk_conv_weight_split_bytes(0, 64, 64, ctypes.byref(n)) != 0
 
 
+# the split-precision TMA kernels of each source and how many instantiations of each it compiles
+SPLIT_TMA_KERNELS = {
+    "vqvae_t5.cu": {"conv_wide_kernel": 2, "conv_t5_kernel": 4, "resblock_t5_kernel": 2, "pack_split_kernel": 1},
+    "score.cu": {"xout_head_kernel": 2},
+}
+
+
 @pytest.mark.skipif(shutil.which("nvcc") is None and not os.path.exists("/usr/local/cuda/bin/nvcc"),
                     reason="needs the CUDA toolkit")
 def test_wide_conv_kernels_do_not_spill(tmp_path):
     from jukebox_b200.build import _nvcc
-    src = os.path.join(ROOT, "jukebox_b200", "csrc", "vqvae_t5.cu")
-    cmd = [_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
-           "-Xptxas", "-v", "-c", src, "-o", str(tmp_path / "vqvae_t5.o"), "-I", os.path.join(ROOT, "include")]
-    out = subprocess.run(cmd, capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0, out.stderr[-3000:]
-    report = {}
-    current = None
-    for line in out.stderr.splitlines():
-        m = re.search(r"Compiling entry function '(\w+)'", line)
-        if m:
-            current = m.group(1)
-            continue
-        m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", line)
-        if m and current:
-            report[current] = (int(m.group(1)), int(m.group(2)))
-    wide = {k: v for k, v in report.items() if "conv_wide_kernel" in k or "pack_split_kernel" in k}
-    assert len([k for k in wide if "conv_wide_kernel" in k]) == 2, report       # BN = 64 and BN = 128
-    for name, (st, ld) in wide.items():
-        assert st == 0 and ld == 0, f"{name} spills {st} bytes / loads {ld} bytes"
+    for source, kernels in SPLIT_TMA_KERNELS.items():
+        src = os.path.join(ROOT, "jukebox_b200", "csrc", source)
+        cmd = [_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
+               "-Xptxas", "-v", "-c", src, "-o", str(tmp_path / "kernels.o"), "-I", os.path.join(ROOT, "include")]
+        out = subprocess.run(cmd, capture_output=True, text=True, timeout=600)
+        assert out.returncode == 0, out.stderr[-3000:]
+        report = {}
+        current = None
+        for line in out.stderr.splitlines():
+            m = re.search(r"Compiling entry function '(\w+)'", line)
+            if m:
+                current = m.group(1)
+                continue
+            m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", line)
+            if m and current:
+                report[current] = tuple(int(v) for v in m.groups())
+        for kernel, count in kernels.items():
+            found = {k: v for k, v in report.items() if kernel in k}
+            assert len(found) == count, (source, kernel, report)
+            for name, (stack, st, ld) in found.items():
+                assert stack == 0 and st == 0 and ld == 0, f"{name}: {stack} bytes stack, spills {st} bytes / loads {ld} bytes"
 
 
 def test_only_the_decoder_side_sets_tensor_cores():
