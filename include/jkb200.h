@@ -249,6 +249,31 @@ int jk_prefill_attention_f16(const jk_prefill_attn_args* a, jk_prefill_attn_rout
 
 /* one token position; increments the device-side position counter */
 int jk_prior_step(jk_prior* p, const jk_step_args* a, jk_stream_t stream);
+
+/* Sample selection (csrc/select.cu): row b of the engine becomes a copy of row parents[b], b < n, so that one sample's
+ * history can be continued in several rows (a prime prefilled once and repeated, or the likeliest samples of a window
+ * kept).  The state a row carries from one step to the next is its K / V cache in every layer, the encoder-decoder (6)
+ * and prime (7) layers included; everything else an engine holds is rebuilt by every step.
+ * jk_prior_select_plan is host arithmetic (no device needed): the rows to stash (read by another row AND overwritten,
+ * ascending) and the workspace they need.  Broadcasting one row, or keeping some rows in place and copying them to the
+ * others, stashes nothing; only a permutation that overwrites a row another row still reads does.  n in [1, max_batch]
+ * and every parent in [0, n), else an error. */
+typedef struct jk_select_plan_info {
+    int32_t n_copies;                 /* rows b with parents[b] != b                                    */
+    int32_t n_stash;                  /* rows copied to the workspace first                             */
+    int32_t stash[JK_MAX_BATCH];      /* those rows, ascending; slot i of the workspace holds stash[i]  */
+    uint64_t row_bytes;               /* one row's K and V over every layer                             */
+    uint64_t workspace_bytes;         /* n_stash * row_bytes                                            */
+    uint64_t bytes_moved;             /* read + written: 2 * row_bytes * (n_stash + n_copies)           */
+} jk_select_plan_info;
+int jk_prior_select_plan(const jk_prior_config* cfg, const int32_t* parents, int n, jk_select_plan_info* out);
+/* Reorders rows [0, n) of every layer's K / V cache in place: at most two launches on `stream` (the stashed rows into
+ * `workspace`, then every copy), nothing synchronises.  parents is host memory.  workspace: device memory of at least
+ * the plan's workspace_bytes, 16-byte aligned (NULL when that is 0).  A bad n or parent, a short workspace or an engine
+ * whose last prefill stopped early (jk_prior_position -1) is an error, and nothing is launched.  The position does not
+ * change: every row continues from it. */
+int jk_prior_select(jk_prior* p, const int32_t* parents, int n, void* workspace, size_t workspace_bytes,
+                    jk_stream_t stream);
 /* current position (host copy of the device counter as tracked by the calls made so far); -1 after a truncated prefill
  * (jk_prefill_args.n_layers), until jk_prior_reset */
 int jk_prior_position(const jk_prior* p, int* t);

@@ -85,6 +85,11 @@ class PrefillAttnRoute(C.Structure):
     _fields_ = [("tensor_cores", C.c_int32), ("tile_dh", C.c_int32), ("stage_bytes", C.c_int32)]
 
 
+class SelectPlanInfo(C.Structure):
+    _fields_ = [("n_copies", C.c_int32), ("n_stash", C.c_int32), ("stash", C.c_int32 * JK_MAX_BATCH),
+                ("row_bytes", C.c_uint64), ("workspace_bytes", C.c_uint64), ("bytes_moved", C.c_uint64)]
+
+
 class ConvArgs(C.Structure):
     _fields_ = [("inp", C.c_void_p), ("t_in", C.c_int64), ("c_in", C.c_int32),
                 ("out", C.c_void_p), ("t_out", C.c_int64), ("c_out", C.c_int32),
@@ -115,6 +120,8 @@ SIGNATURES = {
     "jk_pool_rows_f32": (_I, [_P, _I, _I, _I, _I, _I, _P, _L, _P, _P]),
     "jk_prior_position": (_I, [_P, C.POINTER(C.c_int)]),
     "jk_prior_has_logits_gemm": (_I, [_P, C.POINTER(C.c_int)]),
+    "jk_prior_select_plan": (_I, [C.POINTER(PriorConfig), C.POINTER(C.c_int32), _I, C.POINTER(SelectPlanInfo)]),
+    "jk_prior_select": (_I, [_P, C.POINTER(C.c_int32), _I, _P, C.c_size_t, _P]),
     "jk_prior_debug_buffer": (_I, [_P, _I, C.POINTER(_P), C.POINTER(C.c_size_t)]),
     "jk_prefill_attention_f16": (_I, [C.POINTER(PrefillAttnArgs), C.POINTER(PrefillAttnRoute), _P]),
     "jk_conv1d_prefill_f16": (_I, [_P, _P, _P, _P, _I, _I, _I, _P]),

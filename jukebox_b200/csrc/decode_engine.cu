@@ -1679,18 +1679,6 @@ struct Layout {
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-int cache_rows_for(const jk_prior_config& c, int af, int bc, int prime_pad) {
-    switch (af) {
-        case 0: return c.n_ctx;
-        case 1: return bc;
-        case 2: return c.n_ctx;
-        case 3: return 2 * bc;
-        case 6: return c.encoder_dims;
-        case 7: return prime_pad;
-    }
-    return -1;
-}
-
 int compute_layout(const jk_prior_config& c, int G, Layout& L) {
     JK_REQUIRE(c.depth >= 1 && c.depth <= JK_MAX_DEPTH, "depth %d out of range", c.depth);
     JK_REQUIRE(c.max_batch >= 1 && c.max_batch <= JK_MAX_BATCH, "max_batch %d out of range (<= %d)", c.max_batch, JK_MAX_BATCH);
@@ -1698,11 +1686,11 @@ int compute_layout(const jk_prior_config& c, int G, Layout& L) {
                "width/n_state/mlp_width must be multiples of 16 (got %d/%d/%d)", c.width, c.n_state, c.mlp_width);
     JK_REQUIRE(c.n_state % c.heads == 0, "n_state %% heads != 0");
     L.dh = c.n_state / c.heads;
-    L.dh_pad = (int)align_up(L.dh, 16);      // MMA k-steps / output pairs of 16 dims
+    L.dh_pad = head_dim_pad(c);              // MMA k-steps / output pairs of 16 dims
     JK_REQUIRE(L.dh_pad <= 512, "head_dim %d > 512 unsupported", L.dh);
-    L.bc = c.blocks > 0 ? c.n_ctx / c.blocks : c.n_ctx;
+    L.bc = block_len(c);
     JK_REQUIRE(c.blocks == 0 || c.n_ctx % c.blocks == 0, "n_ctx %% blocks != 0");
-    L.prime_pad = c.blocks > 0 ? (c.prime_len / c.blocks + 1) * c.blocks : 0;
+    L.prime_pad = prime_pad_len(c);
     JK_REQUIRE(L.dh % 2 == 0, "head_dim %d must be even", L.dh);
     const int depth = c.depth;
     // K-split factor: CTAs form units of KS that share column groups and split K.  The largest of 4 / 2 / 1 for which

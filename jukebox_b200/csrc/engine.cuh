@@ -52,6 +52,25 @@ struct EngineDev {
     LayerDev layer[JK_MAX_DEPTH];
 };
 
+// Geometry of the K / V caches (DESIGN §4), from the configuration alone: compute_layout sizes the caches with it and the
+// sample selection (select.cu) plans its copies with it, with or without an engine.
+inline int head_dim_pad(const jk_prior_config& c) { return (c.n_state / c.heads + 15) / 16 * 16; }   // MMA k-steps of 16
+inline int block_len(const jk_prior_config& c) { return c.blocks > 0 ? c.n_ctx / c.blocks : c.n_ctx; }
+inline int prime_pad_len(const jk_prior_config& c) { return c.blocks > 0 ? (c.prime_len / c.blocks + 1) * c.blocks : 0; }
+// rows per (sample, head) of a layer's cache: the positions its attention pattern reads, the encoder rows (6) or the
+// padded prime (7); -1 for an attn_func without a decode path
+inline int cache_rows_for(const jk_prior_config& c, int af, int bc, int prime_pad) {
+    switch (af) {
+        case 0: return c.n_ctx;
+        case 1: return bc;
+        case 2: return c.n_ctx;
+        case 3: return 2 * bc;
+        case 6: return c.encoder_dims;
+        case 7: return prime_pad;
+    }
+    return -1;
+}
+
 // the attention scores' scale dh^-1/2, as the reference applies it to q and k in two halves:
 // scale = 1/sqrt(sqrt(dh)); w.mul_(scale*scale)  (factored_attention.py:83-88)
 inline float attn_scale2(int dh) {

@@ -42,6 +42,27 @@ def config_prefill_capacity(device, **kw):
     return out.value if rc == 0 else 0
 
 
+def _parents(parents):
+    """parents (a sequence or 1-D tensor of ints) as a C int32 array and its length"""
+    if isinstance(parents, torch.Tensor):
+        if parents.dim() != 1 or parents.dtype.is_floating_point or parents.dtype == torch.bool:
+            raise RuntimeError(f"parents must be a 1-D integer tensor, got {parents.dtype} {tuple(parents.shape)}")
+        parents = parents.tolist()
+    vals = [int(v) for v in parents]
+    if not 1 <= len(vals) <= _lib.JK_MAX_BATCH:
+        raise RuntimeError(f"parents of {len(vals)} rows: 1 .. {_lib.JK_MAX_BATCH} rows can be selected")
+    return (C.c_int32 * len(vals))(*vals), len(vals)
+
+
+def select_plan(cfg, parents):
+    """the jk_select_plan_info of a selection on an engine of configuration cfg (host arithmetic, no device):
+    row b becomes a copy of row parents[b]"""
+    arr, n = _parents(parents)
+    info = _lib.SelectPlanInfo()
+    check(lib().jk_prior_select_plan(C.byref(cfg), arr, n, C.byref(info)))
+    return info
+
+
 class DecodeEngine:
     def __init__(self, *, width, depth, heads, n_state, mlp_width, n_ctx, blocks, attn_funcs,
                  bins=0, prime_len=0, encoder_dims=0, max_batch=16, add_cond_after=True, device=None):
@@ -224,6 +245,25 @@ class DecodeEngine:
         with torch.cuda.device(self.device):
             check(lib().jk_prior_step(self.handle, C.byref(a), stream_ptr()))
         self.position += 1
+
+    # ---- sample selection ----------------------------------------------------------------
+    def select_plan(self, parents):
+        """what select(parents) would copy (jk_select_plan_info): rows it stashes, workspace and bytes moved"""
+        return select_plan(self.cfg, parents)
+
+    def select(self, parents):
+        """row b of every layer's K / V cache becomes a copy of row parents[b], b < len(parents) (jk_prior_select):
+        the histories of the rows are reordered, the position stays.  A workspace is allocated only when the selection
+        overwrites a row that another row still reads (jk_select_plan_info.n_stash)."""
+        arr, n = _parents(parents)
+        info = select_plan(self.cfg, parents)
+        ws = None
+        if info.workspace_bytes:
+            ws = torch.empty(info.workspace_bytes, dtype=torch.uint8, device=self.device)
+        with torch.cuda.device(self.device):
+            check(lib().jk_prior_select(self.handle, arr, n, ptr(ws), C.c_size_t(info.workspace_bytes), stream_ptr()))
+        # the copies read `ws` on the current stream; torch's allocator is stream-ordered, so it may be released here
+        return info
 
     def debug_buffer(self, which):
         p, n = C.c_void_p(0), C.c_size_t(0)

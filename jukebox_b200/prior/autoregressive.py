@@ -161,11 +161,12 @@ class ConditionalAutoregressive2D(nn.Module):
         return acts + (x_cond[:, t0:t1] if x_cond.shape[1] > 1 else x_cond)
 
     def _run(self, n_samples, prime, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds, sample_tokens,
-             get_logprobs=False):
-        """shared body of sample / primed_sample.  prime: LongTensor [N, P] of given tokens (P may be 0)."""
+             get_logprobs=False, select_every=None, select_keep=None):
+        """shared body of sample / primed_sample.  prime: LongTensor [N, P] of given tokens (P may be 0), or [1, P]
+        with its conditioning of one row too: prefilled once and repeated to the N rows."""
         cls = SamplingWindow if fp16 else SamplingWindowF32
         win = cls(self, n_samples, prime, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds,
-                  sample_tokens, get_logprobs=get_logprobs)
+                  sample_tokens, get_logprobs=get_logprobs, select_every=select_every, select_keep=select_keep)
         win.advance(win.sample_tokens)
         return win.finish()
 
@@ -174,21 +175,30 @@ class ConditionalAutoregressive2D(nn.Module):
     # log-likelihood of the drawn token under the model (log-softmax at temperature 1 of the unfiltered logits), at a
     # given position the teacher-forced log-likelihood of the given token within this window.  The result is then
     # (x, logprobs), or (x, preds, logprobs) with get_preds.  The tokens are those of the same call without it.
+    # select_every=k, select_keep=m (not in the reference; keep-best selection): after every k drawn tokens the rows are
+    # ranked by the log-likelihood of the tokens they drew in this window (keep_best_parents), the m likeliest keep
+    # their rows and the others continue copies of them (SamplingWindow.select).  The result then ends with ancestry,
+    # LongTensor [N]: the input item each returned row descends from.
     def sample(self, n_samples, x_cond=None, y_cond=None, encoder_kv=None, fp16=False, temp=1.0, top_k=0,
-               top_p=0.0, get_preds=False, sample_tokens=None, get_logprobs=False):
+               top_p=0.0, get_preds=False, sample_tokens=None, get_logprobs=False, select_every=None, select_keep=None):
         prime = t.zeros(n_samples, 0, dtype=t.long, device=self.x_emb.weight.device)
         return self._run(n_samples, prime, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds,
-                         sample_tokens, get_logprobs)
+                         sample_tokens, get_logprobs, select_every, select_keep)
 
     def primed_sample(self, n_samples, x, x_cond=None, y_cond=None, encoder_kv=None, fp16=False, temp=1.0,
-                      top_k=0, top_p=0.0, get_preds=False, chunk_size=None, sample_tokens=None, get_logprobs=False):
+                      top_k=0, top_p=0.0, get_preds=False, chunk_size=None, sample_tokens=None, get_logprobs=False,
+                      select_every=None, select_keep=None):
         """`chunk_size` is accepted for compatibility: the prefill runs token by token through the
-        same persistent kernel, which is what chunked prefill computes (reference check_chunks)."""
+        same persistent kernel, which is what chunked prefill computes (reference check_chunks).
+        x may be one row for n_samples > 1 (not in the reference): one prime, n_samples continuations.  x_cond, y_cond
+        and encoder_kv then have one row as well; the prime is run once and its state repeated to every row, whose draws
+        still differ (the sampler's random stream is keyed by row)."""
         with t.no_grad():
             x = self.preprocess(x)
-        assert x.shape[0] == n_samples
+        assert x.shape[0] == n_samples or (x.shape[0] == 1 and x.shape[1] > 0), \
+            f"prime of {x.shape[0]} rows for {n_samples} samples: give n_samples rows, or one row of given tokens"
         return self._run(n_samples, x, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds,
-                         sample_tokens, get_logprobs)
+                         sample_tokens, get_logprobs, select_every, select_keep)
 
     def logprob(self, x, x_cond=None, y_cond=None, encoder_kv=None, fp16=True):
         """log-likelihood in nats of every token of whole sequences x [N, input_dims] given the ones before it, fp32
@@ -371,58 +381,151 @@ class ConditionalAutoregressive2D(nn.Module):
         tr.del_cache()
 
 
-class SamplingWindow:
+def keep_best_parents(scores, keep):
+    """Keep-best selection of a window's rows: rows ranked by score (the log-likelihood of the tokens each drew so far,
+    highest first, ties to the lower row; nan ranks last), the `keep` best keep their rows and every other row, in
+    ascending order, becomes a copy of the kept rows taken round-robin in rank order.  Returns parents: row b continues
+    row parents[b] (SamplingWindow.select)."""
+    scores = [float(v) for v in scores]
+    N = len(scores)
+    assert 1 <= int(keep) <= N, f"select_keep {keep} outside [1, {N}]"
+    order = sorted(range(N), key=lambda r: (-scores[r] if scores[r] == scores[r] else float("inf"), r))
+    kept = order[:int(keep)]
+    parents = list(range(N))
+    for i, r in enumerate(sorted(set(range(N)) - set(kept))):
+        parents[r] = kept[i % len(kept)]
+    return parents
+
+
+class _Rows:
+    """The per-item state shared by both sampling windows: the rows' tokens / log-probabilities / logits and
+    conditioning, which rows run (one row while a one-row prime is given, then every row), the rows' ancestry, and
+    keep-best selection.  A subclass owns the K / V caches (_select_caches)."""
+
+    def _init_rows(self, ca, n_samples, prime, x_cond, y_cond, sample_tokens, get_preds, get_logprobs, select_every,
+                   select_keep):
+        self.ca = ca
+        self.sample_tokens = ca.input_dims if sample_tokens is None else int(sample_tokens)
+        self.N = N = n_samples
+        self.P = P = prime.shape[1]
+        assert P < self.sample_tokens <= ca.input_dims, \
+            f"need given tokens {P} < sample_tokens {self.sample_tokens} <= input_dims {ca.input_dims}"
+        # one given row for N samples: its positions run on one row, then its state is repeated to all N (_fan_out)
+        self.n = prime.shape[0] if P else N
+        assert self.n in (1, N), f"prime of {self.n} rows for {N} samples"
+        self.x_cond, self.y_cond = ca._check_conds(self.n, x_cond, y_cond)
+        dev = ca.x_emb.weight.device
+        self.tokens = t.zeros(N, self.sample_tokens, dtype=t.long, device=dev)
+        if P:
+            assert (0 <= prime).all() and (prime < ca.bins).all()
+            self.tokens[:, :P] = prime
+        if (select_every is None) != (select_keep is None):
+            raise ValueError("keep-best selection needs both select_every and select_keep")
+        if select_every is not None:
+            if not (int(select_every) >= 1 and 1 <= int(select_keep) <= N):
+                raise ValueError(f"select_every {select_every} must be >= 1 and select_keep {select_keep} in [1, {N}]")
+            select_every, select_keep = int(select_every), int(select_keep)
+        self.select_every, self.select_keep = select_every, select_keep
+        self.ancestry = t.arange(N, device=dev)
+        self.get_preds = get_preds
+        self.preds = t.empty(N, self.sample_tokens, ca.bins, dtype=t.float32, device=dev) if get_preds else None
+        # selection ranks rows by the log-likelihoods of their draws, which the sampling launch scores (get_logprobs)
+        self.get_logprobs = get_logprobs
+        self.scored = bool(get_logprobs or select_every)
+        self.logprobs = t.zeros(N, self.sample_tokens, dtype=t.float32, device=dev) if self.scored else None
+        # the key of this call's Philox stream comes from torch's default generator, so t.manual_seed /
+        # seed_per_rank make sampling reproducible exactly as they do for the reference's Categorical
+        self.seed = int(t.empty((), dtype=t.int64).random_().item())
+        self.pos = 0
+        self.fbuf = None
+        self.logit_bias = None
+        self._owned = {"tokens", "logprobs", "preds", "logit_bias"}     # tensors this window made itself
+
+    def select(self, parents):
+        """row b of the window becomes a copy of row parents[b] (b < N, parents[b] < the rows now running): its K / V
+        caches and every per-item tensor the window holds (tokens, logprobs, preds, x_cond, y_cond, logit_bias), and
+        its ancestry.  The window goes on from the same position."""
+        parents = [int(v) for v in (parents.tolist() if isinstance(parents, t.Tensor) else parents)]
+        if len(parents) != self.N or not all(0 <= v < self.n for v in parents):
+            raise ValueError(f"parents {parents}: need {self.N} rows, each in [0, {self.n})")
+        self._select_caches(parents)
+        idx = t.tensor(parents, dtype=t.long, device=self.tokens.device)
+        moved = [b for b, v in enumerate(parents) if v != b]
+        with t.no_grad():
+            for name in ("tokens", "logprobs", "preds", "x_cond", "y_cond", "logit_bias", "encoder_kv"):
+                v = getattr(self, name, None)
+                if v is None:
+                    continue
+                if v.shape[0] == self.N and moved:      # in place, only the rows that change
+                    if name not in self._owned:        # the caller's conditioning is copied, never written
+                        v = v.clone()
+                        setattr(self, name, v)
+                        self._owned.add(name)
+                    m = t.tensor(moved, dtype=t.long, device=v.device)
+                    v[m] = v[idx[m].to(v.device)]
+                elif v.shape[0] != self.N:              # a one-row tensor repeated to the N rows
+                    setattr(self, name, v[idx.to(v.device)].contiguous())
+                    self._owned.add(name)
+            self.ancestry = self.ancestry[idx]
+        self.n = self.N
+
+    def _fan_out(self):
+        """the given positions of a one-row prime are done: every row continues from it"""
+        self.select([0] * self.N)
+
+    def _drawn(self, sample_t, x):
+        """position sample_t of the running rows from their logits x [n, bins], then keep-best selection when the
+        window has drawn a multiple of select_every tokens"""
+        _draw(self, x, sample_t, sample_t >= self.P)
+        if self.select_every and sample_t >= self.P and (sample_t + 1 - self.P) % self.select_every == 0:
+            scores = self.logprobs[:, self.P:sample_t + 1].double().sum(1).cpu()
+            parents = keep_best_parents(scores.tolist(), self.select_keep)
+            if parents != list(range(self.N)):
+                self.select(parents)
+
+    def _result(self, x):
+        out = (x,) + ((self.preds,) if self.get_preds else ()) + ((self.logprobs,) if self.get_logprobs else ()) + \
+              ((self.ancestry,) if self.select_every else ())
+        return out[0] if len(out) == 1 else out
+
+
+class SamplingWindow(_Rows):
     """One sampling window in flight on the decode engine: the body of the reference's sample loop
     (prior/autoregressive.py:222-237, 300-345) split into begin / advance / finish, so that callers which
     need the window in pieces (bench.py times 1/8-window slices) drive the same code as `sample`.
 
     begin (constructor): caches emptied, encoder K/V loaded, the given tokens prefilled in one pass when the
     engine can (else they are stepped by `advance`).  advance(upto): one decode launch + one sampling launch
-    per position, nothing synchronises with the host.  finish(): cache bookkeeping + postprocess."""
+    per position, nothing synchronises with the host.  finish(): cache bookkeeping + postprocess.
+    A prime of one row for N samples is prefilled (or stepped) on one row and then copied to the N rows on the engine
+    (select); keep-best selection (select_every / select_keep) reorders the rows every select_every drawn tokens."""
 
     def __init__(self, ca, n_samples, prime, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds,
-                 sample_tokens, get_logprobs=False):
+                 sample_tokens, get_logprobs=False, select_every=None, select_keep=None):
         assert ca.training is False
         assert not ca.only_encode
         assert fp16, "SamplingWindowF32 is the fp32 loop"
-        self.ca = ca
-        self.sample_tokens = ca.input_dims if sample_tokens is None else int(sample_tokens)
-        self.N = N = n_samples
-        self.x_cond, self.y_cond = ca._check_conds(N, x_cond, y_cond)
-        self.P = P = prime.shape[1]
-        assert P < self.sample_tokens <= ca.input_dims, \
-            f"need given tokens {P} < sample_tokens {self.sample_tokens} <= input_dims {ca.input_dims}"
+        self._init_rows(ca, n_samples, prime, x_cond, y_cond, sample_tokens, get_preds, get_logprobs, select_every,
+                        select_keep)
+        N, n, P = self.N, self.n, self.P
         dev = ca.x_emb.weight.device
         self.eng = eng = ca._fresh_engine(N, encoder_kv)
+        if encoder_kv is not None:
+            assert encoder_kv.shape[0] == n, f"encoder_kv of {encoder_kv.shape[0]} rows for {n} given rows"
         self.tr = ca.transformer
-        self.tokens = t.zeros(N, self.sample_tokens, dtype=t.long, device=dev)
-        if P:
-            assert (0 <= prime).all() and (prime < ca.bins).all()
-            self.tokens[:, :P] = prime
-        self.get_preds = get_preds
         if get_preds:
-            self.preds = t.empty(N, self.sample_tokens, ca.bins, dtype=t.float32, device=dev)
             self.lbuf, self.tstride = self.preds, ca.bins
         else:
-            self.preds = None
             self.lbuf, self.tstride = t.empty(N, ca.bins, dtype=t.float32, device=dev), 0
-        self.get_logprobs = get_logprobs
-        self.logprobs = t.zeros(N, self.sample_tokens, dtype=t.float32, device=dev) if get_logprobs else None
         self.temp, self.top_k, self.top_p, self.fp16 = temp, top_k, top_p, fp16
-        # the key of this call's Philox stream comes from torch's default generator, so t.manual_seed /
-        # seed_per_rank make sampling reproducible exactly as they do for the reference's Categorical
-        self.seed = int(t.empty((), dtype=t.int64).random_().item())
-        self.pos = 0
-        self.fbuf = None
         # x_cond is added BEHIND the stack (autoregressive.py:226-227) and the logits are linear in the activation:
         # x_cond . x_out^T of every position is computed once per window, so that the engine's logits product can take
         # the fp16-valued h on the tensor cores and add this bias in its epilogue (jkb200.h: jk_step_args.logit_bias)
-        self.logit_bias = None
         if ca.add_cond_after_transformer and self.x_cond is not None and eng.has_logits_gemm:
             from ..transformer import f32
             with t.no_grad():
                 Lc = self.x_cond.shape[1]
-                self.logit_bias = f32.linear_nk(self.x_cond.reshape(N * Lc, ca.width), ca.x_out.weight).view(N, Lc, ca.bins)
+                self.logit_bias = f32.linear_nk(self.x_cond.reshape(n * Lc, ca.width), ca.x_out.weight).view(n, Lc, ca.bins)
         with t.no_grad():
             if 1 < P <= eng.prefill_capacity:
                 # the given tokens go through all layers at once (the reference's chunked primed_sample,
@@ -431,30 +534,36 @@ class SamplingWindow:
                 # their log-likelihoods come from the same activations through the fused x_out + log-softmax kernel
                 if get_preds or get_logprobs:
                     from ..transformer import f32
-                    h = t.empty(N, P, ca.width, dtype=t.float32, device=dev)
-                    eng.prefill(N, P, tokens=self.tokens, y_cond=self.y_cond, x_cond=self.x_cond, h_out=h)
+                    h = t.empty(n, P, ca.width, dtype=t.float32, device=dev)
+                    eng.prefill(n, P, tokens=self.tokens, y_cond=self.y_cond, x_cond=self.x_cond, h_out=h)
                     h = ca._add_x_cond(h, self.x_cond, 0, P)
                     if get_preds:
-                        self.preds[:, :P] = f32.linear_nk(h.view(N * P, ca.width), ca.x_out.weight).view(N, P, ca.bins)
+                        self.preds[:n, :P] = f32.linear_nk(h.view(n * P, ca.width), ca.x_out.weight).view(n, P, ca.bins)
                     if get_logprobs:
                         from ..score import xout_logprob
-                        self.logprobs[:, :P] = xout_logprob(h.view(N * P, ca.width), ca.x_out.weight,
-                                                            self.tokens[:, :P].reshape(-1)).view(N, P)
+                        self.logprobs[:n, :P] = xout_logprob(h.view(n * P, ca.width), ca.x_out.weight,
+                                                             self.tokens[:n, :P].reshape(-1)).view(n, P)
                 else:
-                    eng.prefill(N, P, tokens=self.tokens, y_cond=self.y_cond, x_cond=self.x_cond)
+                    eng.prefill(n, P, tokens=self.tokens, y_cond=self.y_cond, x_cond=self.x_cond)
                 self.pos = P
+
+    def _select_caches(self, parents):
+        self.eng.select(parents)
 
     def advance(self, upto):
         """positions [self.pos, upto): given positions are teacher-forced, the others sampled"""
         upto = min(int(upto), self.sample_tokens)
-        eng, N, P, tokens = self.eng, self.N, self.P, self.tokens
+        eng, P, tokens = self.eng, self.P, self.tokens
         with t.no_grad():
             for sample_t in get_range(range(self.pos, upto)):
-                need = self.get_preds or self.get_logprobs or sample_t >= P
-                eng.step(N, tokens=tokens, y_cond=self.y_cond, x_cond=self.x_cond,
+                if sample_t >= P and self.n < self.N:
+                    self._fan_out()
+                n = self.n
+                need = self.get_preds or self.scored or sample_t >= P
+                eng.step(n, tokens=tokens, y_cond=self.y_cond, x_cond=self.x_cond,
                          logits=self.lbuf if need else None, logits_tstride=self.tstride, logit_bias=self.logit_bias)
-                x = self.preds[:, sample_t] if self.get_preds else self.lbuf
-                _draw(self, x, sample_t, sample_t >= P)
+                x = self.preds[:n, sample_t] if self.get_preds else self.lbuf[:n]
+                self._drawn(sample_t, x)
         self.pos = max(self.pos, upto)
 
     def finish(self):
@@ -466,77 +575,82 @@ class SamplingWindow:
             tr.check_cache(self.N, self.sample_tokens, self.fp16)
             tr.del_cache()
             x = self.ca.postprocess(self.tokens, self.sample_tokens)
-        return _result(self, x)
+        return self._result(x)
 
 
 def _draw(win, x, sample_t, drawn):
-    """position sample_t of a window from its logits x [N, bins]: the draw (x / temp -> top-k / nucleus filter, ops.py:
-    113-142, one launch -> Categorical), and with get_logprobs the log-likelihood of the drawn or given token under x,
-    from the same sampling launch"""
-    if not drawn and not win.get_logprobs:
+    """position sample_t of a window's running rows (the first win.n) from their logits x [n, bins]: the draw (x / temp
+    -> top-k / nucleus filter, ops.py:113-142, one launch -> Categorical), and when the window scores its draws
+    (get_logprobs, keep-best selection) the log-likelihood of the drawn or given token under x, from the same sampling
+    launch"""
+    if not drawn and not win.scored:
         return
+    n = x.shape[0]
     samp, temp = x, win.temp
     if drawn and (win.top_k or win.top_p):
         win.fbuf = filter_logits_scaled(x, win.temp, win.top_k, win.top_p, win.fbuf)
         samp, temp = win.fbuf, 1.0
-    if win.get_logprobs:
-        sample_categorical_scored(samp if drawn else None, x, temp, win.seed, sample_t, win.tokens, win.logprobs)
+    if win.scored:
+        sample_categorical_scored(samp if drawn else None, x, temp, win.seed, sample_t, win.tokens[:n], win.logprobs[:n])
     else:
-        sample_categorical(samp, temp, win.seed, sample_t, win.tokens)
+        sample_categorical(samp, temp, win.seed, sample_t, win.tokens[:n])
 
 
-def _result(win, x):
-    out = (x,) + ((win.preds,) if win.get_preds else ()) + ((win.logprobs,) if win.get_logprobs else ())
-    return out[0] if len(out) == 1 else out
-
-
-class SamplingWindowF32:
+class SamplingWindowF32(_Rows):
     """sample(fp16=False) / primed_sample(fp16=False): the same loop on the fp32 path (csrc/f32_path.cu) - embedding
     row, all layers on fp32 K/V caches, + cond, x_out in fp32, then the shared filter / Categorical kernels.  Four C-ABI
-    calls per token instead of one persistent kernel: exactness path, not the hot path (train.py:139 sample logging)."""
+    calls per token instead of one persistent kernel: exactness path, not the hot path (train.py:139 sample logging).
+    Its caches are torch tensors (F32Path.caches), which select indexes."""
 
     def __init__(self, ca, n_samples, prime, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds,
-                 sample_tokens, get_logprobs=False):
+                 sample_tokens, get_logprobs=False, select_every=None, select_keep=None):
         assert ca.training is False and not ca.only_encode and not fp16
-        self.ca = ca
-        self.sample_tokens = ca.input_dims if sample_tokens is None else int(sample_tokens)
-        self.N = N = n_samples
-        self.x_cond, self.y_cond = ca._check_conds(N, x_cond, y_cond)
-        self.P = P = prime.shape[1]
-        assert P < self.sample_tokens <= ca.input_dims, \
-            f"need given tokens {P} < sample_tokens {self.sample_tokens} <= input_dims {ca.input_dims}"
-        dev = ca.x_emb.weight.device
+        self._init_rows(ca, n_samples, prime, x_cond, y_cond, sample_tokens, get_preds, get_logprobs, select_every,
+                        select_keep)
         self.tr = ca.transformer
         self.tr.del_cache()
+        if encoder_kv is not None:
+            assert encoder_kv.shape[0] == self.n, f"encoder_kv of {encoder_kv.shape[0]} rows for {self.n} given rows"
         self.encoder_kv = encoder_kv
-        self.tokens = t.zeros(N, self.sample_tokens, dtype=t.long, device=dev)
-        if P:
-            assert (0 <= prime).all() and (prime < ca.bins).all()
-            self.tokens[:, :P] = prime
-        self.get_preds = get_preds
-        self.preds = t.empty(N, self.sample_tokens, ca.bins, dtype=t.float32, device=dev) if get_preds else None
-        self.get_logprobs = get_logprobs
-        self.logprobs = t.zeros(N, self.sample_tokens, dtype=t.float32, device=dev) if get_logprobs else None
         self.temp, self.top_k, self.top_p = temp, top_k, top_p
-        self.seed = int(t.empty((), dtype=t.int64).random_().item())
-        self.pos = 0
-        self.fbuf = None
+
+    def _select_caches(self, parents):
+        path = self.tr.f32_path()
+        if path.caches is None:
+            return
+        idx = t.tensor(parents, dtype=t.long, device=path.dev)
+        moved = t.tensor([b for b, v in enumerate(parents) if v != b], dtype=t.long, device=path.dev)
+        for i, (k, v) in enumerate(path.caches):
+            if k.shape[0] == self.N:
+                if moved.numel():
+                    k[moved], v[moved] = k[idx[moved]], v[idx[moved]]
+            else:
+                k, v = k[idx].contiguous(), v[idx].contiguous()
+                path.caches[i] = (k, v)
+                path.layers[i].k_cache, path.layers[i].v_cache = k.data_ptr(), v.data_ptr()
+        path.cache_n = self.N
+        for b in self.tr._attn_mods:
+            if b.attn.cache:
+                b.attn.cache["n_samples"] = self.N
 
     def advance(self, upto):
         from ..transformer import f32
-        ca, N, P, tokens = self.ca, self.N, self.P, self.tokens
+        ca, P, tokens = self.ca, self.P, self.tokens
         upto = min(int(upto), self.sample_tokens)
         with t.no_grad():
             for sample_t in get_range(range(self.pos, upto)):
-                self.tr.check_cache(N, sample_t, False)
-                h = f32.embed(ca, tokens, self.y_cond, self.x_cond, N, 1, sample_t)
+                if sample_t >= P and self.n < self.N:
+                    self._fan_out()
+                n = self.n
+                self.tr.check_cache(n, sample_t, False)
+                h = f32.embed(ca, tokens, self.y_cond, self.x_cond, n, 1, sample_t)
                 h = self.tr(h, encoder_kv=self.encoder_kv, sample=True, fp16=False)
                 h = ca._add_x_cond(h, self.x_cond, sample_t, sample_t + 1)
-                if self.get_preds or self.get_logprobs or sample_t >= P:
-                    x = f32.linear_nk(h.view(N, ca.width), ca.x_out.weight)
+                if self.get_preds or self.scored or sample_t >= P:
+                    x = f32.linear_nk(h.view(n, ca.width), ca.x_out.weight)
                     if self.get_preds:
-                        self.preds[:, sample_t] = x
-                    _draw(self, x, sample_t, sample_t >= P)
+                        self.preds[:n, sample_t] = x
+                    self._drawn(sample_t, x)
         self.pos = max(self.pos, upto)
 
     def finish(self):
@@ -545,4 +659,4 @@ class SamplingWindowF32:
             self.tr.check_cache(self.N, self.sample_tokens, False)
             self.tr.del_cache()
             x = self.ca.postprocess(self.tokens, self.sample_tokens)
-        return _result(self, x)
+        return self._result(x)

@@ -227,20 +227,28 @@ class SimplePrior(nn.Module):
 
     # ---- sampling -----------------------------------------------------------------------------------------------
     def sample(self, n_samples, z=None, z_conds=None, y=None, fp16=False, temp=1.0, top_k=0, top_p=0.0,
-               chunk_size=None, sample_tokens=None, get_logprobs=False):
+               chunk_size=None, sample_tokens=None, get_logprobs=False, select_every=None, select_keep=None):
         """one window: z = codes of this level already in the window (None / empty: ancestral), z_conds = codes of the
         level above, y = label rows.  Returns the codes [N, sample_tokens or n_ctx].  With get_logprobs it returns
         (codes, logprobs): fp32 [N, sample_tokens or n_ctx], the log-likelihood in nats of each returned code under the
-        model (ConditionalAutoregressive2D.sample), so that the samples of a window can be ranked."""
-        for name, v in (("z", z), ("y", y), *((f"z_conds[{i}]", c) for i, c in enumerate(z_conds or []))):
-            assert v is None or v.shape[0] == n_samples, f"{name}: expected batch {n_samples}, got {tuple(v.shape)}"
+        model (ConditionalAutoregressive2D.sample), so that the samples of a window can be ranked.
+        z of one row with n_samples > 1 (not in the reference): one prime, n_samples continuations; z_conds and y then
+        have one row too, and the window runs the prime once (ConditionalAutoregressive2D.primed_sample).
+        select_every / select_keep: keep-best selection inside the window (ConditionalAutoregressive2D.sample); the
+        result then ends with ancestry, LongTensor [N], the input item each returned row descends from."""
         fresh = z is None or z.shape[1] == 0
+        rows = 1 if (not fresh and z.shape[0] == 1) else n_samples
+        for name, v in (("z", z), ("y", y), *((f"z_conds[{i}]", c) for i, c in enumerate(z_conds or []))):
+            assert v is None or v.shape[0] == rows, \
+                f"{name}: expected batch {rows}{' (one given row)' if rows != n_samples else ''}, got {tuple(v.shape)}"
         if dist.get_rank() == 0:
             print(f"{'Ancestral' if fresh else 'Primed'} sampling {n_samples} samples with temp={temp}, "
                   f"top_k={top_k}, top_p={top_p}")
         how = dict(fp16=fp16, temp=temp, top_k=top_k, top_p=top_p)
         if get_logprobs:
             how["get_logprobs"] = True
+        if select_every is not None or select_keep is not None:
+            how.update(select_every=select_every, select_keep=select_keep)
         with t.no_grad():
             x_cond, y_cond, lyric = self.get_cond(z_conds, y)
             if self.single_enc_dec:
@@ -248,7 +256,7 @@ class SimplePrior(nn.Module):
             else:
                 out = self._sample_separate(n_samples, None if fresh else z, lyric, x_cond, y_cond, chunk_size, sample_tokens, how)
         if sample_tokens is None:
-            assert_shape(out[0] if get_logprobs else out, (n_samples, *self.z_shape))
+            assert_shape(out[0] if isinstance(out, tuple) else out, (n_samples, *self.z_shape))
         return out
 
     def _sample_joint(self, N, z, lyric, x_cond, y_cond, chunk_size, sample_tokens, how):
@@ -256,11 +264,13 @@ class SimplePrior(nn.Module):
         given = [lyric] if z is None else [lyric, z]
         seq, cond = self.spaces.merge(given, [None, x_cond])
         total = None if sample_tokens is None else sample_tokens + self.n_tokens
-        seq = self.prior.primed_sample(N, seq, cond, y_cond, chunk_size=chunk_size, sample_tokens=total, **how)
+        out = self.prior.primed_sample(N, seq, cond, y_cond, chunk_size=chunk_size, sample_tokens=total, **how)
+        if not isinstance(out, tuple):
+            return self.spaces.last(out)
+        seq, *rest = out
         if how.get("get_logprobs"):
-            seq, lp = seq
-            return self.spaces.last(seq), lp[:, sum(self.spaces.dims[:-1]):]     # the lyric head stripped as from the codes
-        return self.spaces.last(seq)
+            rest[0] = rest[0][:, sum(self.spaces.dims[:-1]):]     # the lyric head stripped as from the codes
+        return (self.spaces.last(seq), *rest)
 
     def _sample_separate(self, N, z, lyric, x_cond, y_cond, chunk_size, sample_tokens, how):
         enc = self.get_encoder_kv(lyric, fp16=how["fp16"], sample=True)

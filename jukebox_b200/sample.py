@@ -80,11 +80,33 @@ class LevelRun:
         if missing <= 0:
             return
         extra = {} if win.sample_tokens == prior.n_ctx else dict(sample_tokens=win.sample_tokens)
-        done = [prior.sample(n_samples=ctx_i.shape[0], z=ctx_i, z_conds=upper_i, y=y_i, **self.opts, **extra)
-                for ctx_i, upper_i, y_i in window_pieces(prior, self.zs, self.labels, level, win.start,
-                                                         win.start + prior.n_ctx, self.max_batch)]
+        selecting = self.opts.get('select_every') is not None
+        done, i0 = [], 0
+        for ctx_i, upper_i, y_i in window_pieces(prior, self.zs, self.labels, level, win.start,
+                                                 win.start + prior.n_ctx, self.max_batch):
+            n = ctx_i.shape[0]
+            if selecting and y_i is not None and not bool((y_i == y_i[:1]).all()):
+                raise ValueError(f"keep-best selection (select_every) copies samples into other samples' rows, but items "
+                                 f"{i0}..{i0 + n - 1} have different labels, which the other levels' labels cannot "
+                                 "follow: give the items of a batch piece one set of labels, or sample without selection")
+            out = prior.sample(n_samples=n, z=ctx_i, z_conds=upper_i, y=y_i, **self.opts, **extra)
+            if selecting:
+                out, ancestry = out
+                self.follow(ancestry, i0)
+            done.append(out)
+            i0 += n
         fresh = t.cat(done, dim=0)[:, -missing:]
         self.zs[level] = t.cat([self.zs[level], fresh], dim=1)
+
+    def follow(self, ancestry, i0):
+        """rows i0 .. i0 + len(ancestry) of a window now descend from those input items: the codes of every level (this
+        level's earlier windows and the upper levels' codes under them) follow their item"""
+        n = ancestry.shape[0]
+        for lv, z in enumerate(self.zs):
+            if z.shape[0] and z.shape[1]:
+                z = z.clone()
+                z[i0:i0 + n] = z[i0:i0 + n][ancestry.to(z.device)]
+                self.zs[lv] = z
 
     def extend_to(self, total_length, hop_length):
         for win in plan_windows(self.have(), total_length, self.prior.n_ctx, hop_length):
