@@ -181,7 +181,14 @@ typedef struct jk_act_capture {
  * the engine stands at position n_positions (K/V caches filled), exactly as after that many jk_prior_step
  * calls.  tokens[b * tok_stride + t] is the token AT position t (the input of position t+1), as in
  * jk_step_args; h_out (optional, fp32 [n_samples, n_positions, width]) receives the transformer output -
- * the `only_encode` forward of the lyric encoder (prior/prior.py:285-301). */
+ * the `only_encode` forward of the lyric encoder (prior/prior.py:285-301).
+ * Continuation: an engine at position t0 > 0 (after steps, a prefill or a jk_prior_select) runs positions
+ * t0 .. t0+n_positions-1 of its first n_samples rows on top of their K/V caches and then stands at t0 + n_positions,
+ * as after that many more jk_prior_step calls.  Row i of h_out is then position t0 + i; the embedding of position t
+ * reads tokens[b * tok_stride + t - 1], pos_emb and x_cond (x_cond_len n_ctx) at t, and y_cond is not read (it feeds
+ * position 0 only).  t0 + n_positions > n_ctx, n_positions beyond the capacity, an engine whose last prefill stopped
+ * early, and record, capture or a truncating n_layers with t0 > 0 are errors: nothing is launched and the position
+ * stays. */
 typedef struct jk_prefill_args {
     int32_t n_samples;
     int32_t n_positions;
@@ -234,6 +241,16 @@ typedef struct jk_prefill_attn_args {
     int32_t attn_func, bc, prime;      /* bc: block length (1, 2, 3); prime: the padded prime length (7) */
     int32_t enc_rows;                  /* attn_func 6: encoder rows of the caches */
     int32_t route;                     /* 0: the prefill's own choice of kernel; 1: the scalar kernels */
+    /* Continuation (q_offset > 0 or cache_rows > 0), as jk_prior_prefill runs an engine at position q_offset: query row
+     * i is position q_offset + i, and the keys (and values) of every pattern are read from k_cache / v_cache,
+     * fp16 [n][heads][cache_rows][dh_pad] in the decode engine's layout (DESIGN §4): position p's keys are cache rows
+     * base(p) + j, j < the pattern's key count at p, with base 0 (0, 1, 7), (p % bc) * blocks (2) or
+     * ((p / bc + 1) % 2) * bc (3).  qkv then holds q only in its first third (K / V columns are not read).  w must be
+     * NULL; cache_rows must cover the rows the pattern reads, and attn_func 2 needs blocks >= 1 with
+     * q_offset + P <= bc * blocks.  Both 0: the head of a window, as above. */
+    int32_t q_offset;
+    int32_t cache_rows;
+    int32_t blocks;
 } jk_prefill_attn_args;
 /* the kernels a call ran: tensor_cores 0 = the scalar kernels (tile_dh, stage_bytes 0); 1 = mma.sync kernels of head
  * tile tile_dh (32, 64, 128, 160, 256) staging K / V in stage_bytes (16 or 4) chunks */
@@ -243,8 +260,8 @@ typedef struct jk_prefill_attn_route {
     int32_t stage_bytes;
 } jk_prefill_attn_route;
 /* qkv, out and the caches must be 16-byte aligned; neither out nor w, an unknown attn_func, a pattern parameter < 1,
- * dh > dh_pad or dh_pad % 16 != 0, or a scalar-route shape with (dh + max(P, enc_rows)) * 4 > 64 KB is an error, and
- * nothing is written.  taken (may be NULL) receives the route. */
+ * dh > dh_pad or dh_pad % 16 != 0, or a scalar-route shape with (dh + max(q_offset + P, enc_rows)) * 4 > 64 KB is an
+ * error, and nothing is written.  taken (may be NULL) receives the route. */
 int jk_prefill_attention_f16(const jk_prefill_attn_args* a, jk_prefill_attn_route* taken, jk_stream_t stream);
 
 /* one token position; increments the device-side position counter */

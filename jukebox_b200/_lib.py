@@ -78,7 +78,8 @@ class PrefillArgs(C.Structure):
 class PrefillAttnArgs(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("qkv", "k_cache", "v_cache", "out", "w")] + \
                [(n, C.c_int32) for n in
-                ("ld", "n", "P", "heads", "dh", "dh_pad", "attn_func", "bc", "prime", "enc_rows", "route")]
+                ("ld", "n", "P", "heads", "dh", "dh_pad", "attn_func", "bc", "prime", "enc_rows", "route", "q_offset",
+                 "cache_rows", "blocks")]
 
 
 class PrefillAttnRoute(C.Structure):

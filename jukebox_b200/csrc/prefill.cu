@@ -16,6 +16,11 @@
 //   x   = x1 + (g . W2 + b)           gemm_f16_tc epi 2         (transformer.py:83)
 // Afterwards the engine stands at position P exactly as if P decode steps had run: only the K/V caches and
 // the position carry over between steps.
+//
+// A continuation (engine at t0 > 0) runs positions t0 .. t0+P-1 on top of the rows' caches: row m = b*P + i is position
+// t0 + i.  Its queries attend FROM the cache (the decode layout, where every pattern's keys are one run of rows), after
+// the new K / V are scattered into it: the whole chunk first for the layouts with a row per position (0, 2, 7), block
+// by block for the rings (1 keeps one block, 3 two), whose rows a later block of the chunk overwrites.
 #include "engine.cuh"
 #include <algorithm>
 
@@ -26,14 +31,15 @@ namespace {
 __device__ __forceinline__ float ldh(const __half* p) { return __half2float(*p); }
 
 // ---- embedding (autoregressive.py:177-197; decode_engine.cu phase P0) ---------------------------------
+// row m = b*P + i is position t0 + i of sample b
 __global__ void embed_rows_kernel(__half* __restrict__ x, const long long* __restrict__ tokens, long long tok_stride,
                                   const float* __restrict__ y_cond, const float* __restrict__ x_cond, long long x_cond_len,
                                   const float* __restrict__ x_emb, const float* __restrict__ pos_emb,
-                                  const float* __restrict__ start_token, int n, int P, int W) {
+                                  const float* __restrict__ start_token, int n, int P, int t0, int W) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (size_t)n * P * W) return;
     const int col = (int)(i % W);
-    const int m = (int)(i / W), b = m / P, t = m % P;
+    const int m = (int)(i / W), b = m / P, t = t0 + m % P;
     float v;
     if (t == 0) v = y_cond ? y_cond[(size_t)b * W + col] : start_token[col];
     else v = x_emb[(size_t)tokens[(size_t)b * tok_stride + t - 1] * W + col];
@@ -83,13 +89,32 @@ __global__ void ln_rows_kernel(const __half* __restrict__ x, const float* __rest
 //   6 encoder-decoder: every encoder row; K / V come from the layer's cache (jk_prior_set_encoder_kv), q from c_attn
 // Scores fp16(fp16(q.k) * dh^-1/2), softmax fp32, P rounded to fp16 (unnormalised), P.V fp32, / sum - the
 // decode kernel's order of roundings.
+// A continuation (cache = 1) runs queries at absolute positions: row i of qkv is position qoff + i, and this launch
+// computes positions [qa, qb).  Its keys are read from the layer's K / V cache in the decode layout, where the keys of
+// every pattern are one run of rows: key j of position p is cache row cache_row0(p) + j (decode_engine.cu attn_geom).
 struct AttnFwd {
     const __half* qkv;   // [n*P][q_stride]: q | k | v per row (q only for an encoder-decoder layer)
     __half* a;           // [n*P][S]
-    const __half *kc, *vc;   // encoder-decoder layers: the layer's K / V cache [n][H][enc_rows][dhp]
+    const __half *kc, *vc;   // the layer's K / V cache [n][H][rows][dhp] (encoder-decoder: rows = enc_rows)
     int P, S, H, dh, bc, attn_func, prime, q_stride, enc_rows, dhp;
+    int qoff, qa, qb;    // position of qkv row 0 and the positions this launch computes (head of window: 0, 0, P)
+    int cache, rows, blocks;   // keys from the cache (continuation), its rows per (sample, head), n_ctx / bc
     float scale2;
 };
+
+// the first cache row of position p's keys in the decode layout (attn_geom.base)
+__device__ __forceinline__ int cache_row0(const AttnFwd& A, int p) {
+    switch (A.attn_func) {
+        case 2: return (p % A.bc) * A.blocks;
+        case 3: return ((p / A.bc + 1) & 1) * A.bc;
+    }
+    return 0;   // 0, 1, 6, 7
+}
+// keys any position of [qa, qb) reads (shared memory of the scalar kernels)
+__host__ __device__ __forceinline__ int fwd_max_keys(const AttnFwd& A) {
+    const int k = A.cache ? A.qb : A.P;
+    return k > A.enc_rows ? k : A.enc_rows;
+}
 
 __device__ __forceinline__ int fwd_nkeys(const AttnFwd& A, int p) {
     switch (A.attn_func) {
@@ -103,6 +128,7 @@ __device__ __forceinline__ int fwd_nkeys(const AttnFwd& A, int p) {
     return 0;
 }
 __device__ __forceinline__ int fwd_key(const AttnFwd& A, int p, int j) {
+    if (A.cache) return cache_row0(A, p) + j;
     switch (A.attn_func) {
         case 1: return p - p % A.bc + j;
         case 2: return p % A.bc + j * A.bc;
@@ -120,12 +146,13 @@ struct FwdKV {
     size_t kstride;
 };
 __device__ __forceinline__ FwdKV fwd_kv(const AttnFwd& A, int h, int b) {
-    const bool enc = A.attn_func == 6;
+    const bool enc = A.attn_func == 6, cached = enc || A.cache;
     const int S = A.S;
+    const size_t cbase = ((size_t)b * A.H + h) * (enc ? A.enc_rows : A.rows) * A.dhp;
     FwdKV R;
-    R.kbase = enc ? A.kc + ((size_t)b * A.H + h) * A.enc_rows * A.dhp : A.qkv + (size_t)b * A.P * 3 * S + S + h * A.dh;
-    R.vbase = enc ? A.vc + ((size_t)b * A.H + h) * A.enc_rows * A.dhp : R.kbase + S;
-    R.kstride = enc ? (size_t)A.dhp : (size_t)3 * S;
+    R.kbase = cached ? A.kc + cbase : A.qkv + (size_t)b * A.P * 3 * S + S + h * A.dh;
+    R.vbase = cached ? A.vc + cbase : R.kbase + S;
+    R.kstride = cached ? (size_t)A.dhp : (size_t)3 * S;
     return R;
 }
 
@@ -134,7 +161,7 @@ __device__ __forceinline__ float fwd_row_scores(const AttnFwd& A, const FwdKV& R
                                                 float* sc, float* red) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int dh = A.dh;
-    const __half* q = A.qkv + ((size_t)b * A.P + p) * A.q_stride + h * dh;
+    const __half* q = A.qkv + ((size_t)b * A.P + (p - A.qoff)) * A.q_stride + h * dh;
     for (int d = tid; d < dh; d += kFwdThreads) qs[d] = ldh(q + d);
     __syncthreads();
     for (int j = warp; j < nk; j += kFwdThreads / 32) {
@@ -160,10 +187,10 @@ __global__ void __launch_bounds__(kFwdThreads) attn_fwd_kernel(AttnFwd A) {
     float* qs = fsm;                 // [dh]
     float* sc = fsm + A.dh;          // [nk]
     __shared__ float red[kFwdThreads / 32];
-    const int p = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+    const int p = A.qa + blockIdx.x, h = blockIdx.y, b = blockIdx.z;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int dh = A.dh, S = A.S;
-    __half* out = A.a + ((size_t)b * A.P + p) * S + h * dh;
+    __half* out = A.a + ((size_t)b * A.P + (p - A.qoff)) * S + h * dh;
     const FwdKV R = fwd_kv(A, h, b);
     const int nk = fwd_nkeys(A, p);
     if (nk == 0) {
@@ -225,12 +252,42 @@ __global__ void __launch_bounds__(kFwdThreads) attn_record_kernel(AttnFwd A, __h
 // head, sample): 4 warps x 16 query rows, Q fragments in registers, K / V tiles of 32 keys staged with cp.async (gathered
 // rows), online softmax in fp32 with the decode kernel's roundings (score = fp16(fp16(q.k) * dh^-1/2); P rounded to fp16
 // for P.V, the row sum kept in fp32 from the unrounded exponentials).  dh <= DH (zero padded), dh even.
+// A continuation (AttnFwd.cache) has the same sequences over the absolute positions [qa, qb): one per block (1, 3) or
+// residue (2) the range touches, else one; its keys are the cache rows krow0 + j (every pattern's keys are one run of
+// cache rows) and start at position 0 of the window, not of the call.
 struct AttnSeqs {
     int attn_func, bc, P, prime, enc_rows, tiles_per_seq;
+    int cache, qa, qb, blocks;
 };
-struct SeqGeom { int q0, qs, nq, k0, ks, nk; };
-__device__ __forceinline__ SeqGeom seq_geom(const AttnSeqs& Q, int s) {
+struct SeqGeom { int q0, qs, nq, k0, ks, nk, krow0; };
+__device__ __forceinline__ SeqGeom seq_geom_cache(const AttnSeqs& Q, int s) {
     SeqGeom g;
+    g.qs = 1; g.ks = 1; g.k0 = 0; g.krow0 = 0; g.q0 = Q.qa; g.nq = Q.qb - Q.qa;
+    const int bc = Q.bc;
+    switch (Q.attn_func) {
+        case 1: case 3: {
+            const int sb = Q.qa / bc + s;                  // the block of this sequence
+            g.q0 = max(Q.qa, sb * bc); g.nq = max(0, min(Q.qb, (sb + 1) * bc) - g.q0);
+            if (Q.attn_func == 1) { g.k0 = sb * bc; g.nk = g.nq ? g.q0 + g.nq - g.k0 : 0; }
+            else { g.k0 = (sb - 1) * bc; g.nk = sb ? bc : 0; g.krow0 = ((sb + 1) & 1) * bc; }
+            break;
+        }
+        case 2: {
+            g.q0 = Q.qa + s; g.qs = bc; g.nq = g.q0 < Q.qb ? (Q.qb - g.q0 + bc - 1) / bc : 0;
+            const int r = g.q0 % bc;
+            g.k0 = r; g.ks = bc; g.nk = g.nq ? (g.q0 - r) / bc + g.nq : 0; g.krow0 = r * Q.blocks;
+            break;
+        }
+        case 6: g.nk = Q.enc_rows; break;
+        case 7: g.nk = min(Q.prime, Q.qb); break;
+        default: g.nk = Q.qb; break;
+    }
+    return g;
+}
+__device__ __forceinline__ SeqGeom seq_geom(const AttnSeqs& Q, int s) {
+    if (Q.cache) return seq_geom_cache(Q, s);
+    SeqGeom g;
+    g.krow0 = 0;
     switch (Q.attn_func) {
         case 1: g.q0 = s * Q.bc; g.qs = 1; g.nq = min(Q.bc, Q.P - g.q0); g.k0 = g.q0; g.ks = 1; g.nk = g.nq; break;
         case 2: g.q0 = s; g.qs = Q.bc; g.nq = s < Q.P ? (Q.P - s + Q.bc - 1) / Q.bc : 0; g.k0 = s; g.ks = Q.bc; g.nk = g.nq; break;
@@ -261,7 +318,7 @@ constexpr int kBQ = 64, kBK = 32;
 // the tile of 64 queries i0.. of one sequence -> shared memory (zero rows / columns beyond nq / dh) -> this warp's A fragments
 template <int DH, bool W16>
 __device__ __forceinline__ void load_q_frags(uint32_t (&qf)[DH / 16][4], __half* qs, const AttnFwd& A, const SeqGeom& G,
-                                             size_t rowbase, int i0, int h) {
+                                             long long rowbase, int i0, int h) {
     constexpr int XS = DH + 8;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int dh = A.dh, nv = dh >> 3;                       // 16-byte chunks per row
@@ -270,7 +327,7 @@ __device__ __forceinline__ void load_q_frags(uint32_t (&qf)[DH / 16][4], __half*
             const int r = i / (DH / 8), c = i % (DH / 8);
             uint4 v = make_uint4(0, 0, 0, 0);
             if (i0 + r < G.nq && c < nv)
-                v = *reinterpret_cast<const uint4*>(A.qkv + (rowbase + G.q0 + (size_t)(i0 + r) * G.qs) * A.q_stride + h * dh + c * 8);
+                v = *reinterpret_cast<const uint4*>(A.qkv + (size_t)(rowbase + G.q0 + (long long)(i0 + r) * G.qs) * A.q_stride + h * dh + c * 8);
             *reinterpret_cast<uint4*>(qs + r * XS + c * 8) = v;
         }
     } else {
@@ -278,7 +335,7 @@ __device__ __forceinline__ void load_q_frags(uint32_t (&qf)[DH / 16][4], __half*
             const int r = i / (DH / 2), c = i % (DH / 2);
             uint32_t v = 0;
             if (i0 + r < G.nq && 2 * c < dh)
-                v = *reinterpret_cast<const uint32_t*>(A.qkv + (rowbase + G.q0 + (size_t)(i0 + r) * G.qs) * A.q_stride + h * dh + c * 2);
+                v = *reinterpret_cast<const uint32_t*>(A.qkv + (size_t)(rowbase + G.q0 + (long long)(i0 + r) * G.qs) * A.q_stride + h * dh + c * 2);
             *reinterpret_cast<uint32_t*>(qs + r * XS + c * 2) = v;
         }
     }
@@ -294,7 +351,7 @@ struct KeyRange {
     size_t kstride;
     int nk;
 };
-__device__ __forceinline__ KeyRange key_range(const AttnFwd& A, const SeqGeom& G, size_t rowbase, int i0, int h, int b, bool enc) {
+__device__ __forceinline__ KeyRange key_range(const AttnFwd& A, const SeqGeom& G, long long rowbase, int i0, int h, int b, bool enc) {
     KeyRange R;
     // keys beyond the last query of this tile are never needed
     int nk = G.nk;
@@ -304,11 +361,12 @@ __device__ __forceinline__ KeyRange key_range(const AttnFwd& A, const SeqGeom& G
         nk = (int)min((long long)nk, jm);
     }
     const int S = A.S;
-    if (enc) {
-        R.kbase = A.kc + ((size_t)b * A.H + h) * A.enc_rows * A.dhp; R.vbase = A.vc + ((size_t)b * A.H + h) * A.enc_rows * A.dhp;
+    if (enc || A.cache) {        // cache rows krow0 + j
+        const size_t base = (((size_t)b * A.H + h) * (enc ? A.enc_rows : A.rows) + G.krow0) * A.dhp;
+        R.kbase = A.kc + base; R.vbase = A.vc + base;
         R.kstride = (size_t)A.dhp;
     } else {
-        R.kbase = A.qkv + (rowbase + (size_t)(nk > 0 ? G.k0 : 0)) * 3 * S + S + h * A.dh; R.vbase = R.kbase + S;
+        R.kbase = A.qkv + (size_t)(rowbase + (nk > 0 ? G.k0 : 0)) * 3 * S + S + h * A.dh; R.vbase = R.kbase + S;
         R.kstride = (size_t)3 * S * G.ks;
     }
     R.nk = nk;
@@ -410,7 +468,7 @@ __global__ void __launch_bounds__(128) attn_fwd_mma_kernel(AttnFwd A, AttnSeqs Q
     if (i0 >= G.nq) return;
     const int dh = A.dh, S = A.S;
     const bool enc = A.attn_func == 6;
-    const size_t rowbase = (size_t)b * A.P;
+    const long long rowbase = (long long)b * A.P - A.qoff;     // qkv row of position 0
     uint32_t qf[DH / 16][4];
     load_q_frags<DH, W16>(qf, qs, A, G, rowbase, i0, h);
     float o[DH / 8][4];
@@ -461,8 +519,8 @@ __global__ void __launch_bounds__(128) attn_fwd_mma_kernel(AttnFwd A, AttnSeqs Q
     for (int n = 0; n < DH / 8; ++n) {
         const int d = n * 8 + 2 * t4;
         if (d < dh) {
-            if (qi0 < G.nq) *reinterpret_cast<uint32_t*>(A.a + (rowbase + qp0) * S + h * dh + d) = pack_h2(o[n][0] * inv0, o[n][1] * inv0);
-            if (qi1 < G.nq) *reinterpret_cast<uint32_t*>(A.a + (rowbase + qp1) * S + h * dh + d) = pack_h2(o[n][2] * inv1, o[n][3] * inv1);
+            if (qi0 < G.nq) *reinterpret_cast<uint32_t*>(A.a + (size_t)(rowbase + qp0) * S + h * dh + d) = pack_h2(o[n][0] * inv0, o[n][1] * inv0);
+            if (qi1 < G.nq) *reinterpret_cast<uint32_t*>(A.a + (size_t)(rowbase + qp1) * S + h * dh + d) = pack_h2(o[n][2] * inv1, o[n][3] * inv1);
         }
     }
 }
@@ -486,7 +544,7 @@ __global__ void __launch_bounds__(128) attn_record_mma_kernel(AttnFwd A, AttnSeq
     const int i0 = qt * kBQ;
     if (i0 >= G.nq) return;
     const bool enc = A.attn_func == 6;
-    const size_t rowbase = (size_t)b * A.P;
+    const long long rowbase = (long long)b * A.P - A.qoff;     // qkv row of position 0
     uint32_t qf[DH / 16][4];
     load_q_frags<DH, W16>(qf, qs, A, G, rowbase, i0, h);
     const int qi0 = i0 + warp * 16 + g, qi1 = qi0 + 8;
@@ -567,10 +625,12 @@ jk_prefill_attn_route attn_route(const AttnFwd& A, bool scalar) {
 int attn_mma(const AttnFwd& A, const jk_prefill_attn_route& r, int n, __half* w, int ld, cudaStream_t stream) {
     AttnSeqs Q;
     Q.attn_func = A.attn_func; Q.bc = A.bc; Q.P = A.P; Q.prime = A.prime; Q.enc_rows = A.enc_rows;
-    int nseq = 1, maxq = A.P;
+    Q.cache = A.cache; Q.qa = A.qa; Q.qb = A.qb; Q.blocks = A.blocks;
+    const int nq = A.qb - A.qa;          // the head of a window: P
+    int nseq = 1, maxq = nq;
     switch (A.attn_func) {
-        case 1: case 3: nseq = (A.P + A.bc - 1) / A.bc; maxq = std::min(A.bc, A.P); break;
-        case 2: nseq = std::min(A.bc, A.P); maxq = (A.P + A.bc - 1) / A.bc; break;
+        case 1: case 3: nseq = (A.qb - 1) / A.bc - A.qa / A.bc + 1; maxq = std::min(A.bc, nq); break;
+        case 2: nseq = std::min(A.bc, nq); maxq = (nq + A.bc - 1) / A.bc; break;
         default: break;
     }
     Q.tiles_per_seq = (maxq + 63) / 64;
@@ -585,11 +645,12 @@ int attn_mma(const AttnFwd& A, const jk_prefill_attn_route& r, int n, __half* w,
 }
 
 // dynamic shared memory of the scalar kernels: q and one score per key
-size_t scalar_attn_smem(const AttnFwd& A) { return (size_t)(A.dh + std::max(A.P, A.enc_rows)) * 4; }
+size_t scalar_attn_smem(const AttnFwd& A) { return (size_t)(A.dh + fwd_max_keys(A)) * 4; }
 constexpr size_t kScalarAttnSmemMax = 64 * 1024;
 
-// One layer's attention, as the prefill runs it: the forward output into A.a (when set) and, when w is set, the recorded
-// weights w [n][H][P][ld] (zeroed first: entries outside the pattern and rows without keys stay 0).  Both take route r.
+// One layer's attention, as the prefill runs it: the forward output of positions [A.qa, A.qb) into A.a (when set) and,
+// when w is set (head of a window only), the recorded weights w [n][H][P][ld] (zeroed first: entries outside the pattern
+// and rows without keys stay 0).  Both take route r.
 int layer_attention(const AttnFwd& A, const jk_prefill_attn_route& r, int n, __half* w, int ld, cudaStream_t stream) {
     const size_t smem = scalar_attn_smem(A);
     if (!r.tensor_cores) {
@@ -600,7 +661,7 @@ int layer_attention(const AttnFwd& A, const jk_prefill_attn_route& r, int n, __h
         if (r.tensor_cores) {
             if (int rc = attn_mma(A, r, n, nullptr, 0, stream)) return rc;
         } else {
-            attn_fwd_kernel<<<dim3(A.P, A.H, n), kFwdThreads, smem, stream>>>(A);
+            attn_fwd_kernel<<<dim3(A.qb - A.qa, A.H, n), kFwdThreads, smem, stream>>>(A);
             JK_CHECK_CUDA(cudaGetLastError());
         }
     }
@@ -617,26 +678,28 @@ int layer_attention(const AttnFwd& A, const jk_prefill_attn_route& r, int n, __h
 }
 
 // ---- K, V of the given positions -> the caches the decode kernel attends -------------------------------
-// cache row of position p (decode_engine.cu attn_geom.wrow); ring layouts keep only the last writer.
+// Positions [pa, pb) (absolute; qkv row i of a sample is position t0 + i) -> cache row of position p
+// (decode_engine.cu attn_geom.wrow); ring layouts keep only the last writer of the range.
 __global__ void kv_scatter_kernel(const __half* __restrict__ qkv, __half* __restrict__ kc, __half* __restrict__ vc, int n,
-                                  int P, int S, int H, int dh, int dhp, int rows, int attn_func, int bc, int blocks,
-                                  int prime) {
+                                  int P, int t0, int pa, int pb, int S, int H, int dh, int dhp, int rows, int attn_func,
+                                  int bc, int blocks, int prime) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= (size_t)n * P * S) return;
+    const int np = pb - pa;
+    if (i >= (size_t)n * np * S) return;
     const int cs = (int)(i % S);
-    const int m = (int)(i / S), b = m / P, p = m % P;
+    const int m = (int)(i / S), b = m / np, p = pa + m % np;
     const int h = cs / dh, d = cs % dh;
     int wrow = -1;
     switch (attn_func) {
         case 0: wrow = p; break;
-        case 1: wrow = (p + bc >= P) ? p % bc : -1; break;
+        case 1: wrow = (p + bc >= pb) ? p % bc : -1; break;
         case 2: wrow = (p % bc) * blocks + p / bc; break;
-        case 3: wrow = (p + 2 * bc >= P) ? ((p / bc) & 1) * bc + p % bc : -1; break;
+        case 3: wrow = (p + 2 * bc >= pb) ? ((p / bc) & 1) * bc + p % bc : -1; break;
         case 7: wrow = (p < prime) ? p : -1; break;
     }
     if (wrow < 0) return;
     const size_t dst = (((size_t)b * H + h) * rows + wrow) * dhp + d;
-    const __half* src = qkv + (size_t)m * 3 * S + cs;
+    const __half* src = qkv + ((size_t)b * P + (p - t0)) * 3 * S + cs;
     kc[dst] = src[S];
     vc[dst] = src[2 * S];
 }
@@ -747,14 +810,36 @@ extern "C" int jk_prefill_attention_f16(const jk_prefill_attn_args* a, jk_prefil
     JK_REQUIRE((((uintptr_t)a->qkv | (uintptr_t)a->out | (uintptr_t)a->k_cache | (uintptr_t)a->v_cache) & 15) == 0,
                "qkv, out and the caches must be 16-byte aligned");
     JK_REQUIRE(a->route == 0 || a->route == 1, "route %d (0: the prefill's choice, 1: the scalar kernels)", a->route);
+    const int t0 = a->q_offset;
+    const bool cont = t0 > 0 || a->cache_rows > 0;          // a continuation: keys from the caches
+    JK_REQUIRE(t0 >= 0 && a->cache_rows >= 0, "q_offset %d and cache_rows %d must be >= 0", t0, a->cache_rows);
+    if (cont && f != 6) {
+        int need = 0;
+        switch (f) {
+            case 0: need = t0 + a->P; break;
+            case 1: need = a->bc; break;
+            case 2: need = a->bc * a->blocks; break;
+            case 3: need = 2 * a->bc; break;
+            case 7: need = a->prime; break;
+        }
+        JK_REQUIRE(a->k_cache && a->v_cache, "a continuation (q_offset %d, cache_rows %d) reads its keys from both caches",
+                   t0, a->cache_rows);
+        JK_REQUIRE(f != 2 || (a->blocks >= 1 && t0 + a->P <= a->bc * a->blocks),
+                   "attn_func 2 needs blocks >= 1 (got %d) and positions up to bc * blocks = %d (got %d)", a->blocks,
+                   a->bc * a->blocks, t0 + a->P);
+        JK_REQUIRE(a->cache_rows >= need, "attn_func %d reads %d cache rows at positions [%d, %d), cache_rows is %d", f,
+                   need, t0, t0 + a->P, a->cache_rows);
+    }
+    JK_REQUIRE(!cont || !a->w, "recorded weights are computed at the head of a window only (q_offset 0, cache_rows 0)");
     AttnFwd A;
     A.qkv = (const __half*)a->qkv; A.a = (__half*)a->out; A.kc = (const __half*)a->k_cache; A.vc = (const __half*)a->v_cache;
     A.P = a->P; A.S = a->heads * a->dh; A.H = a->heads; A.dh = a->dh; A.bc = a->bc; A.attn_func = f; A.prime = a->prime;
     A.q_stride = f == 6 ? A.S : 3 * A.S; A.enc_rows = f == 6 ? a->enc_rows : 0; A.dhp = a->dh_pad; A.scale2 = attn_scale2(a->dh);
+    A.qoff = t0; A.qa = t0; A.qb = t0 + a->P; A.cache = cont; A.rows = a->cache_rows; A.blocks = a->blocks;
     const jk_prefill_attn_route r = attn_route(A, a->route == 1);
     JK_REQUIRE(r.tensor_cores || scalar_attn_smem(A) <= kScalarAttnSmemMax,
-               "the scalar kernels hold dh + max(P, enc_rows) = %d floats in shared memory (at most %d)",
-               a->dh + std::max(A.P, A.enc_rows), (int)(kScalarAttnSmemMax / 4));
+               "the scalar kernels hold dh + the keys of a query = %d floats in shared memory (at most %d)",
+               a->dh + fwd_max_keys(A), (int)(kScalarAttnSmemMax / 4));
     if (int rc = layer_attention(A, r, a->n, (__half*)a->w, a->ld, (cudaStream_t)stream)) return rc;
     if (taken) *taken = r;
     return 0;
@@ -775,11 +860,14 @@ extern "C" int jk_prior_prefill(jk_prior* p, const jk_prefill_args* a, jk_stream
                               "step the given tokens through jk_prior_step");
     JK_REQUIRE(p->t_host >= 0, "the last prefill stopped early (n_layers) and left later layers' caches unfilled: "
                                "call jk_prior_reset first");
-    JK_REQUIRE(p->t_host == 0, "prefill starts at position 0 (engine is at %d)", p->t_host);
+    const int t0 = p->t_host;      // > 0: a continuation of the rows' K / V caches
     const int n = a->n_samples, P = a->n_positions;
     JK_REQUIRE(n >= 1 && n <= c.max_batch, "n_samples %d out of range (max_batch %d)", n, c.max_batch);
-    JK_REQUIRE(P >= 1 && P <= p->pf_len && P <= c.n_ctx, "n_positions %d out of range (capacity %d)", P, p->pf_len);
-    JK_REQUIRE(P == 1 || a->tokens, "tokens required");
+    JK_REQUIRE(P >= 1 && P <= p->pf_len, "n_positions %d out of range (capacity %d)", P, p->pf_len);
+    JK_REQUIRE(t0 + P <= c.n_ctx, "positions [%d, %d) run past the context (n_ctx %d)", t0, t0 + P, c.n_ctx);
+    JK_REQUIRE((P == 1 && t0 == 0) || a->tokens, "tokens required");
+    JK_REQUIRE(t0 == 0 || (a->n_record == 0 && a->n_capture == 0 && (a->n_layers == 0 || a->n_layers == c.depth)),
+               "record, capture and n_layers < depth are head-of-window features (the engine is at %d, not 0)", t0);
     JK_REQUIRE(E.pos_emb && E.x_emb, "embeddings not set (jk_prior_set_embeddings)");
     JK_REQUIRE(a->x_cond_len == 0 || a->x_cond_len == 1 || a->x_cond_len == c.n_ctx, "x_cond_len must be 1 or n_ctx");
     const int W = c.width, S = c.n_state, Mw = c.mlp_width, H = c.heads;
@@ -815,11 +903,11 @@ extern "C" int jk_prior_prefill(jk_prior* p, const jk_prefill_args* a, jk_stream
         const size_t cnt = (size_t)rows * W;
         embed_rows_kernel<<<(unsigned)((cnt + 255) / 256), 256, 0, stream>>>(
             p->pf_x, (const long long*)a->tokens, a->tok_stride, a->y_cond, a->x_cond, a->x_cond_len ? a->x_cond_len : 1,
-            E.x_emb, E.pos_emb, E.start_token, n, P, W);
+            E.x_emb, E.pos_emb, E.start_token, n, P, t0, W);
         JK_CHECK_CUDA(cudaGetLastError());
     }
     const unsigned ln_grid = (unsigned)((rows + 7) / 8);
-    JK_REQUIRE((size_t)(E.dh + std::max(P, E.enc_dims)) * 4 <= kScalarAttnSmemMax, "prefill attention tile too large");
+    JK_REQUIRE((size_t)(E.dh + std::max(t0 + P, E.enc_dims)) * 4 <= kScalarAttnSmemMax, "prefill attention tile too large");
     for (int l = 0; l < depth; ++l) {
         const LayerDev& LD = E.layer[l];
         ln_rows_kernel<<<ln_grid, 256, 0, stream>>>(p->pf_x, LD.ln0_g, LD.ln0_b, p->pf_xn, rows, W);
@@ -832,16 +920,37 @@ extern "C" int jk_prior_prefill(jk_prior* p, const jk_prefill_args* a, jk_stream
         A.qkv = p->pf_qkv; A.a = p->pf_a; A.P = P; A.S = S; A.H = H; A.dh = E.dh; A.bc = E.bc; A.attn_func = LD.attn_func;
         A.prime = E.prime_pad; A.scale2 = E.scale2; A.q_stride = q_stride; A.kc = LD.kc; A.vc = LD.vc; A.enc_rows = E.enc_dims;
         A.dhp = E.dh_pad;
-        // tensor cores when the head geometry allows (dh even, dh <= 256); the recorded weights read q / K only, so they
-        // are taken here, before the next layer overwrites pf_qkv
-        const jk_attn_record* r = rec[l];
-        rc = layer_attention(A, attn_route(A, false), n, r ? (__half*)r->w : nullptr, r ? r->ld : 0, stream);
-        if (rc) return rc;
-        if (!enc) {
-            const size_t cnt = (size_t)rows * S;
-            kv_scatter_kernel<<<(unsigned)((cnt + 255) / 256), 256, 0, stream>>>(p->pf_qkv, LD.kc, LD.vc, n, P, S, H, E.dh, E.dh_pad,
-                                                                                  LD.rows, LD.attn_func, E.bc, E.blocks, E.prime_pad);
+        A.qoff = t0; A.qa = t0; A.qb = t0 + P; A.cache = t0 > 0; A.rows = LD.rows; A.blocks = E.blocks;
+        // tensor cores when the head geometry allows (dh even, dh <= 256)
+        const jk_prefill_attn_route route = attn_route(A, false);
+        auto scatter = [&](int pa, int pb) -> int {
+            const size_t cnt = (size_t)n * (pb - pa) * S;
+            kv_scatter_kernel<<<(unsigned)((cnt + 255) / 256), 256, 0, stream>>>(p->pf_qkv, LD.kc, LD.vc, n, P, t0, pa, pb, S, H,
+                                                                                  E.dh, E.dh_pad, LD.rows, LD.attn_func, E.bc,
+                                                                                  E.blocks, E.prime_pad);
             JK_CHECK_CUDA(cudaGetLastError());
+            return 0;
+        };
+        if (t0 == 0) {
+            // queries and keys from pf_qkv; the recorded weights read q / K only, so they are taken here, before the next
+            // layer overwrites pf_qkv
+            const jk_attn_record* r = rec[l];
+            rc = layer_attention(A, route, n, r ? (__half*)r->w : nullptr, r ? r->ld : 0, stream);
+            if (rc) return rc;
+            if (!enc && (rc = scatter(0, P))) return rc;
+        } else if (LD.attn_func == 1 || LD.attn_func == 3) {
+            // ring layouts: a block's rows overwrite rows earlier blocks' queries read, so the chunk goes block by block,
+            // each block's K / V into the cache and then its queries over the cache
+            for (int pa = t0; pa < t0 + P; pa = (pa / E.bc + 1) * E.bc) {
+                const int pb = std::min(t0 + P, (pa / E.bc + 1) * E.bc);
+                if ((rc = scatter(pa, pb))) return rc;
+                A.qa = pa; A.qb = pb;
+                if ((rc = layer_attention(A, route, n, nullptr, 0, stream))) return rc;
+            }
+        } else {
+            // every position has its own row (0, 2, 7; 6 reads the encoder rows): the whole chunk into the cache first
+            if (!enc && (rc = scatter(t0, t0 + P))) return rc;
+            if ((rc = layer_attention(A, route, n, nullptr, 0, stream))) return rc;
         }
         rc = gemm_f16_tc(p->pf_a, p->wt[1][l], LD.b_o, p->pf_x, p->pf_x1, rows, W, S, 2, stream);
         if (rc) return rc;
@@ -866,8 +975,8 @@ extern "C" int jk_prior_prefill(jk_prior* p, const jk_prefill_args* a, jk_stream
         p->t_host = -1;
         return 0;
     }
-    set_position_kernel<<<1, 1, 0, stream>>>(E.t, P);
+    set_position_kernel<<<1, 1, 0, stream>>>(E.t, t0 + P);
     JK_CHECK_CUDA(cudaGetLastError());
-    p->t_host = P;
+    p->t_host = t0 + P;
     return 0;
 }

@@ -176,8 +176,12 @@ class DecodeEngine:
 
     def prefill(self, n, n_positions, *, tokens=None, y_cond=None, x_cond=None, h_out=None, record=None, n_layers=0,
                 capture=None):
-        """positions 0..n_positions-1 of all samples through every layer at once (wgmma GEMMs);
-        afterwards the engine is at position n_positions.
+        """positions t0..t0+n_positions-1 of the first n rows through every layer at once (wgmma GEMMs), where t0 is the
+        engine's position; afterwards the engine is at t0 + n_positions, as after that many steps.  At t0 = 0 this is
+        the head of a window; at t0 > 0 a continuation on top of the rows' K / V caches (after steps, a prefill or a
+        select): tokens is then the window's token tensor (position t reads tokens[:, t - 1]), x_cond and h_out are as
+        at the head (x_cond indexed by absolute position, h_out row i is position t0 + i), y_cond is not read, and
+        record, capture and a truncating n_layers are errors (jk_prefill_args in include/jkb200.h).
 
         record: {layer: w} - fp16 CUDA tensors [n, heads, n_positions, ld] that receive the layer's normalised attention
         weights (keys by absolute position, or encoder row for an encoder-decoder layer; keys >= ld are dropped; zeros
@@ -220,7 +224,7 @@ class DecodeEngine:
         a.n_layers = int(n_layers)
         with torch.cuda.device(self.device):
             check(lib().jk_prior_prefill(self.handle, C.byref(a), stream_ptr()))
-        self.position = -1 if 0 < n_layers < self.cfg.depth else n_positions
+        self.position = -1 if 0 < n_layers < self.cfg.depth else self.position + n_positions
 
     # ---- one token -----------------------------------------------------------------------
     def step(self, n, *, x_in=None, tokens=None, y_cond=None, x_cond=None, h_out=None, logits=None,

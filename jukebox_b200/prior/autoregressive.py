@@ -268,6 +268,79 @@ class ConditionalAutoregressive2D(nn.Module):
             return loss, acts
         return loss, None
 
+    def regenerate(self, x, start, end, n_candidates, x_cond=None, y_cond=None, encoder_kv=None, fp16=True, temp=1.0,
+                   top_k=0, top_p=0.0):
+        """Resample the span [start, end) of a window x [N, D] (1 < D <= input_dims) given the codes on both sides of it
+        (not in the reference): sampling-importance-resampling.  Per item the prime x[i, :start] runs once on one row
+        and is fanned out to n_candidates rows (primed_sample's one-row prime), the rows draw [start, end), the kept
+        suffix x[i, end:] is teacher-forced on every row and each candidate is scored by the suffix's log-likelihood
+        under it; the likeliest candidate is kept (ties to the lower index).  At temperature 1 (no top-k / top-p) that
+        score is the importance weight of p(span | prefix, suffix).
+        fp16: the drawn rows continue on the decode engine and the suffix is one continuation prefill (stepped when it
+        exceeds the prefill capacity); fp32: the fp32 loop, stepping the suffix.  The scores are x_out + log-softmax at
+        the suffix's codes over the stack's activations + cond, in one fused kernel (jk_xout_logprob).
+        x_cond [N, input_dims or 1, width], y_cond [N, 1, width] and encoder_kv [N, ...] as sample takes them.
+        Returns (x_new [N, D], scores fp32 [N, n_candidates]): x with the kept span, and every candidate's suffix
+        log-likelihood in nats.  Codes outside [start, end) are returned unchanged."""
+        from .._lib import JK_MAX_BATCH
+        from ..score import xout_logprob
+        assert not self.only_encode
+        with t.no_grad():
+            x = self.preprocess(x)
+            N, D = x.shape
+            assert 1 < D <= self.input_dims, f"windows of 2 .. {self.input_dims} tokens, got {D}"
+            start, end, K = int(start), int(end), int(n_candidates)
+            if not 0 <= start < end <= D:
+                raise ValueError(f"span [{start}, {end}) is empty or outside the window of {D} codes")
+            if end == D:
+                raise ValueError(f"span [{start}, {end}) leaves no codes after it to rank the candidates by")
+            if not 1 <= K <= JK_MAX_BATCH:
+                raise ValueError(f"n_candidates {K} outside [1, {JK_MAX_BATCH}]")
+            assert (0 <= x).all() and (x < self.bins).all()
+            x_cond, y_cond = self._check_conds(N, x_cond, y_cond)
+            y_cond = None if y_cond is None else y_cond.view(N, 1, self.width)
+            x_new, scores = x.clone(), t.empty(N, K, dtype=t.float32, device=x.device)
+            rows = lambda v, i: None if v is None else (v[i:i + 1] if start else
+                                                        v[i:i + 1].expand(K, *v.shape[1:]).contiguous())
+            for i in range(N):
+                # the prime runs on one row; without one the K rows start from the start token together
+                prime = x[i:i + 1, :start] if start else x.new_zeros(K, 0)
+                cls = SamplingWindow if fp16 else SamplingWindowF32
+                win = cls(self, K, prime, rows(x_cond, i), rows(y_cond, i), rows(encoder_kv, i), fp16, temp, top_k,
+                          top_p, False, D)
+                win.advance(end)
+                win.tokens[:, end:] = x[i, end:]
+                acts = self._suffix_acts(win, end, D)
+                logp = xout_logprob(acts.reshape(-1, self.width), self.x_out.weight, win.tokens[:, end:].reshape(-1))
+                scores[i] = logp.view(K, D - end).double().sum(1).float()
+                best = int(t.argmax(scores[i]))
+                x_new[i, start:end] = win.tokens[best, start:end]
+                self.transformer.del_cache()
+            return x_new, scores
+
+    def _suffix_acts(self, win, end, D):
+        """the stack's output + cond at positions [end, D) of a window's rows, which stand at position end: one
+        continuation prefill on the decode engine, or steps (beyond its prefill capacity, or on the fp32 loop)"""
+        K = win.N
+        h = t.empty(K, D - end, self.width, dtype=t.float32, device=win.tokens.device)
+        if isinstance(win, SamplingWindow):
+            eng = win.eng
+            if D - end <= eng.prefill_capacity:
+                eng.prefill(K, D - end, tokens=win.tokens, x_cond=win.x_cond, h_out=h)
+            else:
+                for j in range(D - end):
+                    out = t.empty(K, self.width, dtype=t.float32, device=h.device)
+                    eng.step(K, tokens=win.tokens, y_cond=win.y_cond, x_cond=win.x_cond, h_out=out)
+                    h[:, j] = out
+        else:
+            from ..transformer import f32
+            tr = self.transformer
+            for j, pos in enumerate(range(end, D)):
+                tr.check_cache(K, pos, False)
+                e = f32.embed(self, win.tokens, win.y_cond, win.x_cond, K, 1, pos)
+                h[:, j] = tr(e, encoder_kv=win.encoder_kv, sample=True, fp16=False).view(K, self.width)
+        return self._add_x_cond(h, win.x_cond, end, D)
+
     def items_per_prefill(self, N):
         """items one fp16 prefill of this model takes: up to JK_MAX_BATCH, or half that when only the 16-row engine fits
         (5b_lyrics); 0 when the configuration has no prefill"""

@@ -383,6 +383,20 @@ class SimplePrior(nn.Module):
                 st = st._replace(topk_ids=t.where(ids >= 0, ids, t.full_like(ids, -1)))
             return st
 
+    def regenerate(self, z, start, end, n_candidates, z_conds=[], y=None, fp16=True, temp=1.0, top_k=0, top_p=0.0):
+        """Resample codes [start, end) of a window of codes z [N, D] of this level (not in the reference), conditioned as
+        score conditions a window: n_candidates draws of the span per item, ranked by the log-likelihood of the codes
+        after it (ConditionalAutoregressive2D.regenerate).  A single_enc_dec prior takes its lyric head into the
+        sequence (the span moves behind it, and the codes are shifted into its token space as sampled codes are); a
+        separate lyric encoder gives the encoder-decoder layers their keys, repeated to the candidate rows.  Returns
+        (z_new [N, D], scores fp32 [N, n_candidates]): the kept span in z, and each candidate's suffix log-likelihood in
+        nats."""
+        with t.no_grad():
+            seq, x_cond, y_cond, enc, _, pl = self._condition(z, z_conds, y, fp16)
+            out, scores = self.prior.regenerate(seq, pl + int(start), pl + int(end), n_candidates, x_cond, y_cond, enc,
+                                                fp16=fp16, temp=temp, top_k=top_k, top_p=top_p)
+            return (self.spaces.last(out) if self.single_enc_dec else out), scores
+
     def layer_acts(self, z, z_conds=[], y=None, layers=(), fp16=True, pool=True):
         """Representations of codes z [N, D] (D <= n_ctx) of this level, conditioned exactly as z_forward / score
         condition them: {layer: fp32 [N, width]} (pool: the mean over the window's codes) or [N, D, width], the outputs

@@ -150,6 +150,69 @@ def song_token_stats(prior, zs, labels, level, hop_length, fp16=True, top_k=0, m
     return TokenStats(*(None if v[0] is None else t.cat(v, dim=1) for v in zip(*cols)))
 
 
+# ---- regenerating a section --------------------------------------------------------------------------------
+def regen_window(T, start, end, n_ctx):
+    """The window (w0, w1) of a level of T codes in which codes [start, end) are regenerated: it contains the span and
+    splits the rest of the context evenly between the codes before it and the codes after it, moved inside [0, T).
+    The span must be shorter than n_ctx and leave codes after it (end < T) to rank the candidates by."""
+    start, end, T, n_ctx = int(start), int(end), int(T), int(n_ctx)
+    if not 0 <= start < end:
+        raise ValueError(f"span [{start}, {end}) is empty")
+    if end >= T:
+        raise ValueError(f"span [{start}, {end}) leaves no codes after it in a level of {T} codes")
+    if end - start >= n_ctx:
+        raise ValueError(f"span of {end - start} codes does not fit a window of {n_ctx} with a code after it")
+    w0 = min(max(start - (n_ctx - (end - start)) // 2, 0), max(0, T - n_ctx))
+    return w0, min(T, w0 + n_ctx)
+
+
+def regenerate_level(zs, labels, sampling_kwargs, level, prior, start, end, hps, n_candidates=16):
+    """Codes [start, end) of one level drawn again, n_candidates per item, and the candidate under which the level's
+    codes after the span are likeliest kept (SimplePrior.regenerate), in the window regen_window places (its start moved
+    to a code of the level above when the prior reads upper-level codes), conditioned on
+    that window's labels (get_y) and upper-level codes (get_z_conds) as LevelRun conditions a window.  Items go through
+    the prior in pieces of max_batch_size.  Returns (zs with zs[level] replaced, scores fp32 [N, n_candidates]: each
+    candidate's log-likelihood in nats of the codes after the span in the window)."""
+    opts = dict(sampling_kwargs)
+    if opts.get('select_every') is not None:
+        raise ValueError("keep-best selection (select_every) is not combined with regeneration")
+    z = zs[level]
+    T = z.shape[1]
+    w0, w1 = regen_window(T, start, end, prior.n_ctx)
+    ds = prior.cond_downsample if prior.x_cond else 1
+    if w0 % ds:     # the upper-level codes under the window start on a code of the level above (get_z_conds)
+        w0 -= w0 % ds
+        if min(T, w0 + prior.n_ctx) <= end:
+            w0 += ds
+        w1 = min(T, w0 + prior.n_ctx)
+        assert w0 <= start and end < w1, f"no window aligned to {ds} holds [{start}, {end}) and a code after it"
+    how = {k: opts[k] for k in ('fp16', 'temp', 'top_k', 'top_p') if k in opts}
+    done, scores = [], []
+    for ctx_i, upper_i, y_i in window_pieces(prior, zs, labels, level, w0, w1, opts.get('max_batch_size', T)):
+        out, sc = prior.regenerate(ctx_i.contiguous(), start - w0, end - w0, n_candidates, upper_i, y_i, **how)
+        done.append(out)
+        scores.append(sc)
+    zs = list(zs)
+    z = z.clone()
+    z[:, start:end] = t.cat(done, dim=0)[:, start - w0:end - w0].to(z.device)
+    zs[level] = z
+    return zs, t.cat(scores, dim=0)
+
+
+def regenerate(zs, labels, sampling_kwargs, priors, start, end, hps, n_candidates=16):
+    """Regenerate the section [start, end) of raw audio samples of every level, from the top level down: each level's
+    span is [start, end) in its codes (start // raw_to_tokens up to end rounded up), and each level below the top is
+    drawn under the new codes above it and ranked by its own codes after the span (regenerate_level).  labels and
+    sampling_kwargs per level, as _sample takes them.  Returns (zs, {level: scores [N, n_candidates]})."""
+    scores = {}
+    for level in sorted(range(len(priors)), reverse=True):
+        prior = priors[level]
+        r = prior.raw_to_tokens
+        zs, scores[level] = regenerate_level(zs, labels[level], sampling_kwargs[level], level, prior, int(start) // r,
+                                             -(-int(end) // r), hps, n_candidates)
+    return zs, scores
+
+
 # ---- the reference's entry points -------------------------------------------------------------------------
 def sample_partial_window(zs, labels, sampling_kwargs, level, prior, tokens_to_sample, hps):
     """`tokens_to_sample` new tokens at `level`, the context sliding once it is full"""
