@@ -462,6 +462,23 @@ int jk_xout_stats(const float* h, int m, int width, const void* w_split, int bin
 int jk_filter_logits(const float* logits, int64_t logits_stride, int n, int bins, float temp, int top_k,
                      float top_p, float* out, int64_t out_stride, jk_stream_t stream);
 
+/* Guided draw from two conditionings (classifier-free guidance, or a blend of two conditionings), one launch per position.
+ * For pair r = 0..n-1, with c[r] the conditional logits (rows c_stride floats apart) and u[r] the alternative ones (rows
+ * u_stride apart):
+ *   g = c[r] + s (c[r] - u[r])          fp32, each operation rounded to nearest on its own (no FMA): torch's
+ *                                       `c + s * (c - u)` gives the same bits
+ *   tokens[r, position] = tokens_alt[r, position] ~ Categorical(filter(g / temp))
+ * filter: top_k / top_p as jk_filter_logits (at most one set; neither: no filter), and the draw is jk_sample_categorical's
+ * (Philox counter (position, r)), so the token equals jk_filter_logits + jk_sample_categorical of g bit for bit.  s = 0
+ * gives g = c.  raw and logp are both NULL or both given: logp[r * logp_stride + position] = log_softmax(raw[r])[token],
+ * raw rows c_stride floats apart (raw == c: the conditional model's own likelihood at temperature 1, read with c).
+ * tokens / tokens_alt: int64 rows tok_stride / tok_alt_stride apart.  bins <= 4096, s finite, temp > 0, n >= 0.  Each
+ * operand row is read once; pairs are independent. */
+int jk_sample_guided(const float* c, int64_t c_stride, const float* u, int64_t u_stride, int n, int bins, float s,
+                     float temp, int top_k, float top_p, uint64_t seed, int position, int64_t* tokens, int64_t tok_stride,
+                     int64_t* tokens_alt, int64_t tok_alt_stride, const float* raw, float* logp, int64_t logp_stride,
+                     jk_stream_t stream);
+
 /* torch Conv1d weight [c_out, c_in, k] (transposed = 0) or ConvTranspose1d weight
  * [c_in, c_out, k] (transposed = 1) -> packed [k, c_in, c_out] */
 int jk_pack_conv_weight(const float* w, float* packed, int c_out, int c_in, int k, int transposed,

@@ -136,6 +136,7 @@ SIGNATURES = {
     "jk_xout_stats_workspace_bytes": (_I, [_I, _I, _I, _I, C.POINTER(C.c_size_t)]),
     "jk_xout_stats": (_I, [_P, _I, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P, _P, C.c_size_t, _P]),
     "jk_filter_logits": (_I, [_P, _L, _I, _I, _F, _I, _F, _P, _L, _P]),
+    "jk_sample_guided": (_I, [_P, _L, _P, _L, _I, _I, _F, _F, _I, _F, C.c_uint64, _I, _P, _L, _P, _L, _P, _P, _L, _P]),
     "jk_vq_argmin": (_I, [_P, _P, _P, _P, _L, _I, _I, _P]),
     "jk_vq_gather": (_I, [_P, _P, _P, _L, _I, _I, _P]),
     "jk_conv1d_cl": (_I, [C.POINTER(ConvArgs), _P]),

@@ -8,12 +8,15 @@ transformer + fp32 logits, jukebox_b200/csrc/decode_engine.cu) and one sampling 
 front of it) - nothing synchronises with the host inside the loop (the reference's per-token
 `assert (0 <= x).all()` is hoisted out).
 """
+import math
+from typing import NamedTuple
+
 import numpy as np
 import torch as t
 import torch.nn as nn
 import torch.nn.functional as F
 
-from ..transformer.ops import filter_logits_scaled, sample_categorical, sample_categorical_scored
+from ..transformer.ops import filter_logits_scaled, sample_categorical, sample_categorical_scored, sample_guided
 from ..transformer.transformer import Transformer
 from ..utils.logger import get_range
 
@@ -29,6 +32,17 @@ def split_chunks(length, chunk_size):
     chunk_sizes = [*[chunk_size] * (n_passes - 1), (length - 1) % chunk_size + 1]
     assert sum(chunk_sizes) == length
     return chunk_sizes
+
+
+class Guide(NamedTuple):
+    """The alternative conditioning of a guided window (sample / primed_sample with guidance_scale): every drawn token
+    comes from g = c + (scale - 1) (c - u), c the logits under the window's conditioning and u under this one.  x_cond,
+    y_cond and encoder_kv have the shapes of the window's own; x: the alternative given tokens, None for the same ones."""
+    scale: float
+    x_cond: object = None
+    y_cond: object = None
+    encoder_kv: object = None
+    x: object = None
 
 
 class PositionEmbedding(nn.Module):
@@ -161,12 +175,13 @@ class ConditionalAutoregressive2D(nn.Module):
         return acts + (x_cond[:, t0:t1] if x_cond.shape[1] > 1 else x_cond)
 
     def _run(self, n_samples, prime, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds, sample_tokens,
-             get_logprobs=False, select_every=None, select_keep=None):
+             get_logprobs=False, select_every=None, select_keep=None, guide=None):
         """shared body of sample / primed_sample.  prime: LongTensor [N, P] of given tokens (P may be 0), or [1, P]
-        with its conditioning of one row too: prefilled once and repeated to the N rows."""
+        with its conditioning of one row too: prefilled once and repeated to the N rows.  guide: a Guide, or None."""
         cls = SamplingWindow if fp16 else SamplingWindowF32
         win = cls(self, n_samples, prime, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds,
-                  sample_tokens, get_logprobs=get_logprobs, select_every=select_every, select_keep=select_keep)
+                  sample_tokens, get_logprobs=get_logprobs, select_every=select_every, select_keep=select_keep,
+                  guide=guide)
         win.advance(win.sample_tokens)
         return win.finish()
 
@@ -179,15 +194,24 @@ class ConditionalAutoregressive2D(nn.Module):
     # ranked by the log-likelihood of the tokens they drew in this window (keep_best_parents), the m likeliest keep
     # their rows and the others continue copies of them (SamplingWindow.select).  The result then ends with ancestry,
     # LongTensor [N]: the input item each returned row descends from.
+    # guidance_scale (not in the reference; guided sampling): every drawn token comes from g = c + (guidance_scale - 1)
+    # (c - u), c the logits under (x_cond, y_cond, encoder_kv) and u under the alternative (x_cond_alt, y_cond_alt,
+    # encoder_kv_alt, of the same shapes; x_alt: the alternative given tokens, default the same), then temp / top-k /
+    # top-p as unguided.  Scale 1 draws exactly the unguided tokens, > 1 is classifier-free guidance away from u, (0, 1)
+    # blends the two.  The window runs 2N engine rows (rows N.. carry u), so N <= guided_items(); results are the N
+    # conditional rows: logprobs / preds under c, keep-best selection moves each pair together.
     def sample(self, n_samples, x_cond=None, y_cond=None, encoder_kv=None, fp16=False, temp=1.0, top_k=0,
-               top_p=0.0, get_preds=False, sample_tokens=None, get_logprobs=False, select_every=None, select_keep=None):
+               top_p=0.0, get_preds=False, sample_tokens=None, get_logprobs=False, select_every=None, select_keep=None,
+               guidance_scale=None, x_cond_alt=None, y_cond_alt=None, encoder_kv_alt=None):
         prime = t.zeros(n_samples, 0, dtype=t.long, device=self.x_emb.weight.device)
+        guide = None if guidance_scale is None else Guide(guidance_scale, x_cond_alt, y_cond_alt, encoder_kv_alt)
         return self._run(n_samples, prime, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds,
-                         sample_tokens, get_logprobs, select_every, select_keep)
+                         sample_tokens, get_logprobs, select_every, select_keep, guide)
 
     def primed_sample(self, n_samples, x, x_cond=None, y_cond=None, encoder_kv=None, fp16=False, temp=1.0,
                       top_k=0, top_p=0.0, get_preds=False, chunk_size=None, sample_tokens=None, get_logprobs=False,
-                      select_every=None, select_keep=None):
+                      select_every=None, select_keep=None, guidance_scale=None, x_cond_alt=None, y_cond_alt=None,
+                      encoder_kv_alt=None, x_alt=None):
         """`chunk_size` is accepted for compatibility: the prefill runs token by token through the
         same persistent kernel, which is what chunked prefill computes (reference check_chunks).
         x may be one row for n_samples > 1 (not in the reference): one prime, n_samples continuations.  x_cond, y_cond
@@ -197,8 +221,9 @@ class ConditionalAutoregressive2D(nn.Module):
             x = self.preprocess(x)
         assert x.shape[0] == n_samples or (x.shape[0] == 1 and x.shape[1] > 0), \
             f"prime of {x.shape[0]} rows for {n_samples} samples: give n_samples rows, or one row of given tokens"
+        guide = None if guidance_scale is None else Guide(guidance_scale, x_cond_alt, y_cond_alt, encoder_kv_alt, x_alt)
         return self._run(n_samples, x, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds,
-                         sample_tokens, get_logprobs, select_every, select_keep)
+                         sample_tokens, get_logprobs, select_every, select_keep, guide)
 
     def logprob(self, x, x_cond=None, y_cond=None, encoder_kv=None, fp16=True):
         """log-likelihood in nats of every token of whole sequences x [N, input_dims] given the ones before it, fp32
@@ -351,6 +376,12 @@ class ConditionalAutoregressive2D(nn.Module):
                 return n
         return 0
 
+    def guided_items(self):
+        """the most items a guided window takes: its 2N rows must fit one engine of this model (items_per_prefill: 32
+        rows, 16 on 5b_lyrics)"""
+        from .._lib import JK_MAX_BATCH
+        return (self.items_per_prefill(JK_MAX_BATCH) or JK_MAX_BATCH) // 2
+
     def layer_acts(self, x, x_cond=None, y_cond=None, encoder_kv=None, layers=(), fp16=True, pool=True, add_cond=True,
                    t0=0):
         """Representations (not in the reference; JukeMIR, Castellon et al. 2021): the output of intermediate layers of
@@ -454,6 +485,17 @@ class ConditionalAutoregressive2D(nn.Module):
         tr.del_cache()
 
 
+def _pair_rows(a, b, name):
+    """the conditional rows a and the alternative rows b of a guided window as one tensor of 2n rows"""
+    if a is None and b is None:
+        return None
+    if a is None or b is None:
+        raise ValueError(f"guidance: {name}_alt must be given exactly when {name} is")
+    if tuple(a.shape) != tuple(b.shape):
+        raise ValueError(f"guidance: {name}_alt {tuple(b.shape)} must have the shape of {name} {tuple(a.shape)}")
+    return t.cat([a, b.to(a.device, a.dtype)], dim=0)
+
+
 def keep_best_parents(scores, keep):
     """Keep-best selection of a window's rows: rows ranked by score (the log-likelihood of the tokens each drew so far,
     highest first, ties to the lower row; nan ranks last), the `keep` best keep their rows and every other row, in
@@ -473,33 +515,57 @@ def keep_best_parents(scores, keep):
 class _Rows:
     """The per-item state shared by both sampling windows: the rows' tokens / log-probabilities / logits and
     conditioning, which rows run (one row while a one-row prime is given, then every row), the rows' ancestry, and
-    keep-best selection.  A subclass owns the K / V caches (_select_caches)."""
+    keep-best selection.  A subclass owns the K / V caches (_select_caches).
+    A guided window (guide: a Guide) holds G = 2 rows per item: rows [0, items) are conditional, rows [items, 2 items)
+    the alternative, each with its own conditioning and given tokens; self.N counts rows, and the results are the
+    conditional rows."""
 
-    def _init_rows(self, ca, n_samples, prime, x_cond, y_cond, sample_tokens, get_preds, get_logprobs, select_every,
-                   select_keep):
+    def _init_rows(self, ca, n_samples, prime, x_cond, y_cond, encoder_kv, sample_tokens, get_preds, get_logprobs,
+                   select_every, select_keep, guide=None):
+        """returns encoder_kv, paired with the alternative's when guided"""
         self.ca = ca
         self.sample_tokens = ca.input_dims if sample_tokens is None else int(sample_tokens)
-        self.N = N = n_samples
+        self.items = n_samples
+        self.G = G = 1 if guide is None else 2
+        self.guide_s = None
+        if guide is not None:
+            limit = ca.guided_items()
+            if n_samples > limit:
+                raise ValueError(f"{n_samples} guided items need {2 * n_samples} engine rows: at most {limit} guided "
+                                 "items fit one engine of this model")
+            self.guide_s = float(guide.scale) - 1.0
+            if not math.isfinite(self.guide_s):
+                raise ValueError(f"guidance_scale {guide.scale} must be finite")
+            x_alt = prime if guide.x is None else ca.preprocess(guide.x)
+            if x_alt.shape != prime.shape:
+                raise ValueError(f"guidance: x_alt {tuple(x_alt.shape)} must have the shape of x {tuple(prime.shape)}")
+            prime = t.cat([prime, x_alt.to(prime.device)], dim=0)
+            x_cond = _pair_rows(x_cond, guide.x_cond, "x_cond")
+            y_cond = _pair_rows(y_cond, guide.y_cond, "y_cond")
+            encoder_kv = _pair_rows(encoder_kv, guide.encoder_kv, "encoder_kv")
+        self.N = N = G * n_samples
         self.P = P = prime.shape[1]
         assert P < self.sample_tokens <= ca.input_dims, \
             f"need given tokens {P} < sample_tokens {self.sample_tokens} <= input_dims {ca.input_dims}"
-        # one given row for N samples: its positions run on one row, then its state is repeated to all N (_fan_out)
+        # one given row for N samples: its positions run on one row (a pair of rows when guided), then its state is
+        # repeated to all N (_fan_out)
         self.n = prime.shape[0] if P else N
-        assert self.n in (1, N), f"prime of {self.n} rows for {N} samples"
+        assert self.n in (G, N), f"prime of {self.n} rows for {N} samples"
         self.x_cond, self.y_cond = ca._check_conds(self.n, x_cond, y_cond)
         dev = ca.x_emb.weight.device
         self.tokens = t.zeros(N, self.sample_tokens, dtype=t.long, device=dev)
         if P:
             assert (0 <= prime).all() and (prime < ca.bins).all()
-            self.tokens[:, :P] = prime
+            self.tokens[:, :P] = prime.repeat_interleave(N // prime.shape[0], dim=0)    # a one-row prime on every row
         if (select_every is None) != (select_keep is None):
             raise ValueError("keep-best selection needs both select_every and select_keep")
         if select_every is not None:
-            if not (int(select_every) >= 1 and 1 <= int(select_keep) <= N):
-                raise ValueError(f"select_every {select_every} must be >= 1 and select_keep {select_keep} in [1, {N}]")
+            if not (int(select_every) >= 1 and 1 <= int(select_keep) <= self.items):
+                raise ValueError(f"select_every {select_every} must be >= 1 and select_keep {select_keep} in "
+                                 f"[1, {self.items}]")
             select_every, select_keep = int(select_every), int(select_keep)
         self.select_every, self.select_keep = select_every, select_keep
-        self.ancestry = t.arange(N, device=dev)
+        self.ancestry = t.arange(self.items, device=dev).repeat(G)
         self.get_preds = get_preds
         self.preds = t.empty(N, self.sample_tokens, ca.bins, dtype=t.float32, device=dev) if get_preds else None
         # selection ranks rows by the log-likelihoods of their draws, which the sampling launch scores (get_logprobs)
@@ -513,6 +579,9 @@ class _Rows:
         self.fbuf = None
         self.logit_bias = None
         self._owned = {"tokens", "logprobs", "preds", "logit_bias"}     # tensors this window made itself
+        if guide is not None:
+            self._owned |= {"x_cond", "y_cond", "encoder_kv"}             # the paired copies
+        return encoder_kv
 
     def select(self, parents):
         """row b of the window becomes a copy of row parents[b] (b < N, parents[b] < the rows now running): its K / V
@@ -543,22 +612,27 @@ class _Rows:
         self.n = self.N
 
     def _fan_out(self):
-        """the given positions of a one-row prime are done: every row continues from it"""
-        self.select([0] * self.N)
+        """the given positions of a one-row prime are done: every row continues from it (guided: every conditional
+        row from row 0, every alternative row from row 1)"""
+        self.select([g for g in range(self.G) for _ in range(self.items)])
 
     def _drawn(self, sample_t, x):
         """position sample_t of the running rows from their logits x [n, bins], then keep-best selection when the
         window has drawn a multiple of select_every tokens"""
         _draw(self, x, sample_t, sample_t >= self.P)
         if self.select_every and sample_t >= self.P and (sample_t + 1 - self.P) % self.select_every == 0:
-            scores = self.logprobs[:, self.P:sample_t + 1].double().sum(1).cpu()
+            scores = self.logprobs[:self.items, self.P:sample_t + 1].double().sum(1).cpu()
             parents = keep_best_parents(scores.tolist(), self.select_keep)
+            # a guided item's two rows move together: the alternative rows follow their conditional rows
+            parents = [q + g * self.items for g in range(self.G) for q in parents]
             if parents != list(range(self.N)):
                 self.select(parents)
 
     def _result(self, x):
-        out = (x,) + ((self.preds,) if self.get_preds else ()) + ((self.logprobs,) if self.get_logprobs else ()) + \
-              ((self.ancestry,) if self.select_every else ())
+        """x: the postprocessed tokens of the conditional rows"""
+        k = self.items
+        out = (x,) + ((self.preds[:k],) if self.get_preds else ()) + \
+              ((self.logprobs[:k],) if self.get_logprobs else ()) + ((self.ancestry[:k],) if self.select_every else ())
         return out[0] if len(out) == 1 else out
 
 
@@ -574,12 +648,12 @@ class SamplingWindow(_Rows):
     (select); keep-best selection (select_every / select_keep) reorders the rows every select_every drawn tokens."""
 
     def __init__(self, ca, n_samples, prime, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds,
-                 sample_tokens, get_logprobs=False, select_every=None, select_keep=None):
+                 sample_tokens, get_logprobs=False, select_every=None, select_keep=None, guide=None):
         assert ca.training is False
         assert not ca.only_encode
         assert fp16, "SamplingWindowF32 is the fp32 loop"
-        self._init_rows(ca, n_samples, prime, x_cond, y_cond, sample_tokens, get_preds, get_logprobs, select_every,
-                        select_keep)
+        encoder_kv = self._init_rows(ca, n_samples, prime, x_cond, y_cond, encoder_kv, sample_tokens, get_preds,
+                                     get_logprobs, select_every, select_keep, guide)
         N, n, P = self.N, self.n, self.P
         dev = ca.x_emb.weight.device
         self.eng = eng = ca._fresh_engine(N, encoder_kv)
@@ -647,7 +721,7 @@ class SamplingWindow(_Rows):
                 b.attn._advance(self.N, self.sample_tokens, self.fp16)
             tr.check_cache(self.N, self.sample_tokens, self.fp16)
             tr.del_cache()
-            x = self.ca.postprocess(self.tokens, self.sample_tokens)
+            x = self.ca.postprocess(self.tokens[:self.items], self.sample_tokens)
         return self._result(x)
 
 
@@ -659,6 +733,11 @@ def _draw(win, x, sample_t, drawn):
     if not drawn and not win.scored:
         return
     n = x.shape[0]
+    if drawn and win.G == 2:     # guided: one launch draws each pair's token from its two rows (n = 2 items)
+        k = win.items
+        sample_guided(x[:k], x[k:], win.guide_s, win.temp, win.top_k, win.top_p, win.seed, sample_t, win.tokens[:k],
+                      win.tokens[k:], win.logprobs[:k] if win.scored else None)
+        return
     samp, temp = x, win.temp
     if drawn and (win.top_k or win.top_p):
         win.fbuf = filter_logits_scaled(x, win.temp, win.top_k, win.top_p, win.fbuf)
@@ -676,10 +755,10 @@ class SamplingWindowF32(_Rows):
     Its caches are torch tensors (F32Path.caches), which select indexes."""
 
     def __init__(self, ca, n_samples, prime, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p, get_preds,
-                 sample_tokens, get_logprobs=False, select_every=None, select_keep=None):
+                 sample_tokens, get_logprobs=False, select_every=None, select_keep=None, guide=None):
         assert ca.training is False and not ca.only_encode and not fp16
-        self._init_rows(ca, n_samples, prime, x_cond, y_cond, sample_tokens, get_preds, get_logprobs, select_every,
-                        select_keep)
+        encoder_kv = self._init_rows(ca, n_samples, prime, x_cond, y_cond, encoder_kv, sample_tokens, get_preds,
+                                     get_logprobs, select_every, select_keep, guide)
         self.tr = ca.transformer
         self.tr.del_cache()
         if encoder_kv is not None:
@@ -731,5 +810,5 @@ class SamplingWindowF32(_Rows):
         with t.no_grad():
             self.tr.check_cache(self.N, self.sample_tokens, False)
             self.tr.del_cache()
-            x = self.ca.postprocess(self.tokens, self.sample_tokens)
+            x = self.ca.postprocess(self.tokens[:self.items], self.sample_tokens)
         return self._result(x)

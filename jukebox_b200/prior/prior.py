@@ -189,8 +189,9 @@ class SimplePrior(nn.Module):
             out = block(codes, out)
         return out
 
-    def get_cond(self, z_conds, y):
-        """-> (x_cond [N, n_ctx, W] or [N, 1, W] or None, y_cond [N, 1, W] or None, lyric tokens or None)"""
+    def get_cond(self, z_conds, y, x_up=None):
+        """-> (x_cond [N, n_ctx, W] or [N, 1, W] or None, y_cond [N, 1, W] or None, lyric tokens or None).  x_up: the
+        upper-level codes through the conditioner (x_emb(z_conds)) when the caller has them already"""
         lyric = None
         if y is not None:
             n_labels = 4 + self.y_emb.max_bow_genre_size
@@ -200,8 +201,22 @@ class SimplePrior(nn.Module):
         y_cond = y_pos = None
         if self.y_cond:
             y_cond, y_pos = self.y_emb(y)
-        x_cond = self.x_emb(z_conds) if self.x_cond else y_pos
+        if self.x_cond:
+            x_cond = self.x_emb(z_conds) if x_up is None else x_up
+        else:
+            x_cond = y_pos
         return x_cond, y_cond, lyric
+
+    def null_y(self, y):
+        """the null label rows of y [N, label width]: the same total length, offset and window length, unknown artist,
+        unknown genre and no lyrics (the labeller's row for artist "unknown", genre "unknown", lyrics "") - what
+        classifier-free guidance steers away from.  A prior without labels has none: ValueError."""
+        if isinstance(self.labeller, EmptyLabeller):
+            raise ValueError("this prior has no labels, so there is no null conditioning to guide with")
+        null = self.labeller.get_label(artist="unknown", genre="unknown", lyrics="", total_length=1, offset=0)["y"]
+        out = y.clone()
+        out[:, 3:] = t.as_tensor(null[3:], dtype=y.dtype, device=y.device)
+        return out
 
     # single_enc_dec token-space helpers under the reference's names
     def prior_preprocess(self, xs, conds):
@@ -227,7 +242,8 @@ class SimplePrior(nn.Module):
 
     # ---- sampling -----------------------------------------------------------------------------------------------
     def sample(self, n_samples, z=None, z_conds=None, y=None, fp16=False, temp=1.0, top_k=0, top_p=0.0,
-               chunk_size=None, sample_tokens=None, get_logprobs=False, select_every=None, select_keep=None):
+               chunk_size=None, sample_tokens=None, get_logprobs=False, select_every=None, select_keep=None,
+               guidance_scale=None, guidance_y=None):
         """one window: z = codes of this level already in the window (None / empty: ancestral), z_conds = codes of the
         level above, y = label rows.  Returns the codes [N, sample_tokens or n_ctx].  With get_logprobs it returns
         (codes, logprobs): fp32 [N, sample_tokens or n_ctx], the log-likelihood in nats of each returned code under the
@@ -235,7 +251,11 @@ class SimplePrior(nn.Module):
         z of one row with n_samples > 1 (not in the reference): one prime, n_samples continuations; z_conds and y then
         have one row too, and the window runs the prime once (ConditionalAutoregressive2D.primed_sample).
         select_every / select_keep: keep-best selection inside the window (ConditionalAutoregressive2D.sample); the
-        result then ends with ancestry, LongTensor [N], the input item each returned row descends from."""
+        result then ends with ancestry, LongTensor [N], the input item each returned row descends from.
+        guidance_scale: guided sampling (ConditionalAutoregressive2D.sample) away from, or towards, the alternative
+        conditioning of the label rows guidance_y (the rows and layout of y; None: the null rows, null_y): its label
+        embedding, its lyrics (merged ahead of the codes, or through the lyric encoder) and the same upper-level codes,
+        whose conditioner runs once.  At most prior.guided_items() items per call."""
         fresh = z is None or z.shape[1] == 0
         rows = 1 if (not fresh and z.shape[0] == 1) else n_samples
         for name, v in (("z", z), ("y", y), *((f"z_conds[{i}]", c) for i, c in enumerate(z_conds or []))):
@@ -250,19 +270,33 @@ class SimplePrior(nn.Module):
         if select_every is not None or select_keep is not None:
             how.update(select_every=select_every, select_keep=select_keep)
         with t.no_grad():
-            x_cond, y_cond, lyric = self.get_cond(z_conds, y)
+            x_up = self.x_emb(z_conds) if self.x_cond else None
+            x_cond, y_cond, lyric = self.get_cond(z_conds, y, x_up)
+            alt = None
+            if guidance_scale is not None:
+                if isinstance(self.labeller, EmptyLabeller):
+                    raise ValueError("guidance needs labels: this prior has none, so there is no other conditioning "
+                                     "to guide with")
+                y_alt = self.null_y(y) if guidance_y is None else guidance_y
+                assert y_alt.shape == y.shape, f"guidance_y {tuple(y_alt.shape)}: expected the shape of y {tuple(y.shape)}"
+                alt = self.get_cond(z_conds, y_alt.to(y.device), x_up)
+                how["guidance_scale"] = guidance_scale
             if self.single_enc_dec:
-                out = self._sample_joint(n_samples, None if fresh else z, lyric, x_cond, y_cond, chunk_size, sample_tokens, how)
+                out = self._sample_joint(n_samples, None if fresh else z, lyric, x_cond, y_cond, chunk_size, sample_tokens, how, alt)
             else:
-                out = self._sample_separate(n_samples, None if fresh else z, lyric, x_cond, y_cond, chunk_size, sample_tokens, how)
+                out = self._sample_separate(n_samples, None if fresh else z, lyric, x_cond, y_cond, chunk_size, sample_tokens, how, alt)
         if sample_tokens is None:
             assert_shape(out[0] if isinstance(out, tuple) else out, (n_samples, *self.z_shape))
         return out
 
-    def _sample_joint(self, N, z, lyric, x_cond, y_cond, chunk_size, sample_tokens, how):
+    def _sample_joint(self, N, z, lyric, x_cond, y_cond, chunk_size, sample_tokens, how, alt=None):
         # the lyric tokens are the head of the sequence: always a primed run of the joint model
         given = [lyric] if z is None else [lyric, z]
         seq, cond = self.spaces.merge(given, [None, x_cond])
+        if alt is not None:     # the alternative's own lyric head ahead of the same codes
+            x_alt, y_alt, lyric_alt = alt
+            seq_alt, cond_alt = self.spaces.merge([lyric_alt] + given[1:], [None, x_alt])
+            how = dict(how, x_alt=seq_alt, x_cond_alt=cond_alt, y_cond_alt=y_alt)
         total = None if sample_tokens is None else sample_tokens + self.n_tokens
         out = self.prior.primed_sample(N, seq, cond, y_cond, chunk_size=chunk_size, sample_tokens=total, **how)
         if not isinstance(out, tuple):
@@ -272,8 +306,12 @@ class SimplePrior(nn.Module):
             rest[0] = rest[0][:, sum(self.spaces.dims[:-1]):]     # the lyric head stripped as from the codes
         return (self.spaces.last(seq), *rest)
 
-    def _sample_separate(self, N, z, lyric, x_cond, y_cond, chunk_size, sample_tokens, how):
+    def _sample_separate(self, N, z, lyric, x_cond, y_cond, chunk_size, sample_tokens, how, alt=None):
         enc = self.get_encoder_kv(lyric, fp16=how["fp16"], sample=True)
+        if alt is not None:
+            x_alt, y_alt, lyric_alt = alt
+            how = dict(how, x_cond_alt=x_alt, y_cond_alt=y_alt,
+                       encoder_kv_alt=self.get_encoder_kv(lyric_alt, fp16=how["fp16"], sample=True))
         if z is None:
             return self.prior.sample(N, x_cond, y_cond, enc, sample_tokens=sample_tokens, **how)
         return self.prior.primed_sample(N, z, x_cond, y_cond, enc, chunk_size=chunk_size, sample_tokens=sample_tokens, **how)
@@ -382,6 +420,10 @@ class SimplePrior(nn.Module):
                 ids = st.topk_ids - self.spaces.shift[-1]
                 st = st._replace(topk_ids=t.where(ids >= 0, ids, t.full_like(ids, -1)))
             return st
+
+    def guided_items(self):
+        """the most items one guided sample call takes (ConditionalAutoregressive2D.guided_items)"""
+        return self.prior.guided_items()
 
     def regenerate(self, z, start, end, n_candidates, z_conds=[], y=None, fp16=True, temp=1.0, top_k=0, top_p=0.0):
         """Resample codes [start, end) of a window of codes z [N, D] of this level (not in the reference), conditioned as

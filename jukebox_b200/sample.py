@@ -57,14 +57,35 @@ def window_pieces(prior, zs, labels, level, start, end, max_batch):
         yield ctx_i, None if upper_i is None else [u.contiguous() for u in upper_i], y_i
 
 
+def null_labels(prior, labels):
+    """The null labels of a level's labels dict (y [N, label width] and info): for each item the same total length,
+    offset and window length, unknown artist, unknown genre and no lyrics (SimplePrior.null_y) - the alternative that
+    classifier-free guidance steers away from.  A prior without labels has none: ValueError."""
+    y = prior.null_y(None if labels is None else labels['y'])
+    info = [dict(artist="unknown", genre="unknown", lyrics="", full_tokens=[]) for _ in range(y.shape[0])]
+    return dict(y=y, info=info)
+
+
 class LevelRun:
-    """One level of one sampling job: the codes sampled so far and what is needed to extend them."""
+    """One level of one sampling job: the codes sampled so far and what is needed to extend them.
+    sampling_kwargs may hold guidance_scale and guidance_labels (guided sampling, SimplePrior.sample): a labels dict like
+    `labels`, or None for null_labels(prior, labels); it is windowed as the labels are (get_y), lyrics included."""
 
     def __init__(self, zs, labels, sampling_kwargs, level, prior, hps):
         self.zs, self.labels, self.level, self.prior, self.hps = zs, labels, level, prior, hps
         opts = dict(sampling_kwargs)
         opts.pop('sample_tokens', None)           # per-window, set by run_window
         self.max_batch = opts.pop('max_batch_size')
+        self.guidance_labels = opts.pop('guidance_labels', None)
+        if opts.get('guidance_scale') is not None:
+            limit = prior.guided_items()
+            if self.max_batch > limit:
+                raise ValueError(f"guided sampling runs 2 engine rows per item: max_batch_size {self.max_batch} needs "
+                                 f"{2 * self.max_batch} rows, at most {limit} guided items fit one engine of this model")
+            if self.guidance_labels is None:
+                self.guidance_labels = null_labels(prior, labels)
+        elif self.guidance_labels is not None:
+            raise ValueError("guidance_labels are given without a guidance_scale")
         self.opts = opts
 
     def have(self):
@@ -81,10 +102,15 @@ class LevelRun:
             return
         extra = {} if win.sample_tokens == prior.n_ctx else dict(sample_tokens=win.sample_tokens)
         selecting = self.opts.get('select_every') is not None
+        guided = self.guidance_labels is not None
+        alts = split_batch(prior.get_y(self.guidance_labels, win.start), self.zs[level].shape[0], self.max_batch) \
+            if guided else None
         done, i0 = [], 0
-        for ctx_i, upper_i, y_i in window_pieces(prior, self.zs, self.labels, level, win.start,
-                                                 win.start + prior.n_ctx, self.max_batch):
+        for j, (ctx_i, upper_i, y_i) in enumerate(window_pieces(prior, self.zs, self.labels, level, win.start,
+                                                                win.start + prior.n_ctx, self.max_batch)):
             n = ctx_i.shape[0]
+            if guided:
+                extra['guidance_y'] = alts[j]
             if selecting and y_i is not None and not bool((y_i == y_i[:1]).all()):
                 raise ValueError(f"keep-best selection (select_every) copies samples into other samples' rows, but items "
                                  f"{i0}..{i0 + n - 1} have different labels, which the other levels' labels cannot "
@@ -176,6 +202,8 @@ def regenerate_level(zs, labels, sampling_kwargs, level, prior, start, end, hps,
     opts = dict(sampling_kwargs)
     if opts.get('select_every') is not None:
         raise ValueError("keep-best selection (select_every) is not combined with regeneration")
+    if opts.get('guidance_scale') is not None or opts.get('guidance_labels') is not None:
+        raise ValueError("guided sampling (guidance_scale / guidance_labels) is not combined with regeneration")
     z = zs[level]
     T = z.shape[1]
     w0, w1 = regen_window(T, start, end, prior.n_ctx)

@@ -129,3 +129,26 @@ def sample_categorical_scored(logits, raw, temp, seed, position, tokens, logp):
                                              C.c_uint64(seed & (2 ** 64 - 1)), int(position),
                                              C.c_void_p(tokens.data_ptr()), tokens.stride(0),
                                              C.c_void_p(logp.data_ptr()), logp.stride(0), stream_ptr()))
+
+
+def sample_guided(c, u, s, temp, top_k, top_p, seed, position, tokens, tokens_alt, logp=None):
+    """One guided draw per pair in one launch (jk_sample_guided): g = c + s * (c - u), then filter_logits_scaled(g, temp,
+    top_k, top_p) when a filter is set and the draw of sample_categorical - the same token, written to both
+    tokens[:, position] and tokens_alt[:, position].  With logp: logp[:, position] = log_softmax(c)[token], the
+    conditional likelihood at temperature 1.  c / u: fp32 CUDA [n, bins] with unit inner stride; tokens / tokens_alt
+    int64 [n, L]; logp fp32 [n, L]."""
+    from .._lib import lib, check, stream_ptr
+    import ctypes as C
+    for x in (c, u):
+        assert x.dtype == t.float32 and x.dim() == 2 and x.stride(1) == 1 and x.is_cuda
+    assert c.shape == u.shape
+    for x in (tokens, tokens_alt):
+        assert x.dtype == t.int64 and x.dim() == 2 and x.stride(1) == 1 and x.is_cuda and x.shape[0] == c.shape[0]
+    if logp is not None:
+        assert logp.dtype == t.float32 and logp.dim() == 2 and logp.stride(1) == 1 and logp.is_cuda
+    vp = lambda x: C.c_void_p(0 if x is None else x.data_ptr())
+    check(lib().jk_sample_guided(vp(c), c.stride(0), vp(u), u.stride(0), c.shape[0], c.shape[1], float(s), float(temp),
+                                 int(top_k), float(top_p), C.c_uint64(seed & (2 ** 64 - 1)), int(position), vp(tokens),
+                                 tokens.stride(0), vp(tokens_alt), tokens_alt.stride(0),
+                                 vp(None if logp is None else c), vp(logp), 0 if logp is None else logp.stride(0),
+                                 stream_ptr()))
