@@ -241,12 +241,21 @@ extern "C" int jk_f32_forward(const jk_f32_args* a, const jk_f32_layer* layers, 
     float* enc_tmp = g + (size_t)M * Mw;
     double sc = 1.0 / sqrt(sqrt((double)dh));
     const float scale2 = (float)(sc * sc);
+    // every layer is checked before the first launch: x is rewritten in place, so a table that fails at layer l must
+    // not leave layers 0 .. l-1 applied
+    for (int l = 0; l < a->depth; ++l) {
+        const jk_f32_layer& L = layers[l];
+        const int af = L.attn_func;
+        JK_REQUIRE(af == 0 || af == 1 || af == 2 || af == 3 || af == 6 || af == 7, "layer %d: attn_func %d is not built in the fp32 path", l, af);
+        JK_REQUIRE(L.k_cache && L.v_cache, "layer %d: K/V cache (or forward-mode scratch) is required", l);
+        JK_REQUIRE(af != 6 || a->encoder_kv || a->p0 > 0, "layer %d: encoder_kv is required at position 0", l);
+        const int Lc = (af == 6) ? a->encoder_dims : a->n_ctx;
+        JK_REQUIRE((size_t)(dh + Lc) * sizeof(float) <= 96 * 1024, "layer %d: attention row of %d keys does not fit shared memory in the fp32 path", l, Lc);
+    }
     if (int rc = jk::set_max_smem_once<attn_f32_kernel>(96 * 1024)) return rc;
     for (int l = 0; l < a->depth; ++l) {
         const jk_f32_layer& L = layers[l];
         const int af = L.attn_func;
-        JK_REQUIRE(af == 0 || af == 1 || af == 2 || af == 3 || af == 6 || af == 7, "attn_func %d is not built in the fp32 path", af);
-        JK_REQUIRE(L.k_cache && L.v_cache, "layer %d: K/V cache (or forward-mode scratch) is required", l);
         int rc = jk_layernorm_f32(a->x, L.ln0_g, L.ln0_b, xn, M, W, 1e-5f, stream_);
         if (rc) return rc;
         const int Lc = (af == 6) ? a->encoder_dims : a->n_ctx;
@@ -254,7 +263,6 @@ extern "C" int jk_f32_forward(const jk_f32_args* a, const jk_f32_layer* layers, 
         A.kc = L.k_cache; A.vc = L.v_cache; A.out = att; A.w_out = L.attn_w; A.P = P; A.p0 = a->p0; A.S = S; A.H = H; A.dh = dh;
         A.bc = bc; A.attn_func = af; A.prime = prime; A.Lc = Lc; A.Lk = Lc; A.scale2 = scale2;
         if (af == 6) {
-            JK_REQUIRE(a->encoder_kv || a->p0 > 0, "layer %d: encoder_kv is required at position 0", l);
             rc = sgemm(xn, L.c_attn_w, L.c_attn_b, nullptr, qkv, M, S, W, 0, F32_EPI_NONE, stream);
             if (rc) return rc;
             if (a->p0 == 0) {      // c_enc_kv(encoder_kv) once per window (factored_attention.py:273-287)
@@ -275,7 +283,6 @@ extern "C" int jk_f32_forward(const jk_f32_args* a, const jk_f32_layer* layers, 
             A.q = qkv; A.q_stride = 3 * S;
         }
         const size_t smem = (size_t)(dh + Lc) * sizeof(float);
-        JK_REQUIRE(smem <= 96 * 1024, "attention row of %d keys does not fit shared memory in the fp32 path", Lc);
         attn_f32_kernel<<<dim3(P, H, n), 128, smem, stream>>>(A);
         JK_CHECK_CUDA(cudaGetLastError());
         rc = sgemm(att, L.c_proj_w, L.c_proj_b, a->x, a->x, M, W, S, 0, F32_EPI_RESIDUAL, stream);      // x1 = x + a
