@@ -321,7 +321,7 @@ __device__ __forceinline__ void stage_acts_body(const unsigned long long* in, in
             // those are kilobytes of library code in the instruction cache)
             const double rk = (double)(1.0f / (float)K);    // K is a multiple of 16: exact for powers of two, 1e-7 rel otherwise
             const double m = (double)val * (1.0 / 65536.0) * rk;
-            double var = (double)sq * (1.0 / 16384.0) * rk - m * m;
+            double var = fma(rk, (double)sq * (1.0 / 16384.0), -(m * m));   // one rounding: oracle/decode_stats.py states it so
             var = var < 0.0 ? 0.0 : var;
             rstd = 1.0f / sqrtf((float)var + 1e-5f);
             mean = -(float)m * rstd;                        // staged as x * rstd + (-mean * rstd), then * gamma + beta
