@@ -294,7 +294,7 @@ class ConditionalAutoregressive2D(nn.Module):
         return loss, None
 
     def regenerate(self, x, start, end, n_candidates, x_cond=None, y_cond=None, encoder_kv=None, fp16=True, temp=1.0,
-                   top_k=0, top_p=0.0):
+                   top_k=0, top_p=0.0, pack=False):
         """Resample the span [start, end) of a window x [N, D] (1 < D <= input_dims) given the codes on both sides of it
         (not in the reference): sampling-importance-resampling.  Per item the prime x[i, :start] runs once on one row
         and is fanned out to n_candidates rows (primed_sample's one-row prime), the rows draw [start, end), the kept
@@ -306,9 +306,12 @@ class ConditionalAutoregressive2D(nn.Module):
         the suffix's codes over the stack's activations + cond, in one fused kernel (jk_xout_logprob).
         x_cond [N, input_dims or 1, width], y_cond [N, 1, width] and encoder_kv [N, ...] as sample takes them.
         Returns (x_new [N, D], scores fp32 [N, n_candidates]): x with the kept span, and every candidate's suffix
-        log-likelihood in nats.  Codes outside [start, end) are returned unchanged."""
+        log-likelihood in nats.  Codes outside [start, end) are returned unchanged.
+        pack (not in the reference): the N items share ONE window of N * n_candidates engine rows (at most
+        engine_rows()): the N primes run once on N rows, select fans item i out to rows [i K, (i + 1) K), the span is
+        drawn on every row and the suffixes are teacher-forced in one continuation prefill.  One item draws exactly what
+        the unpacked form draws; with more, the draws differ from it, since the sampler's stream is keyed by row."""
         from .._lib import JK_MAX_BATCH
-        from ..score import xout_logprob
         assert not self.only_encode
         with t.no_grad():
             x = self.preprocess(x)
@@ -321,27 +324,42 @@ class ConditionalAutoregressive2D(nn.Module):
                 raise ValueError(f"span [{start}, {end}) leaves no codes after it to rank the candidates by")
             if not 1 <= K <= JK_MAX_BATCH:
                 raise ValueError(f"n_candidates {K} outside [1, {JK_MAX_BATCH}]")
+            if pack and N * K > self.engine_rows():
+                raise ValueError(f"{N} packed items of {K} candidates need {N * K} engine rows: at most "
+                                 f"{self.engine_rows()} fit one engine of this model")
             assert (0 <= x).all() and (x < self.bins).all()
             x_cond, y_cond = self._check_conds(N, x_cond, y_cond)
             y_cond = None if y_cond is None else y_cond.view(N, 1, self.width)
             x_new, scores = x.clone(), t.empty(N, K, dtype=t.float32, device=x.device)
-            rows = lambda v, i: None if v is None else (v[i:i + 1] if start else
-                                                        v[i:i + 1].expand(K, *v.shape[1:]).contiguous())
-            for i in range(N):
-                # the prime runs on one row; without one the K rows start from the start token together
-                prime = x[i:i + 1, :start] if start else x.new_zeros(K, 0)
-                cls = SamplingWindow if fp16 else SamplingWindowF32
-                win = cls(self, K, prime, rows(x_cond, i), rows(y_cond, i), rows(encoder_kv, i), fp16, temp, top_k,
-                          top_p, False, D)
-                win.advance(end)
-                win.tokens[:, end:] = x[i, end:]
-                acts = self._suffix_acts(win, end, D)
-                logp = xout_logprob(acts.reshape(-1, self.width), self.x_out.weight, win.tokens[:, end:].reshape(-1))
-                scores[i] = logp.view(K, D - end).double().sum(1).float()
-                best = int(t.argmax(scores[i]))
-                x_new[i, start:end] = win.tokens[best, start:end]
-                self.transformer.del_cache()
+            M = N if pack else 1
+            part = lambda v, i: None if v is None else v[i:i + M]
+            for i in range(0, N, M):
+                x_new[i:i + M], scores[i:i + M] = self._regenerate_items(
+                    x[i:i + M], start, end, K, part(x_cond, i), part(y_cond, i), part(encoder_kv, i), fp16, temp,
+                    top_k, top_p)
             return x_new, scores
+
+    def _regenerate_items(self, x, start, end, K, x_cond, y_cond, encoder_kv, fp16, temp, top_k, top_p):
+        """regenerate's span of the M items x [M, D] in one window of M K rows: item i's candidates are rows
+        [i K, (i + 1) K).  Returns (x_new [M, D], scores fp32 [M, K])."""
+        from ..score import xout_logprob
+        M, D = x.shape
+        # the primes run on M rows; without one the M K rows start from the start token together
+        prime = x[:, :start] if start else x.new_zeros(M * K, 0)
+        rows = lambda v: None if v is None else (v if start else v.repeat_interleave(K, dim=0))
+        cls = SamplingWindow if fp16 else SamplingWindowF32
+        win = cls(self, M * K, prime, rows(x_cond), rows(y_cond), rows(encoder_kv), fp16, temp, top_k, top_p, False, D)
+        win.advance(end)
+        win.tokens[:, end:] = x[:, end:].repeat_interleave(K, dim=0)
+        acts = self._suffix_acts(win, end, D)
+        logp = xout_logprob(acts.reshape(-1, self.width), self.x_out.weight, win.tokens[:, end:].reshape(-1))
+        scores = logp.view(M * K, D - end).double().sum(1).float().view(M, K)
+        x_new = x.clone()
+        for i in range(M):
+            best = int(t.argmax(scores[i]))
+            x_new[i, start:end] = win.tokens[i * K + best, start:end]
+        self.transformer.del_cache()
+        return x_new, scores
 
     def _suffix_acts(self, win, end, D):
         """the stack's output + cond at positions [end, D) of a window's rows, which stand at position end: one
@@ -376,11 +394,14 @@ class ConditionalAutoregressive2D(nn.Module):
                 return n
         return 0
 
-    def guided_items(self):
-        """the most items a guided window takes: its 2N rows must fit one engine of this model (items_per_prefill: 32
-        rows, 16 on 5b_lyrics)"""
+    def engine_rows(self):
+        """the most rows one window of this model runs on one engine (items_per_prefill: 32 rows, 16 on 5b_lyrics)"""
         from .._lib import JK_MAX_BATCH
-        return (self.items_per_prefill(JK_MAX_BATCH) or JK_MAX_BATCH) // 2
+        return self.items_per_prefill(JK_MAX_BATCH) or JK_MAX_BATCH
+
+    def guided_items(self):
+        """the most items a guided window takes: its 2N rows must fit one engine of this model (engine_rows)"""
+        return self.engine_rows() // 2
 
     def layer_acts(self, x, x_cond=None, y_cond=None, encoder_kv=None, layers=(), fp16=True, pool=True, add_cond=True,
                    t0=0):
@@ -548,15 +569,18 @@ class _Rows:
         assert P < self.sample_tokens <= ca.input_dims, \
             f"need given tokens {P} < sample_tokens {self.sample_tokens} <= input_dims {ca.input_dims}"
         # one given row for N samples: its positions run on one row (a pair of rows when guided), then its state is
-        # repeated to all N (_fan_out)
+        # repeated to all N (_fan_out); M given rows for N = M K rows (packed regeneration): row i's state goes to
+        # rows [i K, (i + 1) K)
         self.n = prime.shape[0] if P else N
-        assert self.n in (G, N), f"prime of {self.n} rows for {N} samples"
+        assert self.n in (G, N) or (G == 1 and N % self.n == 0), f"prime of {self.n} rows for {N} samples"
         self.x_cond, self.y_cond = ca._check_conds(self.n, x_cond, y_cond)
         dev = ca.x_emb.weight.device
         self.tokens = t.zeros(N, self.sample_tokens, dtype=t.long, device=dev)
         if P:
             assert (0 <= prime).all() and (prime < ca.bins).all()
-            self.tokens[:, :P] = prime.repeat_interleave(N // prime.shape[0], dim=0)    # a one-row prime on every row
+            # the given rows in rows [0, n), which the prefill and the steps of given positions read; _fan_out copies
+            # them to the other rows
+            self.tokens[:self.n, :P] = prime
         if (select_every is None) != (select_keep is None):
             raise ValueError("keep-best selection needs both select_every and select_keep")
         if select_every is not None:
@@ -613,8 +637,8 @@ class _Rows:
 
     def _fan_out(self):
         """the given positions of a one-row prime are done: every row continues from it (guided: every conditional
-        row from row 0, every alternative row from row 1)"""
-        self.select([g for g in range(self.G) for _ in range(self.items)])
+        row from row 0, every alternative row from row 1; n given rows: each to N / n consecutive rows)"""
+        self.select([b // (self.N // self.n) for b in range(self.N)])
 
     def _drawn(self, sample_t, x):
         """position sample_t of the running rows from their logits x [n, bins], then keep-best selection when the

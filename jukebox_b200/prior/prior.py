@@ -425,18 +425,24 @@ class SimplePrior(nn.Module):
         """the most items one guided sample call takes (ConditionalAutoregressive2D.guided_items)"""
         return self.prior.guided_items()
 
-    def regenerate(self, z, start, end, n_candidates, z_conds=[], y=None, fp16=True, temp=1.0, top_k=0, top_p=0.0):
+    def engine_rows(self):
+        """the most rows one window of this level runs on one engine (ConditionalAutoregressive2D.engine_rows)"""
+        return self.prior.engine_rows()
+
+    def regenerate(self, z, start, end, n_candidates, z_conds=[], y=None, fp16=True, temp=1.0, top_k=0, top_p=0.0,
+                   pack=False):
         """Resample codes [start, end) of a window of codes z [N, D] of this level (not in the reference), conditioned as
         score conditions a window: n_candidates draws of the span per item, ranked by the log-likelihood of the codes
         after it (ConditionalAutoregressive2D.regenerate).  A single_enc_dec prior takes its lyric head into the
         sequence (the span moves behind it, and the codes are shifted into its token space as sampled codes are); a
         separate lyric encoder gives the encoder-decoder layers their keys, repeated to the candidate rows.  Returns
         (z_new [N, D], scores fp32 [N, n_candidates]): the kept span in z, and each candidate's suffix log-likelihood in
-        nats."""
+        nats.  pack: the N items (windows of one geometry) in one engine window of N * n_candidates <= engine_rows()
+        rows, with their own conditioning (ConditionalAutoregressive2D.regenerate)."""
         with t.no_grad():
             seq, x_cond, y_cond, enc, _, pl = self._condition(z, z_conds, y, fp16)
             out, scores = self.prior.regenerate(seq, pl + int(start), pl + int(end), n_candidates, x_cond, y_cond, enc,
-                                                fp16=fp16, temp=temp, top_k=top_k, top_p=top_p)
+                                                fp16=fp16, temp=temp, top_k=top_k, top_p=top_p, pack=pack)
             return (self.spaces.last(out) if self.single_enc_dec else out), scores
 
     def layer_acts(self, z, z_conds=[], y=None, layers=(), fp16=True, pool=True):

@@ -10,6 +10,8 @@ continue_sample, upsample, primed_sample, load_codes.  The work itself is organi
   * `LevelRun` owns one level's codes / labels / sampling options and executes windows: slice the context,
     fetch the per-window conditioning from the prior, split the batch into engine-sized pieces
     (`max_batch_size`), call `prior.sample`, append the new tokens.
+  * `plan_segments` / `SegmentedLevel` (sampling_kwargs key `segments`): an upsampler level drawn as many equal
+    stretches on the engine's rows at once, each seam then redrawn by packed regeneration (DESIGN.md).
   * priors stay on the GPU between levels; `hps.offload_priors` restores the reference's cpu() shuffling.  At
     `max_batch_size` 32 the decode engines' arenas alone (`jk_prior_plan`, computed) are 23.5 GB for `1b_lyrics` and
     20.6 GB for each `upsampler_level_*`, 64.7 GB of an 80 GB H100 (INTEGRATION.md lists what that leaves out).
@@ -69,13 +71,22 @@ def null_labels(prior, labels):
 class LevelRun:
     """One level of one sampling job: the codes sampled so far and what is needed to extend them.
     sampling_kwargs may hold guidance_scale and guidance_labels (guided sampling, SimplePrior.sample): a labels dict like
-    `labels`, or None for null_labels(prior, labels); it is windowed as the labels are (get_y), lyrics included."""
+    `labels`, or None for null_labels(prior, labels); it is windowed as the labels are (get_y), lyrics included.
+    They may hold segments (default 1), seam_tokens (default n_ctx // 8) and seam_candidates (default 4): with
+    segments > 1, extend_to draws an upsampler level from nothing as that many stretches side by side on the engine's
+    rows and redraws each seam (SegmentedLevel); max_batch_size then counts rows (items x segments), not items, and
+    the seam pass packs up to prior.engine_rows() rows (32; 16 on 5b_lyrics) whatever max_batch_size is.  Only a whole
+    level (extend_to: sample_level, _sample) is drawn in segments; sample_partial_window and sample_single_window refuse
+    segments > 1."""
 
     def __init__(self, zs, labels, sampling_kwargs, level, prior, hps):
         self.zs, self.labels, self.level, self.prior, self.hps = zs, labels, level, prior, hps
         opts = dict(sampling_kwargs)
         opts.pop('sample_tokens', None)           # per-window, set by run_window
         self.max_batch = opts.pop('max_batch_size')
+        self.segments = int(opts.pop('segments', 1))
+        self.seam_tokens = opts.pop('seam_tokens', None)
+        self.seam_candidates = int(opts.pop('seam_candidates', 4))
         self.guidance_labels = opts.pop('guidance_labels', None)
         if opts.get('guidance_scale') is not None:
             limit = prior.guided_items()
@@ -90,6 +101,12 @@ class LevelRun:
 
     def have(self):
         return self.zs[self.level].shape[1]
+
+    def one_window(self):
+        """a single window is asked for: segments > 1 draws a whole level, so it is refused"""
+        if self.segments > 1:
+            raise ValueError(f"segments {self.segments} draws a whole level (sample_level): a single window is not cut "
+                             "into segments")
 
     def run_window(self, win):
         prior, level = self.prior, self.level
@@ -135,6 +152,8 @@ class LevelRun:
                 self.zs[lv] = z
 
     def extend_to(self, total_length, hop_length):
+        if self.segments > 1:
+            return SegmentedLevel(self).extend_to(total_length, hop_length)
         for win in plan_windows(self.have(), total_length, self.prior.n_ctx, hop_length):
             self.run_window(win)
         return self.zs
@@ -192,6 +211,19 @@ def regen_window(T, start, end, n_ctx):
     return w0, min(T, w0 + n_ctx)
 
 
+def aligned_regen_window(T, start, end, n_ctx, ds):
+    """regen_window with its start moved to a multiple of ds, where the upper-level codes under a window start
+    (get_z_conds)"""
+    w0, w1 = regen_window(T, start, end, n_ctx)
+    if w0 % ds:
+        w0 -= w0 % ds
+        if min(T, w0 + n_ctx) <= end:
+            w0 += ds
+        w1 = min(T, w0 + n_ctx)
+        assert w0 <= start and end < w1, f"no window aligned to {ds} holds [{start}, {end}) and a code after it"
+    return w0, w1
+
+
 def regenerate_level(zs, labels, sampling_kwargs, level, prior, start, end, hps, n_candidates=16):
     """Codes [start, end) of one level drawn again, n_candidates per item, and the candidate under which the level's
     codes after the span are likeliest kept (SimplePrior.regenerate), in the window regen_window places (its start moved
@@ -206,14 +238,7 @@ def regenerate_level(zs, labels, sampling_kwargs, level, prior, start, end, hps,
         raise ValueError("guided sampling (guidance_scale / guidance_labels) is not combined with regeneration")
     z = zs[level]
     T = z.shape[1]
-    w0, w1 = regen_window(T, start, end, prior.n_ctx)
-    ds = prior.cond_downsample if prior.x_cond else 1
-    if w0 % ds:     # the upper-level codes under the window start on a code of the level above (get_z_conds)
-        w0 -= w0 % ds
-        if min(T, w0 + prior.n_ctx) <= end:
-            w0 += ds
-        w1 = min(T, w0 + prior.n_ctx)
-        assert w0 <= start and end < w1, f"no window aligned to {ds} holds [{start}, {end}) and a code after it"
+    w0, w1 = aligned_regen_window(T, start, end, prior.n_ctx, prior.cond_downsample if prior.x_cond else 1)
     how = {k: opts[k] for k in ('fp16', 'temp', 'top_k', 'top_p') if k in opts}
     done, scores = [], []
     for ctx_i, upper_i, y_i in window_pieces(prior, zs, labels, level, w0, w1, opts.get('max_batch_size', T)):
@@ -241,10 +266,175 @@ def regenerate(zs, labels, sampling_kwargs, priors, start, end, hps, n_candidate
     return zs, scores
 
 
+# ---- segment-parallel sampling of an upsampler level ---------------------------------------------------------
+@dataclass(frozen=True)
+class Seam:
+    start: int              # first code redrawn: a boundary between two kept ranges
+    end: int                # end of the redrawn span
+    w0: int                 # the window [w0, w1) of the level it is redrawn in (aligned_regen_window)
+    w1: int
+
+    @property
+    def geometry(self):
+        """(window length, offset of the span in it): seams of one geometry run packed on one engine window"""
+        return self.w1 - self.w0, self.start - self.w0
+
+
+@dataclass(frozen=True)
+class SegmentPlan:
+    length: int             # L: codes of every segment
+    starts: tuple           # s_j: first code of segment j in the level
+    windows: tuple          # the windows every segment runs, from its own start: plan_windows(0, L, ...)
+    kept: tuple             # (k_j, k_j+1): the codes of the level segment j supplies; they partition [0, T)
+    seams: tuple            # a Seam at every k_j, j >= 1
+
+    def groups(self):
+        """{geometry: [Seam, ...]}"""
+        out = {}
+        for seam in self.seams:
+            out.setdefault(seam.geometry, []).append(seam)
+        return out
+
+
+def _segment_length(T, n, n_ctx, ds, seam_tokens):
+    """the length L of n segments of a level of T codes (T / n rounded up to a multiple of ds), or None when they do not
+    fit: L < n_ctx, or the last kept range too short to hold a seam span and a code after it"""
+    L = -(-T // n)
+    L = -(-L // ds) * ds
+    return L if L >= n_ctx and T - (n - 1) * L > seam_tokens else None
+
+
+def plan_segments(T, n_ctx, hop_length, n_segments, cond_downsample, seam_tokens):
+    """A level of T codes drawn as n_segments stretches side by side.  Every segment has the same length L >= n_ctx and
+    runs the same windows plan_windows(0, L, n_ctx, hop_length) from its own start, so that all of them stand at one
+    position of the engine.  Segment j starts at s_j = j L (the last at T - L, so that it ends at T) and supplies the
+    codes [k_j, k_j+1) = [j L, (j + 1) L) (the last [(n - 1) L, T): its leading overlap with the segment before is
+    dropped).  Starts and windows are multiples of cond_downsample (get_z_conds).  At every k_j, j >= 1, a Seam: its span
+    [k_j, k_j + seam_tokens) is drawn again in the window aligned_regen_window places, which holds kept codes after it.
+    n_segments 1: the windows of plan_windows(0, T, ...) and no seams.  ValueError when the count does not fit."""
+    T, n_ctx, hop, n, st = int(T), int(n_ctx), int(hop_length), int(n_segments), int(seam_tokens)
+    ds = int(cond_downsample or 1)
+    if n < 1:
+        raise ValueError(f"segments {n} must be >= 1")
+    if n == 1:
+        return SegmentPlan(T, (0,), tuple(plan_windows(0, T, n_ctx, hop)), ((0, T),), ())
+    if T % ds or n_ctx % ds or hop % ds:
+        raise ValueError(f"segments start on codes of the level above: T {T}, n_ctx {n_ctx} and hop {hop} must be "
+                         f"multiples of {ds}")
+    if not 0 < st < n_ctx:
+        raise ValueError(f"seam_tokens {st} outside [1, {n_ctx})")
+    L = _segment_length(T, n, n_ctx, ds, st)
+    if L is None:
+        most = max([m for m in range(2, T // n_ctx + 2) if _segment_length(T, m, n_ctx, ds, st)], default=1)
+        raise ValueError(f"{n} segments of a level of {T} codes do not fit: each needs >= n_ctx {n_ctx} codes and the "
+                         f"last a seam of {st} codes with a code after it; at most {most} fit")
+    bounds = [j * L for j in range(n)] + [T]
+    seams = []
+    for k in bounds[1:-1]:
+        w0, w1 = aligned_regen_window(T, k, k + st, n_ctx, ds)
+        seams.append(Seam(k, k + st, w0, w1))
+    return SegmentPlan(L, tuple(bounds[:n - 1]) + (T - L,), tuple(plan_windows(0, L, n_ctx, hop)),
+                       tuple(zip(bounds[:-1], bounds[1:])), tuple(seams))
+
+
+def row_conditioning(prior, zs, labels, items, starts):
+    """the upper-level codes (a list, or None) and label rows (or None) of engine rows that each read item items[r] in
+    the window of this level that starts at starts[r] (get_z_conds / get_y of that window)"""
+    per_start, ups, ys = {}, [], []
+    for i, s in zip(items, starts):
+        if s not in per_start:
+            per_start[s] = prior.get_z_conds(zs, s, s + prior.n_ctx), prior.get_y(labels, s)
+        up, y = per_start[s]
+        ups.append(None if up is None else [u[i] for u in up])
+        ys.append(None if y is None else y[i])
+    up = None if ups[0] is None else [t.stack([u[k] for u in ups]) for k in range(len(ups[0]))]
+    return up, (None if ys[0] is None else t.stack(ys))
+
+
+class SegmentedLevel:
+    """A LevelRun with segments > 1: the level is drawn from nothing as plan_segments' stretches.  Rows are items x
+    segments, item-major (row i S + j: item i, segment j); in every window of the shared plan each row reads its own
+    context, the upper-level codes under its own stretch and labels at its own offset (get_z_conds / get_y at
+    s_j + window start), and the rows run through prior.sample in pieces of max_batch_size rows.  The kept ranges are
+    stitched into zs[level], then every seam is redrawn given the codes on both sides of it: seam_candidates draws of its
+    span, the one under which the kept codes after it are likeliest is kept (SimplePrior.regenerate, packed: seams of one
+    geometry x items in pieces of the engine's rows).  No seam window holds another seam's span, so the order of the
+    seams does not matter."""
+
+    def __init__(self, run):
+        prior = run.prior
+        if not prior.x_cond:
+            raise ValueError("segments > 1 needs an upsampler: the top level has no upper-level codes to carry the "
+                             "song's structure across its stretches")
+        if run.have():
+            raise ValueError(f"segments > 1 draws a level from nothing, but level {run.level} already holds "
+                             f"{run.have()} codes: the stretches could not share one engine position with them")
+        if run.opts.get('select_every') is not None:
+            raise ValueError("keep-best selection (select_every) is not combined with segments > 1")
+        if run.guidance_labels is not None or run.opts.get('guidance_scale') is not None:
+            raise ValueError("guided sampling (guidance_scale / guidance_labels) is not combined with segments > 1")
+        self.run = run
+
+    def extend_to(self, total_length, hop_length):
+        run, prior = self.run, self.run.prior
+        zs, level = run.zs, run.level
+        N = zs[level].shape[0]
+        st = prior.n_ctx // 8 if run.seam_tokens is None else int(run.seam_tokens)
+        plan = plan_segments(total_length, prior.n_ctx, hop_length, run.segments, prior.cond_downsample, st)
+        S, L = len(plan.starts), plan.length
+        items = [i for i in range(N) for _ in range(S)]
+        offsets = [s for _ in range(N) for s in plan.starts]
+        codes = zs[level].new_zeros(N * S, 0)
+        for win in plan.windows:
+            codes = self.run_window(codes, win, items, offsets)
+        codes = codes.view(N, S, L)
+        zs[level] = t.cat([codes[:, j, k0 - s:k1 - s] for j, (s, (k0, k1)) in enumerate(zip(plan.starts, plan.kept))],
+                          dim=1)
+        self.redraw_seams(plan, st)
+        return zs
+
+    def run_window(self, codes, win, items, offsets):
+        """codes [rows, have]: every row's stretch so far, extended by window win (from each row's own start)"""
+        run, prior = self.run, self.run.prior
+        context = codes[:, win.start:win.start + prior.n_ctx]
+        missing = win.sample_tokens - context.shape[1]
+        print_once(f"Sampling {win.sample_tokens} tokens for [{win.start},{win.start + win.sample_tokens}] of "
+                   f"{codes.shape[0]} segment rows. Conditioning on {context.shape[1]} tokens")
+        if missing <= 0:
+            return codes
+        extra = {} if win.sample_tokens == prior.n_ctx else dict(sample_tokens=win.sample_tokens)
+        up, y = row_conditioning(prior, run.zs, run.labels, items, [s + win.start for s in offsets])
+        part = lambda v, r: None if v is None else v[r:r + run.max_batch]
+        done = []
+        for r in range(0, codes.shape[0], run.max_batch):
+            ctx = context[r:r + run.max_batch]
+            done.append(prior.sample(n_samples=ctx.shape[0], z=ctx, z_conds=None if up is None else
+                                     [u[r:r + run.max_batch].contiguous() for u in up], y=part(y, r),
+                                     **run.opts, **extra))
+        return t.cat([codes, t.cat(done, dim=0)[:, -missing:]], dim=1)
+
+    def redraw_seams(self, plan, seam_tokens):
+        run, prior = self.run, self.run.prior
+        z = run.zs[run.level]
+        K = run.seam_candidates
+        how = {k: run.opts[k] for k in ('fp16', 'temp', 'top_k', 'top_p') if k in run.opts}
+        per_call = max(1, prior.engine_rows() // K)
+        for (_, off), seams in plan.groups().items():
+            pairs = [(seam, i) for seam in seams for i in range(z.shape[0])]
+            for p0 in range(0, len(pairs), per_call):
+                piece = pairs[p0:p0 + per_call]
+                ctx = t.stack([z[i, seam.w0:seam.w1] for seam, i in piece])
+                up, y = row_conditioning(prior, run.zs, run.labels, [i for _, i in piece], [seam.w0 for seam, _ in piece])
+                out, _ = prior.regenerate(ctx, off, off + seam_tokens, K, up, y, pack=True, **how)
+                for r, (seam, i) in enumerate(piece):
+                    z[i, seam.start:seam.end] = out[r, off:off + seam_tokens].to(z.device)
+
+
 # ---- the reference's entry points -------------------------------------------------------------------------
 def sample_partial_window(zs, labels, sampling_kwargs, level, prior, tokens_to_sample, hps):
     """`tokens_to_sample` new tokens at `level`, the context sliding once it is full"""
     run = LevelRun(zs, labels, sampling_kwargs, level, prior, hps)
+    run.one_window()
     have = run.have()
     if have + tokens_to_sample < prior.n_ctx:
         win = Window(0, have + tokens_to_sample)
@@ -257,6 +447,7 @@ def sample_partial_window(zs, labels, sampling_kwargs, level, prior, tokens_to_s
 def sample_single_window(zs, labels, sampling_kwargs, level, prior, start, hps):
     """the window of prior.n_ctx tokens that starts at `start`; tokens already there are the prime"""
     run = LevelRun(zs, labels, sampling_kwargs, level, prior, hps)
+    run.one_window()
     run.run_window(Window(start, sampling_kwargs.get('sample_tokens', prior.n_ctx)))
     return zs
 
