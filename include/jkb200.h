@@ -535,6 +535,42 @@ int jk_f32_embed(float* x, const int64_t* tokens, int64_t tok_stride, const floa
 int jk_f32_linear(const float* x, const float* w, const float* b, float* y, int M, int N, int K, int w_is_nk,
                   jk_stream_t stream);
 
+/* ---- gradients of the fp32 path (fine-tuning a prior's decoder) --------------------------------------------------------
+ * Deterministic kernels: no atomics on any gradient sum, so two identical calls give bit-identical results.  Every
+ * gradient is ADDED to what its buffer holds (.grad accumulates over micro-batches and over the tied x_emb / x_out).
+ * One structure per layer mirrors jk_f32_layer's parameters; NULL = frozen, its weight-gradient work is skipped. */
+typedef struct jk_f32_grad_layer {
+    float *ln0_g, *ln0_b, *ln1_g, *ln1_b;
+    float *c_attn_w, *c_attn_b;
+    float *c_enc_kv_w, *c_enc_kv_b;
+    float *c_proj_w, *c_proj_b;
+    float *fc_w, *fc_b;
+    float *proj2_w, *proj2_b;
+} jk_f32_grad_layer;
+
+int jk_f32_backward_workspace_floats(const jk_f32_args* a, size_t* floats);
+/* Backward of jk_f32_forward over a whole window (p0 = 0, P = n_ctx) through layers depth-1 .. 0 of the table.  Each
+ * layer's forward is recomputed from saved_inputs[l] ([n, P, width], the layer's input), then differentiated.  dx holds
+ * dL/d(output of the last layer) on entry and dL/d(input of layer 0) on return.  a->x is not read; a->work holds
+ * jk_f32_backward_workspace_floats() floats; a->encoder_kv is read by enc-dec layers.  d_encoder_kv ([n, encoder_dims,
+ * width], or NULL) receives the enc-dec layers' gradient of encoder_kv, added.  All arguments are checked first. */
+int jk_f32_backward(const jk_f32_args* a, const jk_f32_layer* layers, const jk_f32_grad_layer* grads,
+                    const float* const* saved_inputs, float* dx, float* d_encoder_kv, jk_stream_t stream);
+/* dw[K, N] (+)= x[M, K]^T . dy[M, N] and db[N] (+)= sum_m dy[m, :] (either may be NULL): a Conv1D's weight gradient.
+ * Also nn.Linear's ([N, K] weight) with x and dy swapped. */
+int jk_f32_linear_wgrad(const float* x, const float* dy, float* dw, float* db, int M, int K, int N, int accumulate,
+                        jk_stream_t stream);
+/* Gradients of jk_f32_embed's tables from dh = dL/dx [n, P, width] (p0 = 0, no x_cond): d_x_emb [bins, width] by token
+ * id (pairs sorted once, then summed per id in row order; work holds 2 n (P-1) ints), d_pos_emb [P, width] (sum over
+ * items), d_start_token [width] (position 0 of every item; NULL when the prior has y_cond).  Any may be NULL. */
+int jk_f32_embed_backward(const float* dh, const int64_t* tokens, int64_t tok_stride, int n, int P, int width, int bins,
+                          float* d_x_emb, float* d_pos_emb, float* d_start_token, int* work, int accumulate,
+                          jk_stream_t stream);
+/* Cross-entropy head over logits [M, bins] (jk_f32_linear's x_out product): loss[m] = logsumexp - logits[m, target]
+ * (nats), and logits overwritten with row_weight[m] (softmax - onehot(target)), the gradient of sum_m w_m loss_m. */
+int jk_f32_xent_backward(float* logits, const int64_t* targets, const float* row_weight, float* loss, int M, int bins,
+                         jk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

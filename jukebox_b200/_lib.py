@@ -50,6 +50,12 @@ class F32Args(C.Structure):
                [("x", C.c_void_p), ("encoder_kv", C.c_void_p), ("work", C.c_void_p)]
 
 
+class F32GradLayer(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in
+                ("ln0_g", "ln0_b", "ln1_g", "ln1_b", "c_attn_w", "c_attn_b", "c_enc_kv_w", "c_enc_kv_b",
+                 "c_proj_w", "c_proj_b", "fc_w", "fc_b", "proj2_w", "proj2_b")]
+
+
 class StepArgs(C.Structure):
     _fields_ = [("n_samples", C.c_int32), ("x_in", C.c_void_p), ("tokens", C.c_void_p),
                 ("tok_stride", C.c_int64), ("y_cond", C.c_void_p), ("x_cond", C.c_void_p),
@@ -154,6 +160,11 @@ SIGNATURES = {
     "jk_f32_forward": (_I, [C.POINTER(F32Args), C.POINTER(F32Layer), _P]),
     "jk_f32_embed": (_I, [_P, _P, _L, _P, _P, _L, _P, _P, _P, _I, _I, _I, _I, _P]),
     "jk_f32_linear": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "jk_f32_backward_workspace_floats": (_I, [C.POINTER(F32Args), C.POINTER(C.c_size_t)]),
+    "jk_f32_backward": (_I, [C.POINTER(F32Args), C.POINTER(F32Layer), C.POINTER(F32GradLayer), C.POINTER(_P), _P, _P, _P]),
+    "jk_f32_linear_wgrad": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "jk_f32_embed_backward": (_I, [_P, _P, _L, _I, _I, _I, _I, _P, _P, _P, _P, _I, _P]),
+    "jk_f32_xent_backward": (_I, [_P, _P, _P, _P, _I, _I, _P]),
 }
 
 _lib = None

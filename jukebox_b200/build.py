@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libjkb200.so")
 STAMP = os.path.join(HERE, ".libjkb200.stamp")
-SOURCES = ["api.cu", "decode_engine.cu", "f32_path.cu", "prefill.cu", "prefill_gemm.cu", "sampling.cu", "score.cu", "select.cu", "stft_loss.cu", "vqvae_kernels.cu", "vqvae_t5.cu"]
+SOURCES = ["api.cu", "decode_engine.cu", "f32_grad.cu", "f32_path.cu", "prefill.cu", "prefill_gemm.cu", "sampling.cu", "score.cu", "select.cu", "stft_loss.cu", "vqvae_kernels.cu", "vqvae_t5.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "--shared", "-Xcompiler", "-fPIC", 
               "-Xcompiler", "-Wno-unused-function", "--expt-relaxed-constexpr", "-rdc=false"]

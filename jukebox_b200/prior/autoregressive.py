@@ -115,9 +115,10 @@ class ConditionalAutoregressive2D(nn.Module):
         x_out = None if self.only_encode else self.x_out.weight
         start = None if self.y_cond else self.start_token
         # the key lives ON the engine object: a freshly built engine (drop_engine after .cuda() /
-        # load_state_dict) always starts without embeddings, whatever address CPython gives it
-        key = (self.x_emb.weight.data_ptr(), self.pos_emb.pos_emb.data_ptr(),
-               None if x_out is None else x_out.data_ptr(), None if start is None else start.data_ptr())
+        # load_state_dict) always starts without embeddings, whatever address CPython gives it.  It holds each
+        # tensor's version counter too, so that an in-place update (an optimiser step) reloads them.
+        key = tuple(None if p is None else (p.data_ptr(), p._version)
+                    for p in (self.x_emb.weight, self.pos_emb.pos_emb, x_out, start))
         if getattr(eng, "_emb_key", None) != key:
             eng.set_embeddings(x_emb=self.x_emb.weight, pos_emb=self.pos_emb.pos_emb, x_out=x_out,
                                start_token=None if start is None else start.view(-1))
@@ -292,6 +293,85 @@ class ConditionalAutoregressive2D(nn.Module):
         if get_acts:
             return loss, acts
         return loss, None
+
+    # ---- gradients (fine-tuning; not in the reference's evaluation API) ---------------------------------------------
+    def grad_refusal(self, D=None):
+        """why loss_grad cannot run on this model (a message), or None.  D: the window's length, when known."""
+        params = [p for p in self.parameters() if p.requires_grad]
+        if not params:
+            return "no parameter of the prior requires grad: call requires_grad_(True) on what should be fine-tuned"
+        if any(p.dtype != t.float32 for p in self.parameters()):
+            return "fp16_params priors have no gradient path (fp32 parameters only)"
+        if self.transformer.res_scale_unsupported():
+            return "res_scale=True priors have no gradient path"
+        bad = sorted({b.attn_func for b in self.transformer._attn_mods} - {0, 1, 2, 3, 6, 7})
+        if bad:
+            return f"attn_func {bad} has no backward in the fp32 path"
+        if self.only_encode:
+            return "an only_encode model has no loss"
+        if D is not None and D != self.input_dims:
+            return f"gradients are taken over whole windows of {self.input_dims} tokens, got {D}"
+        if any(p.device.type != "cuda" for p in self.parameters()):
+            return "loss_grad needs the module on a CUDA device (jukebox_b200 has no CPU path)"
+        return None
+
+    def _lowest_trainable(self):
+        """the lowest layer the backward has to reach: 0 when an embedding table trains, else the lowest layer with a
+        parameter that requires grad, None when only x_out does"""
+        embs = [self.x_emb.weight, self.pos_emb.pos_emb] + ([] if self.y_cond else [self.start_token])
+        if any(p.requires_grad for p in embs):
+            return 0
+        for i, blk in enumerate(self.transformer._attn_mods):
+            if any(p.requires_grad for p in blk.parameters()):
+                return i
+        return None
+
+    def loss_grad(self, x, x_cond=None, y_cond=None, encoder_kv=None, row_weights=None):
+        """Gradients of sum_m w_m CE_m, CE_m the cross-entropy (nats) of token m of whole windows x [N, input_dims]
+        given the tokens before it, with the window conditioned as `forward(fp16=False)` conditions it.  row_weights:
+        w [N, input_dims] (default 1 / (N input_dims ln 2): the loss in bits per token).  Returns CE, fp32 [N, input_dims].
+
+        The gradients are ADDED into p.grad (fp32, created when None) of every parameter of this model that requires
+        grad; x_cond, y_cond and encoder_kv are constants.  The forward runs the fp32 path one layer at a time from the
+        lowest layer that trains, keeping each layer's input; jk_f32_backward then recomputes and differentiates each
+        layer on deterministic kernels (csrc/f32_grad.cu), so two identical calls add bit-identical gradients."""
+        from ..transformer import f32
+        why = self.grad_refusal(self.preprocess(x).shape[1])
+        if why:
+            raise ValueError(why)
+        with t.no_grad():
+            x, x_cond, y_cond = self._given(x, x_cond, y_cond, whole=True)
+            N, D = x.shape
+            if row_weights is None:
+                row_weights = t.full((N, D), 1.0 / (N * D * float(np.log(2.))), dtype=t.float32, device=x.device)
+            assert row_weights.shape == (N, D), f"row_weights {tuple(row_weights.shape)}, expected {(N, D)}"
+            tr = self.transformer
+            has6 = any(b.attn_func == 6 for b in tr._attn_mods)
+            if has6:
+                assert encoder_kv is not None and encoder_kv.shape == (N, tr.encoder_dims, self.width)
+                encoder_kv = encoder_kv.float().contiguous()
+            lowest = self._lowest_trainable()
+            path = tr.f32_path()
+            h0 = f32.embed(self, x, y_cond, x_cond, N, D, 0)
+            out, saved = path.run_saving(h0, encoder_kv, first=self.depth - 1 if lowest is None else lowest)
+            acts = self._add_x_cond(out, x_cond, 0, D).reshape(N * D, self.width).contiguous()
+            w_out = self.x_out.weight
+            dlogits = f32.linear_nk(acts, w_out)
+            ce = f32.xent_backward(dlogits, x.view(-1), row_weights.reshape(-1))
+            # a tied x_out / x_emb sums both of its gradients first and adds them to .grad once, so that a second
+            # identical call doubles .grad exactly
+            tied = w_out is self.x_emb.weight and w_out.requires_grad
+            d_out = t.zeros_like(w_out, dtype=t.float32) if tied else \
+                (f32.grad_buffer(w_out) if w_out.requires_grad else None)
+            if d_out is not None:
+                f32.linear_wgrad(dlogits, acts, dw=d_out)
+            if lowest is not None:
+                dh = path.backward(saved, f32.linear_kn(dlogits, w_out).view(N, D, self.width), encoder_kv, first=lowest)
+                if lowest == 0:
+                    f32.embed_backward(self, x, dh, d_x_emb=d_out if tied else None)
+            if tied:
+                f32.grad_buffer(w_out).add_(d_out)
+            return ce.view(N, D)
 
     def regenerate(self, x, start, end, n_candidates, x_cond=None, y_cond=None, encoder_kv=None, fp16=True, temp=1.0,
                    top_k=0, top_p=0.0, pack=False):

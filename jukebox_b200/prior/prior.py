@@ -14,7 +14,8 @@ the methods are written around two small helpers:
                  LayerNorm = the keys/values of the decoder's enc-dec attention layers (reference :285-301)
 
 z_forward / forward evaluate the loss (bits per token), predictions and recorded attention weights of a full window
-without gradients; optimisation itself is out of scope.
+without gradients; loss_grad evaluates z_forward's loss and adds its gradient into the decoder's .grad (fine-tuning with
+a torch optimiser; the optimiser step itself is torch's).
 """
 import numpy as np
 import torch as t
@@ -356,7 +357,8 @@ class SimplePrior(nn.Module):
         """Evaluation forward over one full window of codes (reference prior.py:312-349): returns (loss, metrics), or -
         with get_attn_weights (True or a set of layer indices) - the recorded attention weights of those layers, which
         is what lyric alignment reads (reference jukebox/align.py get_alignment).
-        No gradients are kept: optimisation is out of scope, the loss is the evaluation metric (bits per token)."""
+        No gradients are kept: the loss is the evaluation metric (bits per token); loss_grad is the same loss with the
+        decoder's gradients."""
         assert isinstance(get_attn_weights, (bool, set))
         tr = self.prior.transformer
         if get_attn_weights:
@@ -377,6 +379,44 @@ class SimplePrior(nn.Module):
         metrics = dict(bpd=gen_loss.clone(), prime_loss=prime_loss.clone(), gen_loss=gen_loss.clone())
         if get_preds:
             metrics["preds"] = preds.clone()
+        return loss, metrics
+
+    def loss_grad(self, z, z_conds=[], y=None):
+        """Fine-tuning: z_forward(fp16=False)'s (loss, metrics) of one full window of codes, and the gradient of that loss
+        ADDED into p.grad (fp32, created when None) of every parameter of self.prior (the ConditionalAutoregressive2D
+        decoder) that requires grad.  The conditioner, the label embedding, the lyric encoder and the VQ-VAE are frozen:
+        x_cond, y_cond and the encoder keys are constants, and a separate encoder's prime loss, which depends on them
+        alone, adds no gradient.  Each token's cross-entropy enters with its weight in the loss: 1 / (N total_loss_dims
+        ln 2) for a code, prime_loss_fraction times that for a lyric token of a single_enc_dec sequence.
+            prior.prior.requires_grad_(True)        # or only the layers to train
+            opt = torch.optim.Adam([p for p in prior.prior.parameters() if p.requires_grad], lr, betas=(0.9, beta2))
+            loss, metrics = prior.loss_grad(z, z_conds, y); opt.step(); opt.zero_grad()
+        Refused before any launch when nothing requires grad, for fp16_params or res_scale priors, attn_func 4 / 5,
+        a partial window or a module off the GPU."""
+        D = int(np.prod(z.shape[1:]))
+        why = self.prior.grad_refusal()
+        if why is None and D != self.gen_loss_dims:
+            why = f"gradients are taken over whole windows of {self.gen_loss_dims} codes, got {D}"
+        if why:
+            raise ValueError(why)
+        with t.no_grad():
+            seq, x_cond, y_cond, enc, lyric, head = self._condition(z, z_conds, y, fp16=False)
+            N = z.shape[0]
+            ln2 = float(np.log(2.))
+            unit = 1.0 / (N * self.total_loss_dims * ln2)
+            w = t.full(tuple(seq.view(N, -1).shape), unit, dtype=t.float32, device=z.device)
+            w[:, :head] = self.prime_loss_fraction * unit
+        ce = self.prior.loss_grad(seq, x_cond, y_cond, enc, row_weights=w)
+        with t.no_grad():
+            ce = ce.double()
+            gen_loss = (ce[:, head:].mean() / ln2).float()
+            if self.single_enc_dec:
+                prime_loss = (ce[:, :head].mean() / ln2).float()
+            else:
+                prime_loss = self.get_prime_loss(enc, lyric) if enc is not None else t.tensor(0.0, device=z.device)
+            total = self.total_loss_dims
+            loss = self.prime_loss_fraction * prime_loss * self.prime_loss_dims / total + gen_loss * self.gen_loss_dims / total
+            metrics = dict(bpd=gen_loss.clone(), prime_loss=prime_loss.clone(), gen_loss=gen_loss.clone())
         return loss, metrics
 
     def score(self, z, z_conds=[], y=None, fp16=True):

@@ -82,6 +82,7 @@ class Transformer(nn.Module):
         self.ws = []
         # decode engine state (not parameters)
         self._engine = None
+        self._engine_version = None
         self._engine_cfg = dict(bins=0, add_cond_after=True)
         self._enc_loaded = False
         self._f32 = None
@@ -111,6 +112,8 @@ class Transformer(nn.Module):
         if dev.type != "cuda":
             raise RuntimeError("Transformer.forward(sample=True) needs the module on a CUDA device: "
                                "jukebox_b200 has no CPU path (use the oracle in tests)")
+        if self._engine is not None and self._engine_version != self._weights_version():
+            self.drop_engine()          # weights changed in place (an optimiser step): the packed copy is stale
         if not self._engine_fits(n_samples, dev):
             if self.res_scale_unsupported():
                 raise NotImplementedError("res_scale=True priors are not supported by the decode engine yet")
@@ -118,10 +121,16 @@ class Transformer(nn.Module):
             for i, blk in enumerate(self._attn_mods):
                 eng.load_layer(i, blk)
             self._engine = eng
+            self._engine_version = self._weights_version()
             self._enc_loaded = False
             for l in self._attn_mods:
                 l.attn.del_cache()
         return self._engine
+
+    def _weights_version(self):
+        """the version counters of the stack's parameters: an in-place update (optimiser step) changes them, as
+        load_state_dict / .cuda() change what drop_engine reacts to"""
+        return tuple(p._version for p in self._attn_mods.parameters())
 
     def _engine_fits(self, n_samples, dev):
         return self._engine is not None and self._engine.max_batch >= n_samples and self._engine.device == dev
